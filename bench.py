@@ -9,9 +9,13 @@ the grid is (256 N) x 256 and each rank owns one contiguous 256x256 slab (weak s
 section 8e); ``--scaling strong`` splits one 2048x2048 grid over the ranks instead.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--scaling weak|strong]
+                    [--dump-outputs DIR]
 
 Prints ONE JSON line (rank 0).  ``--impl reference`` times the reference algorithm's CPU path
-(the numpy oracle, all host threads) on a bounded sample of the same workload.
+(the numpy oracle, all host threads) on a bounded sample of the same workload.  ``--dump-outputs DIR``
+writes what the last timed step returned to its caller (``DIR/safe_set.npy``: float32 0/1 over the
+global grid, ``DIR/c_max.npy``: float64 [1]); the inputs are seeded, so two builds given the same
+arguments can be compared output for output.
 """
 
 from __future__ import annotations
@@ -35,6 +39,12 @@ GRID = 256
 STRONG_GRID = 2048
 M_TRAIN = 500
 
+# Peaks the rooflines divide by.  FP64: DMMA.8x8x4 and exp() throughput measured with
+# tools/fp64_peaks.cu on one H100 SXM (132 SMs) at a 700 W power limit.  HBM: the H100 SXM data sheet.
+DMMA_PEAK_TFLOPS = 33.2
+EXP_PEAK_PER_S = 7.56e11
+HBM_PEAK_GBS = 3350.0
+
 
 def algorithmic_flops_per_point(M, d_in, n_factors, n_outputs):
     """SURVEY.md section 8d: sum over distinct factors of [M^2 + M (3 d_in + 6)] + D M E_exp
@@ -53,7 +63,7 @@ class ClockSampler(object):
 
     QUERY = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
              "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
-             "clocks_event_reasons.sw_power_cap")
+             "clocks_event_reasons.sw_power_cap,power.limit")
 
     def __init__(self, index):
         self.rows, self.proc, self.index = [], None, index
@@ -74,10 +84,12 @@ class ClockSampler(object):
 
     def stop(self):
         if self.proc is None:
-            return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
+            return {"sm_mhz": None, "sm_max_mhz": None, "power_limit_w": None,
+                    "reasons": ["nvidia-smi unavailable"]}
         time.sleep(0.25)
         self.proc.terminate()
-        sm, smax, reasons = [], None, set()
+        self.proc.wait()
+        sm, smax, plimit, reasons = [], None, None, set()
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         for r in self.rows:
             try:
@@ -88,9 +100,13 @@ class ClockSampler(object):
             for name, val in zip(names, r[3:7]):
                 if val.lower().startswith("active"):
                     reasons.add(name)
+            try:
+                plimit = float(r[7])
+            except (ValueError, IndexError):
+                pass
         busy = [v for v in sm if smax and v > 0.4 * smax] or sm
         return {"sm_mhz": float(np.median(busy)) if busy else None, "sm_max_mhz": smax,
-                "samples": len(sm), "reasons": sorted(reasons)}
+                "power_limit_w": plimit, "samples": len(sm), "reasons": sorted(reasons)}
 
 
 # --------------------------------------------------------------------------- CPU reference
@@ -220,7 +236,8 @@ def workload_config(world, scaling="weak"):
 def run_ours(args, rank, world, local_rank):
     import torch
     import __graft_entry__
-    if rank == 0 or not os.path.exists(os.path.join(ROOT, "safe_learning_b200", "libslb200.so")):
+    # the tree may be read-only: build only when the library is missing (build() writes in-tree)
+    if not os.path.exists(os.path.join(ROOT, "safe_learning_b200", "libslb200.so")):
         __graft_entry__.build()
     if not torch.cuda.is_available():
         raise SystemExit("bench.py: no CUDA device (safe_learning_b200 has no CPU fallback)")
@@ -288,18 +305,13 @@ def run_ours(args, rank, world, local_rank):
     ms_total = max_over_ranks(ms_total)
     value = n_total * args.steps / (ms_total * 1e-3)
     safe_points = int(lyap.last_sweep.get("n_safe", -1))     # first host read-back of the run
-
-    # The timed region lasts K x ~0.3 ms, shorter than one nvidia-smi sample.  The SAME step is
-    # therefore continued for ~1.5 s (a fixed count, identical on every rank) under the sampler;
-    # the clock record covers the timed region and this continuation, whose rate is reported too.
-    n_cont = int(min(20000, max(200, 1500.0 / max(ms_total / args.steps, 1e-3))))
-    if dist is not None:
-        t = torch.tensor([n_cont], dtype=torch.int64, device="cuda")
-        dist.broadcast(t, 0)
-        n_cont = int(t.item())
-    c_total, _ = timed(lyap.update_safe_set, n_cont)
-    c_total = max_over_ranks(c_total)
-    barrier()
+    # what the last timed step hands its caller (reading safe_set is collective: every rank reads)
+    outputs = {"safe_set": lyap.safe_set.astype(np.float32),
+               "c_max": np.array([lyap.feed_dict[lyap.c_max]], dtype=np.float64)}
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, array in outputs.items():
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), array)
 
     # ---- what the filter decided (statistics of ONE sweep, summed over ranks)
     cfg = lyap.sweep_descriptor()
@@ -401,38 +413,21 @@ def run_ours(args, rank, world, local_rank):
     # ---- roofline of the full-posterior kernel
     flops_pt = algorithmic_flops_per_point(M_TRAIN, 3, 2, 2)
     achieved_tf = flops_pt * n_local / (kernel_ms * 1e-3) * 1e-12
-    peak_tf, peak_src = 37.1, "fallback 37.1 (tools/fp64_peaks.cu on this pool, r01)"
-    try:
-        with open(os.path.join(ROOT, "profiles", "r01_fp64_peaks.json")) as fh:
-            peak_tf = float(json.load(fh)["dmma_tflops_w8_acc8"])
-            peak_src = "measured DMMA.8x8x4 peak, tools/fp64_peaks.cu (profiles/r01_fp64_peaks.json)"
-    except Exception:
-        pass
-    hbm_peak = 6650.0
-    try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as fh:
-            hbm_peak = float(json.load(fh)["hbm_gbs"])
-    except Exception:
-        pass
-    traffic = None
-    for name in ("r02b_gp_tile_kernel_ncu.json", "r02_gp_tile_kernel_ncu.json", "r01_gp_tile_kernel_ncu.json"):
-        try:
-            with open(os.path.join(ROOT, "profiles", name)) as fh:
-                traffic = json.load(fh).get("dram_bytes_per_launch")
-            break
-        except Exception:
-            pass
+    peak_tf = DMMA_PEAK_TFLOPS
+    peak_src = "DMMA.8x8x4 peak measured with tools/fp64_peaks.cu on an H100 SXM (700 W limit)"
+    hbm_peak = HBM_PEAK_GBS
     hbm_gbs = algorithmic_bytes_per_point(2) * n_local / (kernel_ms * 1e-3) * 1e-9
     roofline = {"bound": "tensor",
                 "kernel": "gp_tile_kernel<3> (fp64 DMMA.8x8x4): the full posterior for EVERY grid "
                           "point, timed with the decision filter switched off; the default step "
                           "runs it only on the points the filter cannot decide (see `filter`)",
                 "achieved": achieved_tf, "peak": peak_tf, "unit": "TFLOP/s",
-                "frac": achieved_tf / peak_tf, "traffic": traffic, "peak_source": peak_src,
+                "frac": achieved_tf / peak_tf, "peak_source": peak_src,
                 "kernel_ms": kernel_ms, "kernel_ms_spread": spread(k_per),
                 "algorithmic_flops_per_point": flops_pt,
                 "hbm": {"achieved": hbm_gbs, "peak": hbm_peak, "unit": "GB/s",
                         "frac": hbm_gbs / hbm_peak,
+                        "peak_source": "H100 SXM data sheet",
                         "note": "path is fp64-compute-bound (AI ~3e4 FLOP/B); HBM fraction "
                                 "reported for completeness"}}
     # Rooflines of the three stages of the DEFAULT step (stage times measured live with the library's
@@ -440,7 +435,7 @@ def run_ours(args, rank, world, local_rank):
     #  * stage 1, fp32 screening kernel (filter_mean32_kernel): per point and training row d_in FFMA for the
     #    exponent, one MUFU.EX2, one FFMA per output for the dot product -> bound by the SFU (16 ex2 per
     #    clock and SM) and the fp32 issue rate; algorithmic flops F_B = D M (3 d_in + 4 + E_exp), E_exp = 1
-    #    (SURVEY.md section 8d), against the fp32 FFMA peak 148 SMs x 128 lanes x 2 x 1.965 GHz.
+    #    (SURVEY.md section 8d), against the fp32 FFMA peak SMs x 128 lanes x 2 x the maximum SM clock.
     #  * stage 1, fp64 mean kernel (filter_mean_kernel, where screening does not apply): the same count on
     #    the fp64 pipe (DFMA shares the pipe and the peak of the DMMA tensor op: tools/fp64_peaks.cu).
     #  * head stage (filter_head_kernel): latency bound at C2 (one 8-point group per warp); reported as
@@ -453,33 +448,26 @@ def run_ours(args, rank, world, local_rank):
     stage_rooflines = None
     if mean_ms:
         stage1 = int(lib.slb_filter_stage1(cfg))
-
-        def ncu_traffic(name):
-            """dram__bytes_read.sum + dram__bytes_write.sum of one launch from the committed ncu summary"""
-            try:
-                with open(os.path.join(ROOT, "profiles", name)) as fh:
-                    return json.load(fh).get("dram_bytes_per_launch")
-            except Exception:
-                return None
         head_ms = stage_ms["mean_head"] - mean_ms
         refine_ms = filter_ms - stage_ms["mean_head"]
         flops_mean = 2 * M_TRAIN * (3 * 3 + 4 + 1)
         ach = flops_mean * n_local / (mean_ms * 1e-3) * 1e-12
         exp_rate1 = 2 * M_TRAIN * n_local / (mean_ms * 1e-3)
-        sm_ghz = 1.965
+        sms = torch.cuda.get_device_properties(local_rank).multi_processor_count
+        sm_ghz = clocks["sm_max_mhz"] * 1e-3 if clocks and clocks["sm_max_mhz"] else 1.98
         if stage1 == 32:
-            fp32_peak = 148 * 128 * 2 * sm_ghz * 1e-3
-            mufu_peak = 148 * 16 * sm_ghz * 1e9
+            fp32_peak = sms * 128 * 2 * sm_ghz * 1e-3
+            mufu_peak = sms * 16 * sm_ghz * 1e9
             r_mean = {
                 "bound": "compute", "bound_detail": "neither HBM nor tensor cores: SFU (MUFU.EX2, 16 per "
-                "clock and SM) and fp32 issue rate; `peak` is the fp32 FFMA peak 148 x 128 x 2 x 1.965 GHz",
+                "clock and SM) and fp32 issue rate; `peak` is the fp32 FFMA peak %d SMs x 128 x 2 x %.3f GHz"
+                % (sms, sm_ghz),
                 "kernel": "filter_mean32_kernel<3>: fp32 screening mean of every grid point (3 FFMA + "
                           "MUFU.EX2 + 1 FFMA per kernel value) with a certified error bound, decision "
                           "over the mean's error box and the prior variance",
                 "achieved": ach, "peak": fp32_peak, "unit": "TFLOP/s", "frac": ach / fp32_peak,
                 "kernel_ms": mean_ms, "algorithmic_flops_per_point": flops_mean,
-                "exp_per_s": exp_rate1, "exp_peak_per_s": mufu_peak, "exp_frac": exp_rate1 / mufu_peak,
-                "traffic": ncu_traffic("r02b_filter_mean_kernel_ncu.json")}
+                "exp_per_s": exp_rate1, "exp_peak_per_s": mufu_peak, "exp_frac": exp_rate1 / mufu_peak}
         else:
             r_mean = {
                 "bound": "tensor", "kernel": "filter_mean_kernel<3> (fp64 pipe: DFMA, the pipe and peak "
@@ -487,16 +475,15 @@ def run_ours(args, rank, world, local_rank):
                 "achieved": ach, "peak": peak_tf, "unit": "TFLOP/s", "frac": ach / peak_tf,
                 "kernel_ms": mean_ms, "algorithmic_flops_per_point": flops_mean,
                 "executed_fp64_ops_per_entry": 12,
-                "exp_per_s": exp_rate1, "exp_peak_per_s": 8.4e11, "exp_frac": exp_rate1 / 8.4e11,
-                "traffic": None}
+                "exp_per_s": exp_rate1, "exp_peak_per_s": EXP_PEAK_PER_S,
+                "exp_frac": exp_rate1 / EXP_PEAK_PER_S}
         ach_ref = flops_pt * fs["refined"] / max(refine_ms * 1e-3, 1e-9) * 1e-12
         r_refine = {
             "bound": "tensor", "kernel": "gp_tile_kernel<3, 32> on the refine list (fp64 DMMA.8x8x4; rows "
                                          "and factors of every 32-point tile split over spare CTAs)",
             "achieved": ach_ref, "peak": peak_tf, "unit": "TFLOP/s", "frac": ach_ref / peak_tf,
             "kernel_ms": refine_ms, "points": fs["refined"], "algorithmic_flops_per_point": flops_pt,
-            "traffic": ncu_traffic("r02b_refine_tile_kernel_ncu.json"),
-            "note": "a few hundred points cannot fill 148 SMs: the pass is bound by the latency of one "
+            "note": "a few hundred points cannot fill the SMs: the pass is bound by the latency of one "
                     "tile's serial chain (generation -> contraction -> reduction), not by the pipe"}
         r_head = {"kernel": "filter_head_kernel<3>", "kernel_ms": head_ms,
                   "points": fs["head"] + fs["refined"],
@@ -518,7 +505,7 @@ def run_ours(args, rank, world, local_rank):
         "refined_by_full_posterior": fs["refined"] / npts, "points": fs["points"],
         "head_rank": nat.SLB_HEAD_RANK,
         "decision_kernels_ms": filter_ms,
-        "exp_per_s": exp_rate, "exp_peak_per_s": 8.4e11, "exp_frac": exp_rate / 8.4e11,
+        "exp_per_s": exp_rate, "exp_peak_per_s": EXP_PEAK_PER_S, "exp_frac": exp_rate / EXP_PEAK_PER_S,
         "note": "flags identical to the full posterior (tests/test_gpu_bench_shapes.py, `parity`); "
                 "the fractions depend on the workload: a point is decided early only when "
                 "`decrease < threshold` has the same outcome for every sigma between 0 and a "
@@ -538,7 +525,8 @@ def run_ours(args, rank, world, local_rank):
         "warmup": n_warm, "ms_per_step": ms_total / args.steps,
         "ms_per_step_spread": spread(per_step),
         "higher_is_better": True, "scaling": args.scaling, "vs_baseline": None, "dtype": "f64",
-        "data": "synthetic", "config": workload_config(world, args.scaling), "clocks": clocks,
+        "data": "synthetic", "config": workload_config(world, args.scaling),
+        "gpu": torch.cuda.get_device_name(local_rank), "clocks": clocks,
         "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": int(h2d),
                 "d2h_bytes_per_step": int(d2h), "ms_per_step": e_total / args.steps,
                 "ms_per_step_spread": spread(e_per),
@@ -559,10 +547,6 @@ def run_ours(args, rank, world, local_rank):
                            "ms_per_step_spread": spread(f_per),
                            "note": "same step with the filter off: every point through the O(M^2) "
                                    "posterior (the round-1 path)"},
-        "sustained": {"steps": n_cont, "ms_per_step": c_total / n_cont,
-                      "value": n_total * n_cont / (c_total * 1e-3),
-                      "note": "the timed step continued for ~1.5 s so that nvidia-smi samples "
-                              "exist under load; `clocks` covers the timed region and this"},
         "cpu_baseline": cpu_baseline,
         "safe_points": safe_points, "parity": parity, "exchange": exchange,
     }
@@ -581,6 +565,8 @@ def main():
                     help="weak: 256x256 per GPU (default); strong: one 2048x2048 grid split over N")
     ap.add_argument("--parity", action="store_true",
                     help="run the oracle parity check even on grids above 2^20 points")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))

@@ -5,7 +5,7 @@ Raw parameters are plain numpy (``make_*``); ``build_product`` instantiates the 
 so parity tests compare like with like.  This module is not part of the product package.
 
 Workloads follow the reference's pendulum experiment
-(/root/reference/examples/adaptive_safety_verification.ipynb cells 7-17) with the RBF kernel
+(upstream examples/adaptive_safety_verification.ipynb cells 7-17) with the RBF kernel
 BASELINE.json names: true pendulum (m=0.15, l=0.5, b=0.1), "wrong" prior model (m=0.1, l=0.4,
 b=0) as linear GP prior mean, LQR policy saturated to [-1, 1], V = x^T P x, per-dimension
 Lipschitz |2 P x|, tau = sum(unit_maxes)/2, initial safe set |x|_2 <= 0.2, beta = 2,

@@ -1,11 +1,11 @@
 /*
- * slb200.h -- C ABI of libslb200.so: the B200 (sm_100a) implementation of the
+ * slb200.h -- C ABI of libslb200.so: the H100 (sm_90a) implementation of the
  * safe_learning region-of-attraction hot path.
  *
  * The reference (befelix/safe_learning @ f1aad5a) has no FFI: the path sits behind
  * Python classes that build a TF1 graph and call Session.run once per 10 000-point
  * batch.  The entry points below are what a binding for that path would bind; each
- * cites the reference code it replaces (paths relative to /root/reference).  The
+ * cites the reference code it replaces (paths relative to the upstream sources).  The
  * Python host side (safe_learning_b200/) loads this library with ctypes -- see
  * INTEGRATION.md for the stub a maintainer of the reference would add.
  *
@@ -317,7 +317,7 @@ int         slb_debug_screening_probe(double* mu_dev, double* dm_dev);
 int         slb_debug_det_fast(int32_t enable);
 /* diagnostics / tuning: the refine pass of slb_lyapunov_sweep_filtered uses 16-point tiles for
  * lists of up to `upto16` points, 32-point tiles up to `upto32`, 64-point tiles beyond (defaults
- * 0 -- no 16-point launch -- and 32 * 148); with 16- and 32-point tiles the rows of a tile are additionally split
+ * 0 -- no 16-point launch -- and 32 points per SM, 32 * 132); with 16- and 32-point tiles the rows of a tile are additionally split
  * over the CTAs a one-per-SM grid has to spare (up to 8 per tile) */
 int         slb_debug_refine_split(int64_t upto16, int64_t upto32);
 

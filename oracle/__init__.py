@@ -22,7 +22,7 @@ Pinning status (see DESIGN.md "Oracle"):
   ``PolicyIteration.future_values`` / ``value_iteration`` /
   ``discrete_policy_optimization``;
 * third-party arithmetic restated from its published algorithm (not under
-  /root/reference): ``gpflow==0.4.0`` ``kernels`` ``K/Kdiag`` (``requirements.txt:3``).  RBF is
+  the upstream sources): ``gpflow==0.4.0`` ``kernels`` ``K/Kdiag`` (``requirements.txt:3``).  RBF is
   anchored by the golden vector above; Matern12/32/52, Linear, Constant, White, Add and Prod
   are PARITY UNPINNED as arithmetic (no vector of theirs exists upstream) -- the reference's
   own GP code around them runs on the fixture shim's restatement of the same formulae;

@@ -1,6 +1,6 @@
 """numpy/scipy fp64 restatement of the reference hot path (TEST INFRASTRUCTURE ONLY).
 
-Reference: befelix/safe_learning @ f1aad5a, paths relative to /root/reference.
+Reference: befelix/safe_learning @ f1aad5a, paths relative to its source tree.
 All objects here are plain numpy callables: ``fun(points) -> ndarray`` where the
 reference builds a TF1 graph node.  Operation order of the cheap element-wise
 pieces (grid coordinates, linear maps, quadratic forms, barycentric weights, the
@@ -293,7 +293,7 @@ def _row_norm1(values):
 # --------------------------------------------------------------------------- GP (gpflow 0.4.0 restated)
 class Kernel(object):
     """``gpflow==0.4.0`` ``kernels.Kern`` algebra (third party, pinned ``requirements.txt:3``; not under
-    /root/reference, restated from its published arithmetic): every primitive works on the columns
+    the upstream sources, restated from its published arithmetic): every primitive works on the columns
     ``active_dims`` (default: the first ``input_dim``), ``k1 + k2`` / ``k1 * k2`` add / multiply the
     covariance matrices (``Add`` / ``Prod``).  Used by the reference's experiments
     (``examples/inverted_pendulum.ipynb`` cell 6, ``1d_region_of_attraction_estimate.ipynb`` cell 5)."""

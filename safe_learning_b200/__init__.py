@@ -1,8 +1,8 @@
-"""safe_learning_b200 -- the region-of-attraction hot path of befelix/safe_learning on B200.
+"""safe_learning_b200 -- the region-of-attraction hot path of befelix/safe_learning on H100.
 
 Drop-in for ``Lyapunov.update_safe_set`` / ``v_decrease_confidence`` / ``v_decrease_bound`` on a
 ``GridWorld`` with ``GaussianProcess`` / ``FunctionStack`` dynamics and the ``PolicyIteration``
-Bellman sweep; the arithmetic runs in hand-written sm_100a CUDA (``libslb200.so``, C ABI in
+Bellman sweep; the arithmetic runs in hand-written sm_90a CUDA (``libslb200.so``, C ABI in
 ``include/slb200.h``).  No CPU fallback.
 """
 

@@ -1,4 +1,4 @@
-"""Build libslb200.so in-tree with nvcc for sm_100a (no JIT cache, the .so travels with the repo).
+"""Build libslb200.so in-tree with nvcc for sm_90a (H100) (no JIT cache, the .so travels with the repo).
 
 Every translation unit is compiled to an object file concurrently (the GP tile kernel is one unit
 per input dimension and tile size, ``gp_tile_inst.cu`` with ``-DSLB_TILE_DIN=k -DSLB_TP=t``), then linked; only units whose
@@ -31,7 +31,7 @@ UNITS += [("gp_sweep.o", "gp_sweep.cu", [], ["gp_args.h"]),
           ("bellman_tile.o", "bellman_tile.cu", [], [])]
 SOURCES = sorted({u[1] for u in UNITS})
 
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 CFLAGS = ARCH + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC"]
 
 

@@ -175,7 +175,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise NativeLibraryError(
             "%s not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a). safe_learning_b200 has no CPU fallback." % LIB_PATH)
+            "(nvcc, sm_90a). safe_learning_b200 has no CPU fallback." % LIB_PATH)
     lib = C.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():
         fn = getattr(lib, name)          # AttributeError if the symbol is not exported

@@ -45,10 +45,10 @@ namespace {
 #define SLB_MEAN_MINB 7
 #endif
 constexpr int FT = SLB_FT;             // stage 1: threads per CTA = points per CTA (1024 CTAs at
-                                       // 256 x 256, 7 resident per SM: single wave, 98.8% balanced)
+                                       // 256 x 256, 7 resident per SM)
 constexpr int HR = SLB_HEAD_RANK;
 constexpr int HT = 512;                // stage 2: threads per CTA (16 warps, 8 or 2 list entries each)
-constexpr int HEAD_CTAS = 148;         // one CTA per SM (it stages the head factors in shared memory)
+constexpr int HEAD_CTAS = SLB_NUM_SMS;  // one CTA per SM (it stages the head factors in shared memory)
 constexpr int64_t CHUNK = 1 << 22;     // points per pass of the three stages (bounds the workspace)
 constexpr int64_t WS_HEAD = 64 + SLB_SPLIT_TICKET_BYTES + (int64_t)SLB_SPLIT_PARTIAL_BYTES;   // bytes before the lists
 
@@ -369,11 +369,9 @@ filter_mean32_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a)
 // ---- stage 2: variance given the head subset, one warp per HP undecided points ---------------------
 // One CTA per SM, 8 warps.  The head factors W = L_S^-1 (column-major, zero padded, 32 KB each) and
 // the subset's inputs are staged ONCE per CTA in shared memory by TMA bulk copies (read from
-// global memory per point they cost an L2/HBM round trip per column: measured 47 us for 5000
-// points); then every warp walks the list in groups of HP = 8 points.  Lane l owns rows l and l + 32
+// global memory per point they cost an L2/HBM round trip per column); then every warp walks the list in groups of HP = 8 points.  Lane l owns rows l and l + 32
 // of a = W k for all HP points (16 independent FMA chains): a column of W read from shared memory
-// serves 8 points -- one point per warp made the stage shared-memory-bandwidth bound (6.4 ms for
-// the 1.9 M list entries of a 2048 x 2048 grid).  The kernel values k_j of the HR subset points are
+// serves 8 points -- one point per warp makes the stage shared-memory-bandwidth bound.  The kernel values k_j of the HR subset points are
 // computed two per lane and point and exchanged through shared memory ([row][point]: one row's
 // HP values are four broadcast 128-bit loads); lane p < HP makes the decision of point p.
 constexpr int HW = HT / 32;            // warps per CTA

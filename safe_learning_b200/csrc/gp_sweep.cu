@@ -92,17 +92,16 @@ static long long* g_timing_buffer = nullptr;
 
 // The full posterior for the points the decision filter (filter.cu) could not decide: `list`
 // holds their indices relative to idx_begin, `count` (device) how many there are.  The list is
-// usually a small fraction of the grid -- too short to fill the 148 SMs with 64-point tiles, and a
+// usually a small fraction of the grid -- too short to fill the SMs with 64-point tiles, and a
 // tile's duration does not shrink with the list -- so the pass is launched once per tile size
 // (16, 32, 64 points per CTA) and only the launch whose range holds the list length does work;
-// the CTAs of the others (and those beyond the list) leave at once.  Measured tile times at
-// M = 500, two factors: see DESIGN.md section 3.5.
-static int64_t g_refine_split[2] = {0, 32 * 148};   // 16-point tiles: diagnostics only (an empty launch costs ~3 us)
+// the CTAs of the others (and those beyond the list) leave at once.
+static int64_t g_refine_split[2] = {0, 32 * SLB_NUM_SMS};   // 16-point tiles: diagnostics only (an empty launch still costs)
 
-// Short lists (<= 32 x 148 points) additionally split every tile's ROWS over the CTAs the grid has
+// Short lists (<= 32 points per SM) additionally split every tile's ROWS over the CTAs the grid has
 // to spare (up to SLB_SPLIT_MAX groups of equal triangular area, gp_tile.cuh): the tile kernel's
-// duration is set by the M^2 / 2 contraction of one tile, so 525 points in 33 16-point tiles kept
-// 33 SMs busy for 88 us while 115 idled; split 8 ways a 32-point tile's share is ~8 times shorter.
+// duration is set by the M^2 / 2 contraction of one tile, so a few hundred points in whole tiles keep
+// a few dozen SMs busy while the rest idle; split 8 ways a 32-point tile's share is ~8 times shorter.
 int slb_launch_refine(cudaStream_t st, const slb_sweep& cfg, int64_t n_max, int64_t idx_begin,
                       const int64_t* list, const unsigned long long* count, uint8_t* negative,
                       double* values, double* split_partial, int* split_ticket) {
@@ -122,7 +121,7 @@ int slb_launch_refine(cudaStream_t st, const slb_sweep& cfg, int64_t n_max, int6
         a.split_partial = nullptr; a.split_ticket = nullptr; a.split_max = 1;
         if (v < 2 && split_partial != nullptr) {
             // at least one CTA per SM, so that short lists have CTAs to spread their rows over
-            if (a.n < (int64_t)148 * tps[v]) a.n = (int64_t)148 * tps[v];
+            if (a.n < (int64_t)SLB_NUM_SMS * tps[v]) a.n = (int64_t)SLB_NUM_SMS * tps[v];
             if ((a.n + tps[v] - 1) / tps[v] <= SLB_SPLIT_ITEMS) {
                 a.split_partial = split_partial; a.split_ticket = split_ticket;
                 static const int split_max = [] {          // SLB200_SPLIT_MAX: A/B timing knob

@@ -1,7 +1,7 @@
 // gp_tile.cuh -- the dominant kernel: GP posterior (mean + variance) of a 64-point tile and,
 // in sweep mode, the fused Lyapunov decision.
 //
-// Replaces, per 10 000-point Session.run of the reference (paths relative to /root/reference):
+// Replaces, per 10 000-point Session.run of the reference (paths relative to upstream safe_learning):
 //   gpflow kern.K(X, Xnew)                       functions.py:438   -> k-row generation phase
 //   tf.matrix_triangular_solve(L, Kx)            functions.py:441   -> a = L^-1 k as DMMA GEMM
 //   a^T alpha (+ prior mean), Kdiag - sum a^2    functions.py:442,450-451 -> panel epilogue
@@ -9,10 +9,9 @@
 //   FunctionStack concat                         functions.py:278-291
 //   v_decrease_bound < threshold                 lyapunov.py:436-441 -> tile epilogue
 //
-// Design (B200, fp64 pipe bound -- see DESIGN.md section 3.1):
+// Design (H100, fp64 pipe bound -- see DESIGN.md section 3.1):
 //   * one CTA = 64 grid points x all M training points, 8 warps, 1 CTA/SM (~178 KB shared
-//     memory, 232 registers, no spills).  Measured alternatives (profiles/r01_kernel_variants.md):
-//     16 warps x (16 rows x 64 points) is +1% with spills, 2 CTAs/SM x 32-point tiles is slower.
+//     memory); SLB_NW=16 builds the 16-warp variant.
 //   * W = L^-1 (lower triangular) is pre-packed in DMMA.8x8x4 A-fragment order, two k-steps
 //     per 128-bit element (slb_pack_factor); each warp streams ITS rows of W straight from L2
 //     into registers with coalesced 512 B loads through a static three-deep register ring --
@@ -64,7 +63,7 @@ static_assert(NW == 8 || NW == 16, "NW must be 8 or 16");
 constexpr int NB = TP / 8;            // 8-point column blocks per warp tile
 constexpr int CTAS_PER_SM = 1;
 constexpr int NRED = 1 + SLB_MAX_OUT;
-constexpr int PREFETCH_CTAS = 148 * CTAS_PER_SM;    // one wave on a B200
+constexpr int PREFETCH_CTAS = SLB_NUM_SMS * CTAS_PER_SM;    // one wave
 
 constexpr size_t SMEM_KS = (size_t)(PANEL / 8) * 4 * KSTR * 2 * sizeof(double);
 constexpr size_t SMEM_Z = (size_t)SLB_MAX_IN * TP * sizeof(double);
@@ -94,8 +93,7 @@ SLB_DEV void dmma884(double& c0, double& c1, double a, double b) {
 // Per pair and row block ONE 128-bit global load brings the A fragments of both k-steps
 // (the packed factor stores them adjacent), per column block ONE 128-bit shared load brings both
 // B fragments.  The A prefetch ring (RING pairs ahead) is unrolled with static registers: no
-// rotation moves.  Measured in isolation (tools/dmma_mix.cu, "wide"): 94% of the DMMA peak with
-// 4 active row blocks and ~90% with 1-3, against 90% / <=85% for one 64-bit load per fragment.
+// rotation moves (tools/dmma_mix.cu, "wide", measures this load pattern in isolation).
 template <int Q0>
 SLB_DEV void mma_run(double (&acc)[RQ][NB][2], const double2* const (&ap)[RQ], int m0, int m1,
                      const double2* ks_lane) {
@@ -227,8 +225,8 @@ SLB_DEV void gp_tile_body(const slb_sweep& cfg, const slb_gp_args& a, unsigned c
 
     // ---- stage 0: warm L2.  Every CTA streams the whole packed L^-1 (1 MB per factor at
     // M=500); if it is not L2-resident when the launch starts (first sweep after add_data_point,
-    // or after anything else evicted it) the first wave of 148 CTAs would pull it from HBM at
-    // streaming latency, in lockstep, and run ~2x slower (measured: +15% on the whole sweep).
+    // or after anything else evicted it) the first wave of CTAs would pull it from HBM at
+    // streaming latency, in lockstep.
     // The first-wave CTAs therefore prefetch disjoint 128-byte lines of it into L2 while the
     // k-row generation phase runs; the demand loads then hit.
     if (first_tile && blockIdx.x < PREFETCH_CTAS) {
@@ -391,7 +389,7 @@ SLB_DEV void gp_tile_body(const slb_sweep& cfg, const slb_gp_args& a, unsigned c
                     // stage the panel's training inputs in shared memory with one coalesced pass:
                     // every row is needed once by every warp, and read straight from global the
                     // first toucher of each row pays an L2 round trip inside the exp dependency
-                    // chain (measured: the generation loop ran at ~45% of its fp64 bound)
+                    // chain
                     for (int i = tid; i < nj * DIN; i += NT) Xp[i] = Xs[(size_t)j0 * DIN + i];
                     __syncthreads();
                     // thread (p_gen, jg): fragment row r = jg % 4 of the pairs m = jg / 4 (mod PS),
@@ -680,8 +678,8 @@ gp_tile_kernel(const __grid_constant__ slb_sweep cfg, const slb_gp_args a) {
             if (FS > 1) fsel = rem / G;
         } else {
             // unsplit refine launches are persistent: the grid is one CTA per SM (the list length is
-            // not known to the host; a grid sized for the longest possible list cost 6 us of empty
-            // CTAs when it was not this launch's turn), every CTA walks the tiles in strides
+            // not known to the host; a grid sized for the longest possible list costs empty CTAs
+            // when it is not this launch's turn), every CTA walks the tiles in strides
             tile_end = ntiles;
             tile_step = gridDim.x;
         }

@@ -194,7 +194,7 @@ det_sweep_kernel(const __grid_constant__ slb_sweep cfg, const double* __restrict
 // LinearSystem), dynamics = LinearSystem on [x, u], V = QuadraticFunction, L_V = a constant or
 // abs(LinearSystem) (one- or two-column), scalar L_f.  det_sweep_kernel interprets generic
 // descriptors through local-memory operand arrays (1.6 KB stack, 64-bit index division, one byte
-// written per thread: 7% of the HBM roofline); here the operands live in registers, the index
+// written per thread); here the operands live in registers, the index
 // arithmetic is one 32-bit division per 8 points and the 8 flags leave as one 8-byte store.  The
 // arithmetic is eval_fn's, operation for operation (__dmul_rn / __dadd_rn, same order): bit-exact.
 struct det_fast_params {

@@ -1,7 +1,7 @@
 """Function objects of the region-of-attraction path, as parameter containers for libslb200.
 
 API surface follows ``safe_learning/functions.py`` of the reference (class names, constructor
-arguments, attributes); cited line numbers are relative to /root/reference.  Where the
+arguments, attributes); cited line numbers are relative to the upstream safe_learning sources.  Where the
 reference's objects emit TF1 graph nodes, these objects (a) describe themselves to the CUDA
 kernels through an ``slb_function`` / ``slb_gp_stack`` descriptor and (b) evaluate eagerly on
 the GPU when called with numpy arrays, returning numpy arrays.  There is no CPU path.

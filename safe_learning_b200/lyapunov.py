@@ -128,9 +128,9 @@ def get_safe_sample(lyapunov, perturbations=None, limits=None, positive=False, n
 
 
 # CUDA-graph replay of the launches of a sweep (memsets + 8 kernels) while nothing they depend on
-# changes: the second sweep with an unchanged descriptor is captured, later ones replay it.  Measured
-# at C2 (profiles/r02_*): -9 us on the device step (0.219 -> 0.210 ms) and -32 us of host enqueue
-# time per sweep, which is what bounds the end-to-end step.  SLB200_GRAPHS=0 switches it off.
+# changes: the second sweep with an unchanged descriptor is captured, later ones replay it.  It saves
+# device time between the launches and the host enqueue time per sweep, which is what bounds the
+# end-to-end step.  SLB200_GRAPHS=0 switches it off.
 _USE_GRAPHS = os.environ.get("SLB200_GRAPHS", "1") == "1"
 
 

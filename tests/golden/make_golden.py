@@ -1,7 +1,8 @@
-"""Generate golden fixtures by executing the UNMODIFIED reference (/root/reference) on the
-numpy-backed TF1 / gpflow API shims in ``tf1_shim/`` (build container only).
+"""Generate golden fixtures by executing the UNMODIFIED reference (a befelix/safe_learning @ f1aad5a
+checkout named by $SAFE_LEARNING_REFERENCE) on the numpy-backed TF1 / gpflow API shims in
+``tf1_shim/``.
 
-    python tests/golden/make_golden.py [grid|gp|gp_kernels|lyapunov|policy|tri_gradient ...]   # rewrites tests/golden/*.npz
+    SAFE_LEARNING_REFERENCE=<checkout> python tests/golden/make_golden.py [grid|gp|gp_kernels|lyapunov|policy|tri_gradient ...]   # rewrites tests/golden/*.npz
 
 Each fixture stores the raw inputs and the reference's outputs; tests/test_golden_fixtures.py
 rebuilds the numpy oracle (CPU tests) and the CUDA product (GPU tests) from the same inputs
@@ -10,7 +11,7 @@ Triangulation, LinearSystem, QuadraticFunction, Saturation, GPRCached (cache + p
 GaussianProcess, FunctionStack, Lyapunov (threshold, v_decrease_*, update_values,
 update_safe_set incl. the batch loop and c_max), PolicyIteration (future_values,
 value_iteration, discrete_policy_optimization), utilities (batchify, dlqr, concatenate_inputs).
-What is restated in the shim (third-party, not under /root/reference): tf ops -> numpy,
+What is restated in the shim (third-party, not part of the reference): tf ops -> numpy,
 gpflow 0.4.0 RBF kernel arithmetic.
 """
 import json

@@ -1,7 +1,7 @@
-"""Import the UNMODIFIED reference package from /root/reference on top of the API shims.
+"""Import the UNMODIFIED reference package (a befelix/safe_learning @ f1aad5a checkout whose
+directory $SAFE_LEARNING_REFERENCE names) on top of the API shims.
 
-Only usable in the build container (the GPU box has no /root/reference); used by
-make_golden.py to produce the committed fixtures.
+Used by make_golden.py to produce the committed fixtures; no test needs the checkout.
 """
 import collections
 import collections.abc
@@ -11,7 +11,7 @@ import sys
 import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-REFERENCE = "/root/reference"
+REFERENCE = os.environ.get("SAFE_LEARNING_REFERENCE", "")
 
 
 def _listify(fn):
@@ -25,7 +25,7 @@ def _listify(fn):
 def load_reference():
     """Returns the imported ``safe_learning`` reference module."""
     if not os.path.isdir(REFERENCE):
-        raise RuntimeError("the reference checkout is not available on this machine")
+        raise RuntimeError("set SAFE_LEARNING_REFERENCE to a befelix/safe_learning checkout")
     # Python >= 3.10 / numpy >= 1.24 compatibility aliases the 2018 sources rely on
     for name in ("Sequence", "Mapping", "Iterable"):
         if not hasattr(collections, name):
@@ -48,5 +48,5 @@ def load_reference():
         if path not in sys.path:
             sys.path.insert(0, path)
     import safe_learning
-    assert safe_learning.__file__.startswith(REFERENCE)
+    assert safe_learning.__file__.startswith(os.path.abspath(REFERENCE))
     return safe_learning

@@ -1,8 +1,8 @@
-"""Stand-in for the slice of gpflow==0.4.0 that /root/reference/safe_learning touches
+"""Stand-in for the slice of gpflow==0.4.0 that the reference's safe_learning package touches
 (fixture generation only; see ../tensorflow/__init__.py).
 
 ``kernels.*`` (RBF, Matern, Linear, Constant, White, Add, Prod) and ``gpr.GPR.build_predict`` restate gpflow 0.4.0's published arithmetic
-(third-party code that is not under /root/reference); everything the reference itself
+(third-party code that is not part of the reference); everything the reference itself
 implements -- ``GPRCached`` caching and prediction, ``GaussianProcess`` beta scaling,
 ``FunctionStack`` -- runs from the reference's own source on top of this.
 """

@@ -1,5 +1,5 @@
 """numpy-backed stand-in for the slice of the TensorFlow 1.x API that
-/root/reference/safe_learning uses on the region-of-attraction path.
+the reference's safe_learning package uses on the region-of-attraction path.
 
 PURPOSE: fixture generation only (tests/golden/make_golden.py).  TF 1.x cannot be installed
 in the build container (Python 3.12, no network); this shim lets the UNMODIFIED reference

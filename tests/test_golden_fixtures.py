@@ -1,5 +1,6 @@
 """Golden fixtures produced by the UNMODIFIED reference (tests/golden/make_golden.py runs
-/root/reference/safe_learning on numpy-backed TF1/gpflow API shims in the build container).
+the reference's safe_learning package on numpy-backed TF1/gpflow API shims; the fixtures are
+committed, so no test needs the reference).
 
 CPU tests pin the numpy oracle to the reference's own outputs; GPU tests (marked ``gpu``) hold
 the CUDA path to the same fixtures: safe sets / c_max / refinement bit-exact, element-wise

@@ -54,7 +54,7 @@ def _sweep_details(lyap):
 
 # ------------------------------------------------------------------ reference known answers
 def test_reference_update_known_answers(sl):
-    """/root/reference/safe_learning/tests/test_lyapunov.py:48-74 through the product API."""
+    """Upstream safe_learning/tests/test_lyapunov.py:48-74 through the product API."""
     def make(eps):
         grid = sl.GridWorld([[-1, 1]], 3)
         return sl.Lyapunov(grid, sl.QuadraticFunction(np.array([[1.0]])),
@@ -418,7 +418,7 @@ def test_refine_pass_tile_sizes(sl, split, label):
             gpu.filter = False
             assert_array_equal(fast, gpu.compute_negative().cpu().numpy(), err_msg=label)
     finally:
-        lib.slb_debug_refine_split(16 * 148, 32 * 148)
+        lib.slb_debug_refine_split(0, 32 * 132)        # the library's default split
 
 
 def test_pivoted_head_subset_matches_greedy_selection(sl):

@@ -1,7 +1,7 @@
 """The oracle against the reference's OWN known-answer tests (SURVEY.md section 8c).
 
 Each test names the reference test it transcribes (paths relative to
-/root/reference/safe_learning/tests).  These pin the numpy restatement before it
+the upstream safe_learning/tests).  These pin the numpy restatement before it
 is trusted as the checker for the CUDA path.
 """
 import numpy as np
@@ -215,7 +215,7 @@ def test_adaptive_closed_form_matches_batch_loop():
 
 
 def test_triangulation_known_answers():
-    """/root/reference/safe_learning/tests/test_functions.py:457-655 (find_simplex, values,
+    """Upstream safe_learning/tests/test_functions.py:457-655 (find_simplex, values,
     projection, three dimensions, gradient, 1-D) restated against the oracle's Triangulation."""
     # find_simplex :457-499
     limits, num = [[-1, 1], [-1, 2]], [3, 7]

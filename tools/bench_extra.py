@@ -26,13 +26,7 @@ import torch  # noqa: E402
 import bench_workloads as W  # noqa: E402
 import safe_learning_b200 as sl  # noqa: E402
 from bench import algorithmic_flops_per_point  # noqa: E402
-
-PEAK_TF, HBM_GBS = 37.1, 6483.3
-try:
-    PEAK_TF = json.load(open(os.path.join(ROOT, "profiles", "r01_fp64_peaks.json")))["dmma_tflops_w8_acc8"]
-    HBM_GBS = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"]
-except Exception:
-    pass
+from bench import DMMA_PEAK_TFLOPS as PEAK_TF, HBM_PEAK_GBS as HBM_GBS  # noqa: E402
 
 
 def timed(fn, steps=10, warmup=3):

@@ -4,12 +4,12 @@
 set -e
 cd "$(dirname "$0")/../safe_learning_b200/csrc"
 mkdir -p ../variants
-FLAGS="-gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC"
+FLAGS="-gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC"
 build() {  # name, extra flags...
   name=$1; shift
   nvcc $FLAGS "$@" -c filter.cu -o ../variants/filter_$name.o
   objs=$(ls build/*.o | grep -v "build/filter.o")
-  nvcc -shared -gencode arch=compute_100a,code=sm_100a -o ../variants/libslb200_$name.so $objs ../variants/filter_$name.o
+  nvcc -shared -gencode arch=compute_90a,code=sm_90a -o ../variants/libslb200_$name.so $objs ../variants/filter_$name.o
   echo built $name
 }
 build u4 &

@@ -1,6 +1,6 @@
-// Microbenchmark: fp64 peaks of a B200 (sm_100a) -- DFMA, DMMA.8x8x4, exp().
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o fp64_peaks fp64_peaks.cu
-// Output: one JSON object on stdout (bench.py / DESIGN.md cite the committed copy in profiles/).
+// Microbenchmark: fp64 peaks of an H100 (sm_90a) -- DFMA, DMMA.8x8x4, exp().
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o fp64_peaks fp64_peaks.cu
+// Output: one JSON object on stdout (the source of the fp64 peaks bench.py divides by).
 #include <cstdio>
 #include <cstdlib>
 #include <cuda_runtime.h>

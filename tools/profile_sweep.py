@@ -29,6 +29,7 @@ if "--phases" in sys.argv:
     from safe_learning_b200 import _native as nat
     lib = nat.load()
     ntiles = (lyap._end - lyap._begin + 63) // 64
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
     buf = torch.zeros((ntiles, 8, 8), dtype=torch.int64, device="cuda")
     flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
     for label, pre in (("back-to-back", lambda: lyap.compute_negative()),
@@ -45,8 +46,8 @@ if "--phases" in sys.argv:
         order = np.argsort(t[:, 0, 4])
         mhz = 1e3 * cyc / ns
         print(label, "| kernel span ms %.3f" % ((t[:, :, 5].max() - t[:, :, 4].min()) * 1e-6),
-              "| SM MHz by tile start order: first 148 %.0f, middle %.0f, last 148 %.0f"
-              % (mhz[order[:148]].mean(), mhz[order[400:600]].mean(), mhz[order[-148:]].mean()),
+              "| SM MHz by tile start order: first wave %.0f, middle %.0f, last wave %.0f"
+              % (mhz[order[:sms]].mean(), mhz[order[400:600]].mean(), mhz[order[-sms:]].mean()),
               "| cycles/tile %.0f" % cyc.mean(),
               "| by start decile", [int(cyc[order[i * len(order) // 10:(i + 1) * len(order) // 10]].mean() / 1000)
                                     for i in range(10)])
