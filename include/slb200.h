@@ -427,6 +427,30 @@ int slb_bellman_argmax(void* stream, const slb_bellman* cfg, int64_t idx_begin, 
 int slb_max_abs_diff(void* stream, const double* a_dev, const double* b_dev, int64_t n,
                      double* result_dev);
 
+/* ---- closed-loop rollouts x <- f(x, pi(x)) (examples/utilities.py:654-686 compute_roa,
+ *      :522-545 reward_rollout).  The slb_bellman descriptor carries the closed loop: `policy`,
+ *      deterministic `dynamics` (gp.num_outputs must be 0), and `reward` for slb_reward_rollout;
+ *      `value`, `gamma` and `action` are ignored, fixed_action must be 0.  The state dimension d is
+ *      grid.ndim.  Start states: the device array states_dev [n, d], or, when states_dev is NULL,
+ *      the grid points of flat indices [idx_begin, idx_begin + n).
+ *      workspace_dev: >= slb_rollout_workspace(cfg, n, reward) bytes (reward = 1 for
+ *      slb_reward_rollout); slb_rollout needs none when horizon <= 33. ---------------------------- */
+int64_t slb_rollout_workspace(const slb_bellman* cfg, int64_t n, int32_t reward);
+/* compute_roa: applies the closed loop horizon - 1 times (none for horizon <= 1);
+ * roa_dev[i] = ||x_end - equilibrium||_2 <= tol (numpy's row norm; NaN / inf end states give 0).
+ * equilibrium_host: HOST array of d doubles, or NULL for the origin.  end_states_dev [n, d] may be
+ * NULL; traj_dev NULL or [n, d, horizon] (trajectory[:, :, 0] = start states, horizon >= 1). */
+int slb_rollout(void* stream, const slb_bellman* cfg, const double* states_dev, int64_t idx_begin,
+                int64_t n, int32_t horizon, const double* equilibrium_host, double tol,
+                uint8_t* roa_dev, double* end_states_dev, double* traj_dev, void* workspace_dev);
+/* reward_rollout: for t = 0 .. horizon - 1:  temp = discount_dev[t] * r(x_t, pi(x_t)),
+ * sums_dev[i] += temp, stop after the first t with max_i |temp_i| < tol (a NaN anywhere: not below),
+ * x_{t+1} = f(x_t, pi(x_t)).  discount_dev [horizon] = discount ** t as computed by the caller.
+ * stop_dev (device int64) receives that first t, or -1 when the sums did not converge. */
+int slb_reward_rollout(void* stream, const slb_bellman* cfg, const double* states_dev, int64_t idx_begin,
+                       int64_t n, int32_t horizon, const double* discount_dev, double tol,
+                       double* sums_dev, int64_t* stop_dev, void* workspace_dev);
+
 #ifdef __cplusplus
 }
 #endif

@@ -10,6 +10,7 @@ from .functions import config  # noqa: F401  (singleton, like safe_learning.conf
 from .functions import *  # noqa: F401,F403
 from .lyapunov import *  # noqa: F401,F403
 from .reinforcement_learning import *  # noqa: F401,F403
+from .rollout import *  # noqa: F401,F403
 from . import utilities  # noqa: F401
 
 __version__ = "0.1.0"

@@ -28,7 +28,8 @@ UNITS = [("gp_tile_%d_%d.o" % (d, tp), "gp_tile_inst.cu",
 UNITS += [("gp_sweep.o", "gp_sweep.cu", [], ["gp_args.h"]),
           ("filter.o", "filter.cu", [], ["bulk_copy.cuh", "exp2_tab512.cuh", "gp_mean_staged.cuh", "gp_args.h"]),
           ("light.o", "light.cu", [], ["bulk_copy.cuh", "exp2_tab512.cuh", "gp_mean_staged.cuh"]),
-          ("bellman_tile.o", "bellman_tile.cu", [], [])]
+          ("bellman_tile.o", "bellman_tile.cu", [], []),
+          ("rollout.o", "rollout.cu", [], [])]
 SOURCES = sorted({u[1] for u in UNITS})
 
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]

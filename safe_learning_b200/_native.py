@@ -162,6 +162,11 @@ SIGNATURES = {
     "slb_bellman_argmax": (C.c_int, [_vp, C.POINTER(SlbBellman), _i64, _i64, _dp, _i32, _dp, _dp,
                                      _dp, _vp]),
     "slb_max_abs_diff": (C.c_int, [_vp, _dp, _dp, _i64, _dp]),
+    "slb_rollout_workspace": (C.c_int64, [C.POINTER(SlbBellman), _i64, _i32]),
+    "slb_rollout": (C.c_int, [_vp, C.POINTER(SlbBellman), _dp, _i64, _i64, _i32, _dp, C.c_double,
+                              _vp, _dp, _dp, _vp]),
+    "slb_reward_rollout": (C.c_int, [_vp, C.POINTER(SlbBellman), _dp, _i64, _i64, _i32, _dp,
+                                     C.c_double, _dp, _vp, _vp]),
 }
 
 _lib = None

@@ -8,8 +8,12 @@
   det_linear  deterministic LinearSystem dynamics on 4096^2 / 8192^2 (closest to the HBM roofline)
   c4        cart-pole 32^4 grid, M=2000, four factors, LyapunovNetwork V (C4 at 1-GPU size)
   nb        the reference's 2001x1501 pendulum experiment with its own covariance expressions
+  roa       compute_roa of the saturated-LQR closed loops: pendulum 2001x1501 (horizon 500),
+            pendulum 101^2 with trajectories, cart-pole 51^4 (horizon 2000)
+  reward_rollout  reward_rollout of the pendulum loop on 2001x1501 (discount 0.95, horizon 1000,
+            tol 1e-2), reporting the stopping step T*
 
-    python tools/bench_extra.py [bellman] [det] [c5] [shared]
+    python tools/bench_extra.py [bellman] [det] [c5] [shared] [roa] [reward_rollout]
 """
 import json
 import os
@@ -211,6 +215,139 @@ def argmax():
                       "speedup": out["per_action_sweeps"]["ms"] / out["factored"]["ms"],
                       "factored_tflops": flops / (out["factored"]["ms"] * 1e-3) * 1e-12,
                       "same_greedy_action_frac": same}))
+
+
+def _rollout_parts(plant):
+    """Saturated-LQR closed loop of reinforcement_learning_{pendulum,cartpole}.ipynb (cells 7-14):
+    (product ClosedLoop dynamics / reward, oracle callables)."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import oracle as O
+    import rollout_oracle as R
+    if plant == "pendulum":
+        norm = [np.array([np.deg2rad(30), np.sqrt(9.81 / 0.5)]), np.array([9.81 * 0.15 * 0.5 * np.sin(np.deg2rad(30))])]
+        args = (0.15, 0.5, 0.1, 0.01)
+        dyn, odyn = sl.InvertedPendulum(*args, normalization=norm), O.InvertedPendulum(*args, normalization=norm)
+    else:
+        m, M = 0.175, 1.732
+        norm = [np.array([0.5, np.deg2rad(30), 2., np.deg2rad(30)]), np.array([(m + M) * 4 / 0.5])]
+        args = (m, M, 0.28, 0.01, 0.01)
+        dyn, odyn = sl.CartPole(*args, normalization=norm), O.CartPole(*args, normalization=norm)
+    A, B = dyn.linearize()
+    d = A.shape[0]
+    Q, Rm = 0.1 * np.eye(d), 0.1 * np.eye(1)
+    K, _ = O.dlqr(A, B, Q, Rm)
+    rew = scipy.linalg.block_diag(-Q, -Rm)
+    pol = sl.Saturation(sl.LinearSystem((-K,)), -1., 1.)
+    opol = O.Saturation(O.LinearSystem((-K,)), -1., 1.)
+    return (sl.ClosedLoop(dyn, pol), sl.ClosedLoop(sl.QuadraticFunction(rew), pol),
+            R.closed_loop(odyn, opol), R.closed_loop(O.QuadraticFunction(rew), opol), R)
+
+
+def _gpu_info(fn):
+    """GPU name, power limit and SM clock while `fn` runs."""
+    from bench import ClockSampler
+    cs = ClockSampler(torch.cuda.current_device())
+    cs.start()
+    fn()
+    torch.cuda.synchronize()
+    c = cs.stop()
+    return {"gpu": torch.cuda.get_device_name(), "power_limit_w": c["power_limit_w"], "sm_mhz": c["sm_mhz"]}
+
+
+def _subset(grid, count=4096, seed=0):
+    idx = np.sort(np.random.default_rng(seed).choice(grid.nindex, count, replace=False))
+    return grid.index_to_state(idx)
+
+
+def roa():
+    """compute_roa of the saturated-LQR closed loops at the notebooks' sizes.  Per step and point:
+    pendulum = policy (2 DMUL + 1 DADD + clamp) + 10 Euler sub-steps (one fp64 sin, ~6 DMUL/DADD);
+    cart-pole = policy (4 DMUL + 3 DADD) + 10 sub-steps (3 fp64 sin/cos, ~40 DMUL/DADD/DFMA, 2 DDIV).
+    CUDA's fp64 sin is a range reduction plus a polynomial on the fp64 FMA pipe (~30 fp64 ops),
+    so both plants are fp64-pipe bound; trajectories add 8 d B per point-step of HBM writes."""
+    import time
+    for plant, num, horizon, tol, no_traj in (("pendulum", [2001, 1501], 500, 1e-2, True),
+                                              ("pendulum", [101, 101], 500, 1e-2, False),
+                                              ("cartpole", [51] * 4, 2000, 0.1, True)):
+        cl, _, ocl, _, R = _rollout_parts(plant)
+        d = 2 if plant == "pendulum" else 4
+        grid = sl.GridWorld([[-1., 1.]] * d, num)
+        n = grid.nindex
+        steps = 3 if n > 10 ** 6 else 10
+        info = _gpu_info(lambda: sl.compute_roa(grid, cl, horizon, tol, no_traj=no_traj))
+        ms = timed(lambda: sl.compute_roa(grid, cl, horizon, tol, no_traj=no_traj), steps=steps, warmup=1)
+        # parity and the numpy oracle's rate on a seeded subset of 4096 start states
+        sub = _subset(grid)
+        t0 = time.perf_counter()
+        want = R.compute_roa(sub, ocl, horizon, tol)
+        cpu_s = time.perf_counter() - t0
+        got = sl.compute_roa(sub, cl, horizon, tol)
+        full = sl.compute_roa(grid, cl, horizon, tol)
+        idx = np.sort(np.random.default_rng(0).choice(n, 4096, replace=False))
+        point_steps = n * max(horizon - 1, 0)
+        line = {"bench": "compute_roa", "plant": plant, "grid": "x".join(map(str, num)), "points": n,
+                "horizon": horizon, "no_traj": no_traj, "ms": ms,
+                "point_steps_per_s": point_steps / (ms * 1e-3),
+                "oracle_point_steps_per_s": 4096 * (horizon - 1) / cpu_s,
+                "oracle_subset": "4096 seeded start states (numpy, one process)",
+                "roa_points": int(full.sum()),
+                "parity": {"subset_flags_equal": int((got == want).sum()), "subset": 4096,
+                           "full_vs_subset_equal": bool(np.array_equal(full[idx], got))}}
+        if not no_traj:
+            traj_bytes = n * d * horizon * 8
+            line["traj_bytes_per_s"] = traj_bytes / (ms * 1e-3)
+            line["traj_frac_of_hbm_datasheet"] = traj_bytes / (ms * 1e-3) / (HBM_GBS * 1e9)
+            line["note"] = ("latency-bound: %d sequential chains in %d blocks of 64 threads, 1-2 warps "
+                            "per SM of 132; the time includes the host copy of the trajectory array"
+                            % (n, -(-n // 64)))
+        line.update(info)
+        print(json.dumps(line))
+        torch.cuda.empty_cache()
+
+
+def reward_rollout():
+    """reward_rollout of the pendulum's saturated-LQR loop on 2001 x 1501, discount 0.95,
+    horizon 1000, tol 1e-2: chunks of 32 steps, grid-wide early stop decided on the device."""
+    import contextlib
+    import io
+    import time
+    cl, rw, ocl, orw, R = _rollout_parts("pendulum")
+    grid = sl.GridWorld([[-1., 1.]] * 2, [2001, 1501])
+    n = grid.nindex
+    quiet = contextlib.redirect_stdout(io.StringIO())
+    with quiet:
+        info = _gpu_info(lambda: sl.reward_rollout(grid, cl, rw, 0.95, 1000, 1e-2))
+        ms = timed(lambda: sl.reward_rollout(grid, cl, rw, 0.95, 1000, 1e-2), steps=5, warmup=1)
+    buf = io.StringIO()
+    with contextlib.redirect_stdout(buf):
+        sums = sl.reward_rollout(grid, cl, rw, 0.95, 1000, 1e-2)
+    msg = buf.getvalue().strip()
+    stop = int(msg.split("after ")[1].split(" ")[0]) - 1 if "after" in msg else -1
+    idx = np.sort(np.random.default_rng(0).choice(n, 4096, replace=False))
+    sub = grid.index_to_state(idx)
+    # the oracle on the subset, summed over the same steps 0..T* (tol 0: no early stop of its own)
+    t0 = time.perf_counter()
+    o_sums, _ = R.reward_rollout(sub, ocl, orw, 0.95, (stop + 1) if stop >= 0 else 1000, 0.0)
+    cpu_s = time.perf_counter() - t0
+    # T* of the subset alone, product against oracle
+    with contextlib.redirect_stdout(io.StringIO()) as b2:
+        sl.reward_rollout(sub, cl, rw, 0.95, 1000, 1e-2)
+    sub_msg = b2.getvalue()
+    sub_stop = int(sub_msg.split("after ")[1].split(" ")[0]) - 1 if "after" in sub_msg else -1
+    o_sub_stop = R.reward_rollout(sub, ocl, orw, 0.95, 1000, 1e-2)[1]
+    rel = np.abs(sums[idx] - o_sums) / np.maximum(np.abs(o_sums), 1e-300)
+    executed = (stop + 1) if stop >= 0 else 1000
+    print(json.dumps({"bench": "reward_rollout", "plant": "pendulum", "grid": "2001x1501", "points": n,
+                      "discount": 0.95, "horizon": 1000, "tol": 1e-2, "T_star": stop, "ms": ms,
+                      "point_steps_per_s": n * executed / (ms * 1e-3),
+                      "oracle_point_steps_per_s": 4096 * executed / cpu_s,
+                      "oracle_subset": "4096 seeded start states (numpy, one process)",
+                      "parity": {"subset_T_star": sub_stop, "oracle_subset_T_star": o_sub_stop,
+                                 "sums_max_rel_diff": float(rel.max()),
+                                 "sums_finite_equal": bool(np.array_equal(np.isfinite(sums[idx]),
+                                                                          np.isfinite(o_sums)))},
+                      "note": "point-steps counted up to T*; the chunk holding T* runs twice "
+                              "(at most 32 extra steps)", **info}))
 
 
 if __name__ == "__main__":
