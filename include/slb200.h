@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define SLB_ABI_VERSION 5   /* 2: slb_gp_factor.kernel (covariance expressions), GRADIENT / MAXABS flags
+#define SLB_ABI_VERSION 6   /* 2: slb_gp_factor.kernel (covariance expressions), GRADIENT / MAXABS flags
                                3: decision filter (slb_gp_factor.Whead, slb_lyapunov_sweep_filtered),
                                   state-dependent lipschitz_dynamics, peer-memory key exchange
                                   (slb_exchange), fixed-action Bellman tables
@@ -36,7 +36,8 @@ extern "C" {
                                   head_rows / hmax, slb_gp_output.gamma_f / gamma_l1): pivoted head
                                   subset, computed error bound of the filter's mean
                                5: fp32 screening stage in front of the filter (slb_debug_screening_probe,
-                                  bit 2 of slb_debug_filter_stages); no structure changed           */
+                                  bit 2 of slb_debug_filter_stages); no structure changed
+                               6: slb_debug_refine_split takes one threshold (no 16-point tiles)    */
 #define SLB_MAX_DIM 6   /* state dimension d                         */
 #define SLB_MAX_IN  8   /* GP input dimension d_in = d + m           */
 #define SLB_MAX_OUT 6   /* stacked one-output GPs (FunctionStack)    */
@@ -315,11 +316,11 @@ int         slb_debug_screening_probe(double* mu_dev, double* dm_dev);
  * linear dynamics, quadratic V, constant / abs-linear L_V) take a specialised register-resident
  * kernel; 0 switches back to the generic interpreter (A/B timing, parity tests). */
 int         slb_debug_det_fast(int32_t enable);
-/* diagnostics / tuning: the refine pass of slb_lyapunov_sweep_filtered uses 16-point tiles for
- * lists of up to `upto16` points, 32-point tiles up to `upto32`, 64-point tiles beyond (defaults
- * 0 -- no 16-point launch -- and 32 points per SM, 32 * 132); with 16- and 32-point tiles the rows of a tile are additionally split
- * over the CTAs a one-per-SM grid has to spare (up to 8 per tile) */
-int         slb_debug_refine_split(int64_t upto16, int64_t upto32);
+/* diagnostics: the refine pass of slb_lyapunov_sweep_filtered uses 32-point tiles for lists of up
+ * to `upto32` points and 64-point tiles beyond (default 32 points per SM, 32 * 132); with 32-point
+ * tiles the rows of a tile are additionally split over the CTAs a one-per-SM grid has to spare (up
+ * to 8 per tile) */
+int         slb_debug_refine_split(int64_t upto32);
 
 /* ---- GP factor packing (after GPRCached.update_cache, functions.py:395-415) ------------ */
 /* doubles needed for the packed L^-1 of an M-point GP */

@@ -19,12 +19,8 @@ OUTPUT = os.path.join(HERE, "libslb200.so")
 HEADER = os.path.join(HERE, "..", "include", "slb200.h")
 
 # (object name, source, extra flags, headers it depends on besides common.cuh / slb200.h)
-# depth of the register ring that streams L^-1 ahead of the DMMAs: the short tiles of the refine pass
-# do 4x / 2x less math per streamed byte, so they need more bytes in flight to cover the L2 latency
-RING = {64: 3, 32: 5, 16: 8}
-UNITS = [("gp_tile_%d_%d.o" % (d, tp), "gp_tile_inst.cu",
-          ["-DSLB_TILE_DIN=%d" % d, "-DSLB_TP=%d" % tp, "-DSLB_RING=%d" % RING[tp]],
-          ["gp_tile.cuh", "gp_args.h"]) for d in range(1, 7) for tp in (64, 32, 16)]
+UNITS = [("gp_tile_%d_%d.o" % (d, tp), "gp_tile_inst.cu", ["-DSLB_TILE_DIN=%d" % d, "-DSLB_TP=%d" % tp],
+          ["gp_tile.cuh", "gp_args.h"]) for d in range(1, 7) for tp in (64, 32)]
 UNITS += [("gp_sweep.o", "gp_sweep.cu", [], ["gp_args.h"]),
           ("filter.o", "filter.cu", [], ["bulk_copy.cuh", "exp2_tab512.cuh", "gp_mean_staged.cuh", "gp_args.h"]),
           ("light.o", "light.cu", [], ["bulk_copy.cuh", "exp2_tab512.cuh", "gp_mean_staged.cuh"]),

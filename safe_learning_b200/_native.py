@@ -25,7 +25,7 @@ FLAG_SATURATE, FLAG_ABS, FLAG_NORM1, FLAG_PROJECT, FLAG_SCALE, FLAG_GRADIENT, FL
     1, 2, 4, 8, 16, 32, 64
 K_RBF, K_MATERN12, K_MATERN32, K_MATERN52, K_LINEAR, K_CONSTANT, K_WHITE = range(7)
 SLB_MAX_KPRIM = 6
-ABI_VERSION = 5
+ABI_VERSION = 6
 
 UINT64_MAX = (1 << 64) - 1
 INT64_MAX = (1 << 63) - 1
@@ -114,9 +114,7 @@ class SlbExchange(C.Structure):
 _STRUCTS = (SlbGrid, SlbFunction, SlbGpFactor, SlbGpOutput, SlbGpStack, SlbSweep, SlbBellman,
             SlbFailKey, SlbPrefixStats, SlbExchange)
 
-# SLB200_LIB lets a diagnostic run load an alternative build (A/B timing of kernel variants)
-LIB_PATH = os.environ.get("SLB200_LIB") or os.path.join(
-    os.path.dirname(os.path.abspath(__file__)), "libslb200.so")
+LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "libslb200.so")
 
 _vp, _i64, _i32, _dp = C.c_void_p, C.c_int64, C.c_int32, C.c_void_p
 
@@ -131,7 +129,7 @@ SIGNATURES = {
     "slb_debug_phase_timing": (C.c_int, [_vp]),
     "slb_record_factor_dependency": (C.c_int, [_vp]),
     "slb_restore_tables": (C.c_int, [_vp, _vp, _i64, _i64, _vp, _vp]),
-    "slb_debug_refine_split": (C.c_int, [_i64, _i64]),
+    "slb_debug_refine_split": (C.c_int, [_i64]),
     "slb_debug_det_fast": (C.c_int, [_i32]),
     "slb_debug_filter_stages": (C.c_int, [_i32]),
     "slb_debug_screening_probe": (C.c_int, [_dp, _dp]),

@@ -9,8 +9,6 @@
 // the CPU oracle.  Only the GP contraction (DMMA) and libm calls (exp/sin/cos/sqrt is exact)
 // differ in rounding.
 #pragma once
-#include <stdlib.h>
-
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <math.h>
@@ -39,48 +37,6 @@ void slb_count_launch();
             return 2;                                                            \
         }                                                                        \
     } while (0)
-
-// ---- programmatic dependent launch (PDL) --------------------------------------------------------
-// The kernels of one sweep form a chain in which every kernel starts with work that does not depend
-// on its predecessor (staging static tables by TMA, L2 prefetches, descriptor loads) -- and with
-// launch latency and CTA ramp-up.  Launched with the programmatic-stream-serialization attribute a
-// kernel may start as soon as every CTA of its predecessor has called pdl_launch_dependents() (or
-// left); it must call pdl_wait() before it touches anything the predecessor produces (the wait
-// returns once the predecessor grid has completed and its writes are visible).  Both calls are
-// no-ops in a kernel launched the ordinary way.  The attribute is OFF by default: the dependents' early
-// CTAs take shared memory and registers the predecessor's last CTAs still want, and the kernels'
-// pre-dependency parts are short.  SLB200_PDL=1 switches it on (all GPU tests pass either way).
-#if defined(__CUDACC__)
-__device__ __forceinline__ void pdl_launch_dependents() {
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-}
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-
-inline bool slb_pdl_enabled() {
-    static const bool on = [] {
-        const char* e = getenv("SLB200_PDL");
-        return e ? (atoi(e) != 0) : false;
-    }();
-    return on;
-}
-
-// kernel<<<grid, block, smem, st>>>(args...) as a programmatic dependent of the previous kernel in `st`
-template <typename... KArgs, typename... Args>
-inline cudaError_t slb_launch_dependent(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem,
-                                        cudaStream_t st, Args&&... args) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = grid;
-    cfg.blockDim = block;
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = slb_pdl_enabled() ? 1 : 0;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
-}
-#endif
 
 #define SLB_LAUNCH_CHECK()                                                       \
     do {                                                                         \

@@ -31,20 +31,13 @@
 
 #include <atomic>
 #include <string.h>
-#include <stdlib.h>
 
 #include "gp_mean_staged.cuh"
 #include "gp_args.h"
 
 namespace {
 
-#ifndef SLB_FT
-#define SLB_FT 64
-#endif
-#ifndef SLB_MEAN_MINB
-#define SLB_MEAN_MINB 7
-#endif
-constexpr int FT = SLB_FT;             // stage 1: threads per CTA = points per CTA (1024 CTAs at
+constexpr int FT = 64;                 // stage 1: threads per CTA = points per CTA (1024 CTAs at
                                        // 256 x 256, 7 resident per SM)
 constexpr int HR = SLB_HEAD_RANK;
 constexpr int HT = 512;                // stage 2: threads per CTA (16 warps, 8 or 2 list entries each)
@@ -199,10 +192,9 @@ SLB_DEV double screening_slack(const slb_sweep& cfg, const double* mu, const dou
 }
 
 template <int DIN>
-__global__ void __launch_bounds__(FT, SLB_MEAN_MINB)
+__global__ void __launch_bounds__(FT, 7)
 filter_mean_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    pdl_launch_dependents();                      // the head stage may start staging its tables
     prefetch_descriptor_operands(cfg);
     mean_pipe P;
     double *tab512, *tab64;
@@ -269,11 +261,10 @@ filter_mean_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
 // threshold and V(x) only; the head stage recomputes their mean in fp64 (warp-cooperatively, on ~8% of
 // the grid at C2), so everything downstream of this kernel is the fp64 arithmetic of the other path.
 template <int DIN>
-__global__ void __launch_bounds__(FT, SLB_MEAN_MINB)
+__global__ void __launch_bounds__(FT, 7)
 filter_mean32_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     __shared__ double s_cen[SLB_MAX_IN];
-    pdl_launch_dependents();                      // the head stage may start staging its tables
     prefetch_descriptor_operands(cfg);
     constexpr int W32 = row32<DIN>::W;
     mean_pipe P;
@@ -636,7 +627,6 @@ template <int DIN>
 __global__ void __launch_bounds__(HT, 1)
 filter_head_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    pdl_launch_dependents();                      // the refine launch may get its CTAs ready
     prefetch_descriptor_operands(cfg);
     uint64_t* bar = reinterpret_cast<uint64_t*>(smem_raw);             // [1]
     unsigned* s_stat = reinterpret_cast<unsigned*>(smem_raw + 8);      // decided / undecided by this CTA
@@ -647,10 +637,10 @@ filter_head_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
     const int nf = cfg.gp.num_factors;
     double* xbuf = wbuf + (size_t)a.head_factors_staged * HR * HR;     // [staged][HR * DIN]
     double* mbuf = xbuf + (size_t)a.head_factors_staged * HR * DIN;    // screened: [Xf | gamma_f ...] per factor
-    // ---- everything that does not depend on stage 1 first (the kernel is a programmatic dependent of
-    // it: this part overlaps stage 1's tail).  The refine pass that follows streams every factor's
-    // packed L^-1 (1 MB at M = 500); if it is not L2-resident by then (first sweep after a cache
-    // update, or evicted in between) its CTAs start with HBM round trips in lockstep: prefetch it.
+    // ---- everything that does not depend on stage 1's lists first.  The refine pass that follows
+    // streams every factor's packed L^-1 (1 MB at M = 500); if it is not L2-resident by then (first
+    // sweep after a cache update, or evicted in between) its CTAs start with HBM round trips in
+    // lockstep: prefetch it.
     if (a.prefetch_factors) {
         for (int f = 0; f < nf; ++f) {
             const slb_gp_factor& F = cfg.gp.factors[f];
@@ -711,7 +701,6 @@ filter_head_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
         reinterpret_cast<int*>(mbuf + a.mean_doubles + 2 * HW * HP * SLB_MAX_OUT)[threadIdx.x] = 0;
     __syncthreads();
     slb_bulk::mbar_wait(bar, 0);                  // also before leaving: the copies land in this CTA's memory
-    pdl_wait();                                   // ---- stage 1 has completed: its lists are visible
     const int64_t count = (int64_t)a.counts[0];
     const int64_t nwarps = (int64_t)gridDim.x * HW;
     const int64_t ngroups = (count + HP - 1) / HP;
@@ -819,11 +808,7 @@ void head_layout(const slb_sweep& cfg, int din, filter_args& ah, size_t& head_sm
     head_smem = head_fixed + ah.head_factors_staged * per_factor;
     ah.screened = 0;
     ah.mean_doubles = 0;
-    static const int head_prefetch = [] {                  // SLB200_HEAD_PREFETCH=0: A/B timing knob
-        const char* e = getenv("SLB200_HEAD_PREFETCH");
-        return e ? (atoi(e) != 0) : 1;
-    }();
-    ah.prefetch_factors = ((g_filter_stages & 2) && head_prefetch) ? 1 : 0;
+    ah.prefetch_factors = (g_filter_stages & 2) ? 1 : 0;
     if (screening_applicable(cfg) && ah.head_factors_staged == cfg.gp.num_factors) {
         int off = 0;
         for (int f = 0; f < cfg.gp.num_factors; ++f) {
@@ -870,7 +855,7 @@ int launch_filter(cudaStream_t st, const slb_sweep& cfg, const filter_args& a, s
     }
     SLB_LAUNCH_CHECK();
     if (!(g_filter_stages & 1)) return 0;
-    SLB_CUDA(slb_launch_dependent(filter_head_kernel<DIN>, dim3(HEAD_CTAS), dim3(HT), head_smem, st, cfg, ah));
+    filter_head_kernel<DIN><<<HEAD_CTAS, HT, head_smem, st>>>(cfg, ah);
     SLB_LAUNCH_CHECK();
     return 0;
 }
@@ -980,10 +965,7 @@ int slb_lyapunov_sweep_filtered(void* stream, const slb_sweep* cfg, int64_t idx_
     // rows per staged slice: two buffers of (d_in + 1 + outputs per factor) doubles per row within
     // ~24 KB, so that 7 CTAs stay resident per SM
     const int din = cfg->gp.input_dim;
-#ifndef SLB_MEAN_SMEM_KB
-#define SLB_MEAN_SMEM_KB 24
-#endif
-    a.chunk_rows = mean_chunk_rows(din, nomax, SLB_MEAN_SMEM_KB);
+    a.chunk_rows = mean_chunk_rows(din, nomax, 24);
     a.max_outputs_per_factor = nomax;
     const size_t smem = mean_smem_bytes(din, nomax, a.chunk_rows);
     for (int64_t off = 0; off < n_all; off += CHUNK) {

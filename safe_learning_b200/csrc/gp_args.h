@@ -23,15 +23,13 @@ struct slb_gp_args {
     const int64_t* index_list;           // refine mode: the tile's points are index_list[rel]
     const unsigned long long* count;     // refine mode: number of list entries (read on the device)
     int64_t count_min, count_max;        // refine mode: this launch works iff count_min < *count <= count_max
-    // refine mode, short lists: the rows of L^-1 of one point tile are split over up to `split_max`
+    // refine mode, short lists: the rows of L^-1 of one point tile are split over up to SLB_SPLIT_MAX
     // CTAs (equal triangular areas); every CTA leaves its partial sums in `split_partial`
     // [CTA][factor][1 + MAX_OUT][tile points], the last one to arrive at `split_ticket[tile]` adds
-    // them in group order and finishes the tile.  NULL / 0: no split.  Grids of at most
+    // them in group order and finishes the tile.  NULL: no split.  Grids of at most
     // SLB_SPLIT_ITEMS CTAs.
     double* split_partial;
     int* split_ticket;
-    int32_t split_max;
-    int32_t split_factors;  // 1: with CTAs to spare, the factors of a tile go to separate CTAs before its rows are split
     long long* timing;      // diagnostics: [tile][warp][8]: cycles in {generate, contract, epilogue, total}, globaltimer ns {start, end}, cycles waiting at barriers, 0
 };
 

@@ -11,10 +11,7 @@
 #include "bulk_copy.cuh"
 #include "exp2_tab512.cuh"
 
-#ifndef SLB_MEAN_UNROLL
-#define SLB_MEAN_UNROLL 4
-#endif
-constexpr int MEAN_UNROLL = SLB_MEAN_UNROLL;   // independent exp chains per thread (rows per iteration)
+constexpr int MEAN_UNROLL = 4;         // independent exp chains per thread (rows per iteration)
 constexpr double EPS_K = 1.0e-13;      // certified relative error of exp_neg_fast incl. its argument
 
 // exp(x) for -700 < x <= 0 (+ rounding) to 3.3e-14 relative (tools/exp_neg_fast_check.c):

@@ -5,14 +5,11 @@
 
 #include <string.h>
 
-#include <stdlib.h>
-
 #include "gp_args.h"
 
 #define SLB_DECLARE_TILE(d) \
     int slb_gp_tile_launch_##d##_64(cudaStream_t, const slb_sweep&, const slb_gp_args&, bool, bool); \
-    int slb_gp_tile_launch_##d##_32(cudaStream_t, const slb_sweep&, const slb_gp_args&, bool, bool); \
-    int slb_gp_tile_launch_##d##_16(cudaStream_t, const slb_sweep&, const slb_gp_args&, bool, bool);
+    int slb_gp_tile_launch_##d##_32(cudaStream_t, const slb_sweep&, const slb_gp_args&, bool, bool);
 SLB_DECLARE_TILE(1) SLB_DECLARE_TILE(2) SLB_DECLARE_TILE(3)
 SLB_DECLARE_TILE(4) SLB_DECLARE_TILE(5) SLB_DECLARE_TILE(6)
 #undef SLB_DECLARE_TILE
@@ -58,7 +55,7 @@ int wait_for_factors(cudaStream_t st) {
     return 0;
 }
 
-// tp: points per CTA (64 for sweeps and point lists; 32 / 16 only in the refine pass)
+// tp: points per CTA (64 for sweeps and point lists; 32 only in the refine pass)
 int dispatch_gp_tile(cudaStream_t st, const slb_sweep& cfg, const slb_gp_args& a, int tp = 64) {
     if (a.n <= 0) return 0;
     if (wait_for_factors(st)) return 1;
@@ -69,8 +66,7 @@ int dispatch_gp_tile(cudaStream_t st, const slb_sweep& cfg, const slb_gp_args& a
 #define SLB_TILE_CASE(d)                                                                   \
     case d:                                                                                \
         return tp == 64 ? slb_gp_tile_launch_##d##_64(st, cfg, a, kexpr, timing)           \
-             : tp == 32 ? slb_gp_tile_launch_##d##_32(st, cfg, a, kexpr, timing)           \
-                        : slb_gp_tile_launch_##d##_16(st, cfg, a, kexpr, timing);
+                        : slb_gp_tile_launch_##d##_32(st, cfg, a, kexpr, timing);
     switch (cfg.gp.input_dim) {
         SLB_TILE_CASE(1) SLB_TILE_CASE(2) SLB_TILE_CASE(3)
         SLB_TILE_CASE(4) SLB_TILE_CASE(5) SLB_TILE_CASE(6)
@@ -94,9 +90,9 @@ static long long* g_timing_buffer = nullptr;
 // holds their indices relative to idx_begin, `count` (device) how many there are.  The list is
 // usually a small fraction of the grid -- too short to fill the SMs with 64-point tiles, and a
 // tile's duration does not shrink with the list -- so the pass is launched once per tile size
-// (16, 32, 64 points per CTA) and only the launch whose range holds the list length does work;
-// the CTAs of the others (and those beyond the list) leave at once.
-static int64_t g_refine_split[2] = {0, 32 * SLB_NUM_SMS};   // 16-point tiles: diagnostics only (an empty launch still costs)
+// (32 and 64 points per CTA) and only the launch whose range holds the list length does work;
+// the CTAs of the other (and those beyond the list) leave at once.
+static int64_t g_refine_split = 32 * SLB_NUM_SMS;   // longest list that gets 32-point tiles
 
 // Short lists (<= 32 points per SM) additionally split every tile's ROWS over the CTAs the grid has
 // to spare (up to SLB_SPLIT_MAX groups of equal triangular area, gp_tile.cuh): the tile kernel's
@@ -111,30 +107,19 @@ int slb_launch_refine(cudaStream_t st, const slb_sweep& cfg, int64_t n_max, int6
     a.negative = negative; a.values = values;
     a.index_list = list; a.count = count;
     a.timing = g_timing_buffer;            // slb_debug_phase_timing: per-warp phase clocks of the refine CTAs
-    const int tps[3] = {16, 32, 64};
-    const int64_t lo[3] = {0, g_refine_split[0], g_refine_split[1]};
-    const int64_t hi[3] = {g_refine_split[0], g_refine_split[1], INT64_MAX};
-    for (int v = 0; v < 3; ++v) {
+    const int tps[2] = {32, 64};
+    const int64_t lo[2] = {0, g_refine_split};
+    const int64_t hi[2] = {g_refine_split, INT64_MAX};
+    for (int v = 0; v < 2; ++v) {
         if (lo[v] >= hi[v] || lo[v] >= n_max) continue;
         a.count_min = lo[v]; a.count_max = hi[v];
         a.n = n_max < hi[v] ? n_max : hi[v];        // the grid never needs to cover more
-        a.split_partial = nullptr; a.split_ticket = nullptr; a.split_max = 1;
-        if (v < 2 && split_partial != nullptr) {
+        a.split_partial = nullptr; a.split_ticket = nullptr;
+        if (v == 0 && split_partial != nullptr) {
             // at least one CTA per SM, so that short lists have CTAs to spread their rows over
             if (a.n < (int64_t)SLB_NUM_SMS * tps[v]) a.n = (int64_t)SLB_NUM_SMS * tps[v];
             if ((a.n + tps[v] - 1) / tps[v] <= SLB_SPLIT_ITEMS) {
                 a.split_partial = split_partial; a.split_ticket = split_ticket;
-                static const int split_max = [] {          // SLB200_SPLIT_MAX: A/B timing knob
-                    const char* e = getenv("SLB200_SPLIT_MAX");
-                    const int v = e ? atoi(e) : SLB_SPLIT_MAX;
-                    return v < 1 ? 1 : (v > SLB_SPLIT_MAX ? SLB_SPLIT_MAX : v);
-                }();
-                a.split_max = split_max;
-                static const int split_factors = [] {      // SLB200_SPLIT_FACTORS=0: A/B timing knob
-                    const char* e = getenv("SLB200_SPLIT_FACTORS");
-                    return e ? atoi(e) : 1;
-                }();
-                a.split_factors = split_factors;
             }
         }
         const int rc = dispatch_gp_tile(st, cfg, a, tps[v]);
@@ -145,10 +130,9 @@ int slb_launch_refine(cudaStream_t st, const slb_sweep& cfg, int64_t n_max, int6
 
 extern "C" {
 
-/* diagnostics: list lengths up to which the refine pass uses 16- and 32-point tiles */
-int slb_debug_refine_split(int64_t upto16, int64_t upto32) {
-    g_refine_split[0] = upto16 < 0 ? 0 : upto16;
-    g_refine_split[1] = upto32 < g_refine_split[0] ? g_refine_split[0] : upto32;
+/* diagnostics: list length up to which the refine pass uses 32-point tiles */
+int slb_debug_refine_split(int64_t upto32) {
+    g_refine_split = upto32 < 0 ? 0 : upto32;
     return 0;
 }
 

@@ -11,7 +11,7 @@
 //
 // Design (H100, fp64 pipe bound -- see DESIGN.md section 3.1):
 //   * one CTA = 64 grid points x all M training points, 8 warps, 1 CTA/SM (~178 KB shared
-//     memory); SLB_NW=16 builds the 16-warp variant.
+//     memory).
 //   * W = L^-1 (lower triangular) is pre-packed in DMMA.8x8x4 A-fragment order, two k-steps
 //     per 128-bit element (slb_pack_factor); each warp streams ITS rows of W straight from L2
 //     into registers with coalesced 512 B loads through a static three-deep register ring --
@@ -42,10 +42,10 @@ namespace {
 #ifndef SLB_TP
 #define SLB_TP SLB_TILE_POINTS
 #endif
-constexpr int TP = SLB_TP;            // points per CTA: 64 for sweeps; 32 / 16 for the refine pass of
-                                      // the filtered sweep, whose short point list would otherwise
-                                      // fill only a fraction of the SMs (one translation unit each)
-static_assert(TP == 16 || TP == 32 || TP == 64, "TP must be 16, 32 or 64");
+constexpr int TP = SLB_TP;            // points per CTA: 64 for sweeps; 32 for the refine pass of the
+                                      // filtered sweep, whose short point list would otherwise fill
+                                      // only a fraction of the SMs (one translation unit each)
+static_assert(TP == 32 || TP == 64, "TP must be 32 or 64");
 constexpr int PANEL = 256;            // rows per i-panel, columns per j-panel
 // K-row tile layout in shared memory: k-steps are handled in PAIRS (8 rows of K).  Row j of a
 // panel lives at pair m = j / 8, half h = (j / 4) % 2, fragment row r = j % 4; element (j, p) is
@@ -53,13 +53,9 @@ constexpr int PANEL = 256;            // rows per i-panel, columns per j-panel
 // k-steps of a pair.  KSTR = 66: (r * 66 + c) mod 8 is distinct for r in 0..3, c in 0..1, i.e. the
 // eight lanes of a quarter-warp hit eight different 16-byte bank groups (conflict-free LDS.128).
 constexpr int KSTR = TP + 2;
-#ifndef SLB_NW
-#define SLB_NW 8
-#endif
-constexpr int NW = SLB_NW;            // warps per CTA (8 or 16)
+constexpr int NW = 8;                 // warps per CTA
 constexpr int NT = NW * 32;
 constexpr int RQ = 32 / NW;           // 8-row blocks per warp per 256-row panel (RQ * NW = 32)
-static_assert(NW == 8 || NW == 16, "NW must be 8 or 16");
 constexpr int NB = TP / 8;            // 8-point column blocks per warp tile
 constexpr int CTAS_PER_SM = 1;
 constexpr int NRED = 1 + SLB_MAX_OUT;
@@ -89,6 +85,11 @@ SLB_DEV void dmma884(double& c0, double& c1, double a, double b) {
                  : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
 }
 
+// depth of the register ring that streams L^-1 ahead of the DMMAs: the 32-point tiles of the refine
+// pass do half the math per streamed byte, so they need more bytes in flight to cover the L2 latency
+constexpr int RING = TP == 64 ? 3 : 5;
+constexpr int BG = 4;                 // column blocks whose B fragments are loaded together
+
 // Pairs [m0, m1) of k-steps of the current j-panel for row blocks q >= Q0 of this warp.
 // Per pair and row block ONE 128-bit global load brings the A fragments of both k-steps
 // (the packed factor stores them adjacent), per column block ONE 128-bit shared load brings both
@@ -97,14 +98,6 @@ SLB_DEV void dmma884(double& c0, double& c1, double a, double b) {
 template <int Q0>
 SLB_DEV void mma_run(double (&acc)[RQ][NB][2], const double2* const (&ap)[RQ], int m0, int m1,
                      const double2* ks_lane) {
-#ifndef SLB_RING
-#define SLB_RING 3
-#endif
-#ifndef SLB_BGROUP
-#define SLB_BGROUP 4
-#endif
-    constexpr int RING = SLB_RING;
-    constexpr int BG = SLB_BGROUP < NB ? SLB_BGROUP : NB;   // column blocks whose B fragments are loaded together
     double2 ar[RING][RQ];
     const int m1m = m1 - 1;
 #pragma unroll
@@ -148,7 +141,7 @@ SLB_DEV void mma_run(double (&acc)[RQ][NB][2], const double2* const (&ap)[RQ], i
 // lanes that share T%4 (lane bits 4, 3, 2) and add them to red_q[column * NRED].  Reduce-scatter:
 // every step halves the values a lane still carries (send one half, keep and add the other) --
 // NBT = 8: 8+4+2 shuffles instead of 3 per value, every lane ends with two finished columns;
-// NBT = 4: one column per lane; NBT = 2: the last step is a plain exchange (half the lanes write).
+// NBT = 4: one column per lane.
 template <int NBT>
 SLB_DEV void row_lane_reduce(const double (&v)[2 * NBT], int lane, double* red_q) {
     constexpr int NV = 2 * NBT;
@@ -178,18 +171,14 @@ SLB_DEV void row_lane_reduce(const double (&v)[2 * NBT], int lane, double* red_q
         double* slot = red_q + (8 * (lane >> 2) + 2 * (lane & 3)) * NRED;
         slot[0] += w2[0];
         slot[NRED] += w2[1];
-    } else if constexpr (NBT == 4) {
+    } else {
+        static_assert(NBT == 4, "written for 8 or 4 column blocks");
         const double send = g0 ? w4[0] : w4[1];
         const double keep = g0 ? w4[1] : w4[0];
         const double w1 = keep + __shfl_xor_sync(0xffffffffu, send, 4);
         // value index g = lane / 4  <->  nb = g / 2, e = g % 2
         const int g = lane >> 2;
         red_q[(8 * (g >> 1) + 2 * (lane & 3) + (g & 1)) * NRED] += w1;
-    } else {
-        static_assert(NBT == 2, "written for 8, 4 or 2 column blocks");
-        const double w1 = w4[0] + __shfl_xor_sync(0xffffffffu, w4[0], 4);
-        // value index 2 g2 + g1  <->  nb = g2, e = g1; the g0 = 1 lanes hold duplicates
-        if (!g0) red_q[(8 * (g2 ? 1 : 0) + 2 * (lane & 3) + (g1 ? 1 : 0)) * NRED] += w1;
     }
 }
 
@@ -286,11 +275,8 @@ SLB_DEV void gp_tile_body(const slb_sweep& cfg, const slb_gp_args& a, unsigned c
 
     // Row blocks are dealt by `wslot`; warps w and w+4 share an SMSP (and its fp64 pipe), so
     // their slots sum to 7 and every SMSP gets the same share of the triangular panels.
-    // SMSP partners (warps with equal warp % 4) get slots with equal sums: {g, 7-g} for 8 warps,
-    // {g, 7-g, 8+g, 15-g} for 16
     const int wg_ = warp & 3, wr_ = warp >> 2;
-    const int wslot = NW == 8 ? (wr_ == 0 ? wg_ : 7 - wg_)
-                              : (wr_ == 0 ? wg_ : wr_ == 1 ? 7 - wg_ : wr_ == 2 ? 8 + wg_ : 15 - wg_);
+    const int wslot = wr_ == 0 ? wg_ : 7 - wg_;
     const int p_gen = tid & (TP - 1);
     const int jg = tid / TP;                          // 0..NT/TP-1
     const double2* ks_lane = reinterpret_cast<const double2*>(Ks) + (lane & 3) * KSTR + (lane >> 2);
@@ -476,10 +462,8 @@ SLB_DEV void gp_tile_body(const slb_sweep& cfg, const slb_gp_args& a, unsigned c
                 int mprev = 0;
                 if (mend[0] > mprev) { mma_run<0>(acc, ap, mprev, mend[0], ks_lane); mprev = mend[0]; }
                 if (mend[1] > mprev) { mma_run<1>(acc, ap, mprev, mend[1], ks_lane); mprev = mend[1]; }
-                if constexpr (RQ == 4) {
-                    if (mend[2] > mprev) { mma_run<2>(acc, ap, mprev, mend[2], ks_lane); mprev = mend[2]; }
-                    if (mend[3] > mprev) { mma_run<3>(acc, ap, mprev, mend[3], ks_lane); mprev = mend[3]; }
-                }
+                if (mend[2] > mprev) { mma_run<2>(acc, ap, mprev, mend[2], ks_lane); mprev = mend[2]; }
+                if (mend[3] > mprev) { mma_run<3>(acc, ap, mprev, mend[3], ks_lane); mprev = mend[3]; }
                 if (TIMING) t_mma += clock64() - t_mark;
             }
             if (TIMING) t_mark = clock64();
@@ -630,7 +614,7 @@ SLB_DEV void gp_tile_body(const slb_sweep& cfg, const slb_gp_args& a, unsigned c
 
 // KEXPR: at least one factor carries a covariance expression (slb_kernel) instead of the plain
 // RBF; the RBF-only instantiation keeps the lean generation loop.
-// TPV (= TP) only makes the kernel's NAME unique per translation unit: the units for the three tile
+// TPV (= TP) only makes the kernel's NAME unique per translation unit: the units for the two tile
 // sizes are compiled from this one source file, nvcc derives the prefix of internal-linkage
 // kernels from the file name, and equally named kernels of different modules were resolved to
 // the same device function (observed: the 64-point launch ran the 32-point code).
@@ -647,11 +631,7 @@ gp_tile_kernel(const __grid_constant__ slb_sweep cfg, const slb_gp_args a) {
     // kernel, its length lives in device memory; CTAs beyond it leave before the first barrier
     int64_t npts = a.n;
     if (a.count != nullptr) {
-        // the refine launches are programmatic dependents of the filter's head stage (and of each
-        // other): CTAs may be resident before the list exists
-        pdl_launch_dependents();
         prefetch_descriptor_operands(cfg);
-        pdl_wait();
         npts = (int64_t)*a.count;
         // one launch per tile size; only the one whose range holds the list length does work
         if (npts <= a.count_min || npts > a.count_max) return;
@@ -663,12 +643,11 @@ gp_tile_kernel(const __grid_constant__ slb_sweep cfg, const slb_gp_args a) {
             // go to different CTAs first (half the generation phases and barriers in every CTA's
             // serial chain), the rest of the spare CTAs splits the rows
             const int nfac = cfg.gp.num_factors;
-            // (split_factors 2: already with one CTA per factor and no row split -- A/B knob)
-            if (a.split_factors && nfac > 1 && spare >= (a.split_factors > 1 ? 1 : 2) * nfac) {
+            if (nfac > 1 && spare >= 2 * nfac) {
                 FS = nfac;
                 spare /= nfac;
             }
-            G = (int)(spare < 1 ? 1 : (spare > a.split_max ? a.split_max : spare));
+            G = (int)(spare < 1 ? 1 : (spare > SLB_SPLIT_MAX ? SLB_SPLIT_MAX : spare));
             const int per_tile = G * FS;
             if ((int64_t)blockIdx.x >= ntiles * per_tile) return;
             tile_index = blockIdx.x / per_tile;
@@ -692,7 +671,7 @@ gp_tile_kernel(const __grid_constant__ slb_sweep cfg, const slb_gp_args a) {
 }
 
 // TPV: see gp_tile_kernel -- nvcc emits templates of this unnamed namespace as WEAK symbols under a
-// prefix derived from the source file name, so the three tile-size units would otherwise share
+// prefix derived from the source file name, so the two tile-size units would otherwise share
 // one launch function (the first one linked: every refine pass ran with 64-point tiles).
 template <int DIN, bool TIMING, bool KEXPR, int TPV = TP>
 int launch_gp_tile(cudaStream_t st, const slb_sweep& cfg, const slb_gp_args& a) {
@@ -711,11 +690,7 @@ int launch_gp_tile(cudaStream_t st, const slb_sweep& cfg, const slb_gp_args& a) 
     int64_t tiles = (a.n + TP - 1) / TP;
     // unsplit refine launches are persistent (see gp_tile_kernel): one CTA per SM
     if (a.count != nullptr && a.split_partial == nullptr && tiles > PREFETCH_CTAS) tiles = PREFETCH_CTAS;
-    if (a.count != nullptr)
-        SLB_CUDA(slb_launch_dependent(gp_tile_kernel<DIN, TIMING, KEXPR, TP>, dim3((unsigned)tiles), dim3(NT),
-                                      SMEM_TOTAL, st, cfg, a));
-    else
-        gp_tile_kernel<DIN, TIMING, KEXPR, TP><<<(unsigned)tiles, NT, SMEM_TOTAL, st>>>(cfg, a);
+    gp_tile_kernel<DIN, TIMING, KEXPR, TP><<<(unsigned)tiles, NT, SMEM_TOTAL, st>>>(cfg, a);
     SLB_LAUNCH_CHECK();
     return 0;
 }

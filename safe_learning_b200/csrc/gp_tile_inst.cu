@@ -1,5 +1,5 @@
 // gp_tile_inst.cu -- one translation unit per GP input dimension and tile size (compiled with
-// -DSLB_TILE_DIN=1..6 -DSLB_TP=64|32|16, in parallel): the instantiations of gp_tile_kernel
+// -DSLB_TILE_DIN=1..6 -DSLB_TP=64|32, in parallel): the instantiations of gp_tile_kernel
 // (gp_tile.cuh) -- plain RBF, covariance expressions, and (d_in = 3, 64 points) the phase-timing
 // build.
 #include "gp_tile.cuh"

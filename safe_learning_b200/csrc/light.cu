@@ -356,8 +356,6 @@ __global__ void __launch_bounds__(LT)
 first_fail_partial_kernel(const double* __restrict__ values, const uint8_t* __restrict__ negative,
                           const uint8_t* __restrict__ initial, int64_t n, int64_t idx_begin,
                           ff_partial* __restrict__ partial) {
-    pdl_launch_dependents();
-    pdl_wait();                                // programmatic dependent of the sweep's last decision kernel
     uint64_t kv = ~0ull;
     int64_t ki = INT64_MAX, nok = 0;
     for (int64_t i = (int64_t)blockIdx.x * LT + threadIdx.x; i < n; i += (int64_t)gridDim.x * LT) {
@@ -398,8 +396,6 @@ __global__ void __launch_bounds__(FF_BLOCKS)
 first_fail_final_kernel(const ff_partial* __restrict__ partial, int nparts,
                         slb_fail_key* __restrict__ result, const slb_exchange x) {
     __shared__ int64_t s_key[4];
-    pdl_launch_dependents();
-    pdl_wait();
     uint64_t kv = ~0ull;
     int64_t ki = INT64_MAX, nok = 0;
     if ((int)threadIdx.x < nparts) {
@@ -453,7 +449,6 @@ apply_prefix_kernel(const double* __restrict__ values, const uint8_t* __restrict
                     int64_t idx_begin, slb_fail_key* __restrict__ key,
                     uint8_t* __restrict__ safe, slb_prefix_stats* __restrict__ stats,
                     const slb_exchange x) {
-    pdl_wait();
     uint64_t kv;
     int64_t ki;
     if (X) {
@@ -781,13 +776,13 @@ int slb_first_fail(void* stream, const double* values_dev, const uint8_t* negati
     const int64_t want = (n + LT - 1) / LT;
     const int nparts = (int)(want < 1 ? 1 : (want > FF_BLOCKS ? FF_BLOCKS : want));
     cudaStream_t st = (cudaStream_t)stream;
-    SLB_CUDA(slb_launch_dependent(first_fail_partial_kernel, dim3(nparts), dim3(LT), 0, st, values_dev,
-                                  negative_dev, initial_dev, n, idx_begin, (ff_partial*)workspace_dev));
+    first_fail_partial_kernel<<<nparts, LT, 0, st>>>(values_dev, negative_dev, initial_dev, n, idx_begin,
+                                                     (ff_partial*)workspace_dev);
     SLB_LAUNCH_CHECK();
     slb_exchange none;
     memset(&none, 0, sizeof(none));
-    SLB_CUDA(slb_launch_dependent(first_fail_final_kernel, dim3(1), dim3(FF_BLOCKS), 0, st,
-                                  (const ff_partial*)workspace_dev, nparts, result_dev, none));
+    first_fail_final_kernel<<<1, FF_BLOCKS, 0, st>>>((const ff_partial*)workspace_dev, nparts, result_dev,
+                                                     none);
     SLB_LAUNCH_CHECK();
     return 0;
 }
@@ -813,11 +808,11 @@ int slb_first_fail_x(void* stream, const double* values_dev, const uint8_t* nega
     const int64_t want = (n + LT - 1) / LT;
     const int nparts = (int)(want < 1 ? 1 : (want > FF_BLOCKS ? FF_BLOCKS : want));
     cudaStream_t st = (cudaStream_t)stream;
-    SLB_CUDA(slb_launch_dependent(first_fail_partial_kernel, dim3(nparts), dim3(LT), 0, st, values_dev,
-                                  negative_dev, initial_dev, n, idx_begin, (ff_partial*)workspace_dev));
+    first_fail_partial_kernel<<<nparts, LT, 0, st>>>(values_dev, negative_dev, initial_dev, n, idx_begin,
+                                                     (ff_partial*)workspace_dev);
     SLB_LAUNCH_CHECK();
-    SLB_CUDA(slb_launch_dependent(first_fail_final_kernel, dim3(1), dim3(FF_BLOCKS), 0, st,
-                                  (const ff_partial*)workspace_dev, nparts, result_dev, *xchg));
+    first_fail_final_kernel<<<1, FF_BLOCKS, 0, st>>>((const ff_partial*)workspace_dev, nparts, result_dev,
+                                                     *xchg);
     SLB_LAUNCH_CHECK();
     return 0;
 }
@@ -836,11 +831,11 @@ int slb_apply_prefix_x(void* stream, const double* values_dev, const uint8_t* in
     const int64_t want = (n + LT - 1) / LT;
     const unsigned blocks = (unsigned)(want > 2048 ? 2048 : (want < 1 ? 1 : want));
     if (xchg->world > 1)
-        SLB_CUDA(slb_launch_dependent(apply_prefix_kernel<true>, dim3(blocks), dim3(LT), 0, st, values_dev,
-                                      initial_dev, n, idx_begin, key_out_dev, safe_dev, stats_dev, *xchg));
+        apply_prefix_kernel<true><<<blocks, LT, 0, st>>>(values_dev, initial_dev, n, idx_begin, key_out_dev,
+                                                         safe_dev, stats_dev, *xchg);
     else
-        SLB_CUDA(slb_launch_dependent(apply_prefix_kernel<false>, dim3(blocks), dim3(LT), 0, st, values_dev,
-                                      initial_dev, n, idx_begin, key_out_dev, safe_dev, stats_dev, *xchg));
+        apply_prefix_kernel<false><<<blocks, LT, 0, st>>>(values_dev, initial_dev, n, idx_begin, key_out_dev,
+                                                          safe_dev, stats_dev, *xchg);
     SLB_LAUNCH_CHECK();
     return 0;
 }
@@ -867,9 +862,9 @@ int slb_apply_prefix(void* stream, const double* values_dev, const uint8_t* init
     const unsigned blocks = (unsigned)(want > 2048 ? 2048 : want);
     slb_exchange none;
     memset(&none, 0, sizeof(none));
-    SLB_CUDA(slb_launch_dependent(apply_prefix_kernel<false>, dim3(blocks), dim3(LT), 0, st, values_dev,
-                                  initial_dev, n, idx_begin, const_cast<slb_fail_key*>(key_dev), safe_dev,
-                                  stats_dev, none));
+    apply_prefix_kernel<false><<<blocks, LT, 0, st>>>(values_dev, initial_dev, n, idx_begin,
+                                                      const_cast<slb_fail_key*>(key_dev), safe_dev, stats_dev,
+                                                      none);
     SLB_LAUNCH_CHECK();
     return 0;
 }

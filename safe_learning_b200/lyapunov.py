@@ -13,7 +13,6 @@ inside the reduction kernels (``slb_exchange``), without a collective call or a 
 
 from __future__ import annotations
 
-import os
 import zlib
 
 import numpy as np
@@ -125,13 +124,6 @@ def get_safe_sample(lyapunov, perturbations=None, limits=None, positive=False, n
         return state_actions[[max_id]], bound[max_id].squeeze()
     max_id = int(np.argmax(bound_safe))
     return state_actions[maps_inside, :][[max_id]], bound_safe[max_id].squeeze()
-
-
-# CUDA-graph replay of the launches of a sweep (memsets + 8 kernels) while nothing they depend on
-# changes: the second sweep with an unchanged descriptor is captured, later ones replay it.  It saves
-# device time between the launches and the host enqueue time per sweep, which is what bounds the
-# end-to-end step.  SLB200_GRAPHS=0 switches it off.
-_USE_GRAPHS = os.environ.get("SLB200_GRAPHS", "1") == "1"
 
 
 class _CMax(object):
@@ -296,7 +288,7 @@ class Lyapunov(object):
         self.c_max = _CMax()
         dict.__setitem__(self.feed_dict, self.c_max, 0.)
         # decision filter in front of the O(M^2) posterior: "auto" (on when every GP's certified
-        # variance floor is far above fp64 rounding), True, or False; SLB200_FILTER=0 disables it
+        # variance floor is far above fp64 rounding), True, or False
         self.filter = "auto"
         self.refinement_mode = "mesh"     # or "reference": lyapunov.py:474-478 as written
 
@@ -613,8 +605,6 @@ class Lyapunov(object):
         """Whether the sweep goes through the decision filter (csrc/filter.cu)."""
         if cfg.gp.num_outputs == 0 or self.filter is False:
             return False
-        if os.environ.get("SLB200_FILTER", "1") == "0":
-            return False
         if self.filter == "auto":
             return self.dynamics.variance_floor() >= 1e-9
         return True
@@ -829,10 +819,13 @@ class Lyapunov(object):
                                            self._safe_dev.data_ptr(), self._workspace.data_ptr(),
                                            self._stats_dev.data_ptr()), "slb_apply_prefix")
 
-        # Optional CUDA-graph replay of the launches of a sweep (no collective call inside when
-        # the keys travel through peer memory), while nothing they depend on has changed.
+        # CUDA-graph replay of the launches of a sweep (memsets + 8 kernels; no collective call
+        # inside when the keys travel through peer memory) while nothing they depend on changes:
+        # the second sweep with an unchanged descriptor is captured, later ones replay it.  It saves
+        # device time between the launches and the host enqueue time per sweep, which is what
+        # bounds the end-to-end step.
         token = None
-        if (_USE_GRAPHS and not adaptive and not self._is_composed()
+        if (not adaptive and not self._is_composed()
                 and (world == 1 or xchg is not None)):
             token = (self._descriptor_token(), self._values_dev.data_ptr(),
                      0 if initial is None else initial.data_ptr(), n_local,

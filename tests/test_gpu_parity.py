@@ -399,8 +399,7 @@ def test_screening_mean_error_is_within_its_certified_bound(sl, case):
     assert_array_equal(fast, gpu.compute_negative().cpu().numpy())
 
 
-@pytest.mark.parametrize("split,label", [((0, 0), "64-point tiles"), ((0, 1 << 40), "32-point tiles"),
-                                         ((1 << 40, 1 << 40), "16-point tiles")])
+@pytest.mark.parametrize("split,label", [((0,), "64-point tiles"), ((1 << 40,), "32-point tiles")])
 def test_refine_pass_tile_sizes(sl, split, label):
     """The refine pass of the filtered sweep picks its tile size from the list length; every tile
     size (forced through slb_debug_refine_split) must reproduce the full posterior's flags, with
@@ -418,7 +417,7 @@ def test_refine_pass_tile_sizes(sl, split, label):
             gpu.filter = False
             assert_array_equal(fast, gpu.compute_negative().cpu().numpy(), err_msg=label)
     finally:
-        lib.slb_debug_refine_split(0, 32 * 132)        # the library's default split
+        lib.slb_debug_refine_split(32 * 132)           # the library's default split
 
 
 def test_pivoted_head_subset_matches_greedy_selection(sl):

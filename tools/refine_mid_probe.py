@@ -1,5 +1,5 @@
 """Refine pass on mid-size lists (between ~600 and 4736 points: fewer spare CTAs per 32-point tile): stage time
-of the refine pass for a few discretisation constants of the C2 workload.  Run with SLB200_SPLIT_FACTORS=1 / 2."""
+of the refine pass for a few discretisation constants of the C2 workload."""
 import json, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
