@@ -452,6 +452,40 @@ int slb_reward_rollout(void* stream, const slb_bellman* cfg, const double* state
                        int64_t n, int32_t horizon, const double* discount_dev, double tol,
                        double* sums_dev, int64_t* stop_dev, void* workspace_dev);
 
+/* ---- exact policy evaluation (reinforcement_learning.py:142-211 optimize_value_function): the
+ *      fixed point of  v = r + gamma T v,  T = the value Triangulation's barycentric rows at the mean
+ *      next states (DESIGN.md §3.9).  Row i of T: cols_dev[i * (d + 1) + j] (int32, or int64 when the
+ *      value grid has more than 2^31 - 1 vertices), weights_dev[i * (d + 1) + j] (fp64), d = the
+ *      value grid's dimension.  stats_dev: SLB_VALUE_STATS uint64 slots:
+ *        [0] ~key(min weight)  (order-preserving key of the smallest weight, complemented)
+ *        [1] rho = max_i sum_j |w_ij|, fp64 bits     [2] rows re-searched (grid-line lookups, Q6)
+ *        [3] rows with a NaN next state / reward     [4] iterations   [5] last ||dv||_inf, fp64 bits
+ *        [6] certified bound, fp64 bits              [7] status (SLB_VALUE_*)   [8] solver tier (1, 2)
+ *      The assembly entry points write [0..3]; slb_value_solve writes [0, 1] and [4..8]. ---------- */
+#define SLB_VALUE_STATS 16
+#define SLB_VALUE_CONVERGED 0
+#define SLB_VALUE_MAX_ITERS 1
+#define SLB_VALUE_NEGATIVE_WEIGHT 2
+#define SLB_VALUE_NOT_CONTRACTIVE 3
+#define SLB_VALUE_NAN 4
+/* fused assembly for flat indices [idx_begin, idx_end): u = policy(x), x+ = mean dynamics(x, u)
+ * (deterministic function or GP stack), rewards_dev[i] = reward(x, u); cfg->value is a one-output
+ * Triangulation; fixed_action must be 0 */
+int slb_value_operator(void* stream, const slb_bellman* cfg, int64_t idx_begin, int64_t idx_end,
+                       void* cols_dev, double* weights_dev, double* rewards_dev, uint64_t* stats_dev);
+/* composed assembly: the rows of next_states_dev [n, d] */
+int slb_value_operator_points(void* stream, const slb_function* value, const double* next_states_dev,
+                              int64_t n, void* cols_dev, double* weights_dev, uint64_t* stats_dev);
+/* bytes of workspace slb_value_solve needs: 0 when n <= 12288 (one-CTA tier), else n doubles + 128 */
+int64_t slb_value_solve_workspace(int64_t n, int32_t ncols);
+/* iterate v <- r + gamma T v from v_inout_dev [n] until gamma rho / (1 - gamma rho) ||dv||_inf <=
+ * tol max(1, ||v||_inf), then write v to v_inout_dev.  The status (stats slot 7) says why it stopped;
+ * v_inout_dev is left unchanged when the operator has a weight < -1e-12, gamma rho >= 1, or a NaN in a
+ * weight, a reward or v_inout_dev itself. */
+int slb_value_solve(void* stream, int64_t n, int32_t ncols, const void* cols_dev, const double* weights_dev,
+                    const double* rewards_dev, double gamma, double tol, int64_t max_iters,
+                    double* v_inout_dev, void* workspace_dev, uint64_t* stats_dev);
+
 #ifdef __cplusplus
 }
 #endif

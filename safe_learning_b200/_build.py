@@ -23,9 +23,11 @@ UNITS = [("gp_tile_%d_%d.o" % (d, tp), "gp_tile_inst.cu", ["-DSLB_TILE_DIN=%d" %
           ["gp_tile.cuh", "gp_args.h"]) for d in range(1, 7) for tp in (64, 32)]
 UNITS += [("gp_sweep.o", "gp_sweep.cu", [], ["gp_args.h"]),
           ("filter.o", "filter.cu", [], ["bulk_copy.cuh", "exp2_tab512.cuh", "gp_mean_staged.cuh", "gp_args.h"]),
-          ("light.o", "light.cu", [], ["bulk_copy.cuh", "exp2_tab512.cuh", "gp_mean_staged.cuh"]),
+          ("light.o", "light.cu", [], ["bulk_copy.cuh", "exp2_tab512.cuh", "gp_mean_staged.cuh", "bellman.cuh"]),
           ("bellman_tile.o", "bellman_tile.cu", [], []),
-          ("rollout.o", "rollout.cu", [], [])]
+          ("rollout.o", "rollout.cu", [], []),
+          ("value_opt.o", "value_opt.cu", [], ["bulk_copy.cuh", "exp2_tab512.cuh", "gp_mean_staged.cuh",
+                                               "bellman.cuh"])]
 SOURCES = sorted({u[1] for u in UNITS})
 
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]

@@ -26,6 +26,9 @@ FLAG_SATURATE, FLAG_ABS, FLAG_NORM1, FLAG_PROJECT, FLAG_SCALE, FLAG_GRADIENT, FL
 K_RBF, K_MATERN12, K_MATERN32, K_MATERN52, K_LINEAR, K_CONSTANT, K_WHITE = range(7)
 SLB_MAX_KPRIM = 6
 ABI_VERSION = 6
+# slb_value_solve: stats slots and status codes (include/slb200.h)
+VALUE_STATS = 16
+VALUE_CONVERGED, VALUE_MAX_ITERS, VALUE_NEGATIVE_WEIGHT, VALUE_NOT_CONTRACTIVE, VALUE_NAN = range(5)
 
 UINT64_MAX = (1 << 64) - 1
 INT64_MAX = (1 << 63) - 1
@@ -165,6 +168,11 @@ SIGNATURES = {
                               _vp, _dp, _dp, _vp]),
     "slb_reward_rollout": (C.c_int, [_vp, C.POINTER(SlbBellman), _dp, _i64, _i64, _i32, _dp,
                                      C.c_double, _dp, _vp, _vp]),
+    "slb_value_operator": (C.c_int, [_vp, C.POINTER(SlbBellman), _i64, _i64, _vp, _dp, _dp, _vp]),
+    "slb_value_operator_points": (C.c_int, [_vp, C.POINTER(SlbFunction), _dp, _i64, _vp, _dp, _vp]),
+    "slb_value_solve_workspace": (C.c_int64, [_i64, _i32]),
+    "slb_value_solve": (C.c_int, [_vp, _i64, _i32, _vp, _dp, _dp, C.c_double, C.c_double, _i64, _dp,
+                                  _vp, _vp]),
 }
 
 _lib = None

@@ -318,6 +318,115 @@ SLB_DEV double fmod_exact_pos(double a, double b) {
 }
 
 // ---- Triangulation (functions.py:1103-1158 lookup, :1473-1499 evaluation) ----------------
+// Simplex of the unit cell for unit coordinates `unit`: the first simplex whose barycentric weights
+// are all >= -tol, else the one with the largest smallest weight.  `skip`: return `best` unsearched.
+SLB_DEV int tri_find_simplex(const slb_function& f, const double* unit, int best = 0, bool skip = false) {
+    const slb_grid& g = f.grid;
+    const int d = g.ndim;
+    double best_min = -1e300;
+    for (int s = 0; s < f.nsimplex && !skip; ++s) {
+        const int64_t v0 = f.unit_simplices[s * (d + 1)];
+        double o[SLB_MAX_DIM];
+        if (g.nindex <= 0x7fffffffll) {        // 32-bit index arithmetic (same integers)
+            unsigned t = (unsigned)v0;
+            for (int c = d - 1; c >= 0; --c) {
+                const unsigned n = (unsigned)g.num_points[c];
+                const unsigned qq = t / n;
+                o[c] = (double)(t - qq * n) * g.unit_maxes[c];
+                t = qq;
+            }
+        } else {
+            int64_t t = v0;
+            for (int c = d - 1; c >= 0; --c) {
+                o[c] = (double)(t % g.num_points[c]) * g.unit_maxes[c];
+                t /= g.num_points[c];
+            }
+        }
+        const double* H = f.hyperplanes + (size_t)s * d * d;
+        double wsum = 0.0, wmin = 1e300;
+        for (int c = 0; c < d; ++c) {
+            double w = 0.0;
+            for (int k = 0; k < d; ++k) w += (unit[k] - o[k]) * H[k * d + c];
+            wsum += w;
+            wmin = fmin(wmin, w);
+        }
+        wmin = fmin(wmin, 1.0 - wsum);
+        if (wmin > best_min) { best_min = wmin; best = s; }
+        if (wmin >= -1e-12) break;
+    }
+    return best;
+}
+
+// Barycentric weights w[0..d] of the point xin (clipped to the limits when projected) in simplex
+// `s` of the rectangle whose lowest vertex is `corner`   (:1479-1491)
+SLB_DEV void tri_barycentric(const slb_function& f, const double* xin, int64_t corner, int s,
+                             double* w) {
+    const slb_grid& g = f.grid;
+    const int d = g.ndim;
+    const int64_t* simp = f.unit_simplices + (size_t)s * (d + 1);
+    const double* H = f.hyperplanes + (size_t)s * d * d;
+    double origin[SLB_MAX_DIM], off[SLB_MAX_DIM];
+    grid_index_to_state(g, simp[0] + corner, origin);
+    for (int c = 0; c < d; ++c) {
+        double xc = xin[c];
+        if (f.flags & SLB_FLAG_PROJECT) xc = fmin(fmax(xc, g.offset[c]), g.upper[c]);
+        off[c] = f64sub(xc, origin[c]);
+    }
+    for (int c = 0; c < d; ++c) {
+        double acc = f64mul(off[0], H[c]);
+        for (int k = 1; k < d; ++k) acc = f64add(acc, f64mul(off[k], H[k * d + c]));
+        w[c + 1] = acc;
+    }
+    double acc = w[1];
+    for (int c = 2; c <= d; ++c) acc = f64add(acc, w[c]);
+    w[0] = f64sub(1.0, acc);
+}
+
+// The reference's lookup of xin: rectangle (lowest vertex -> *corner_out), simplex (returned) and
+// barycentric weights w[0..d] -- eval_triangulation's lookup operation for operation.  The value
+// operator (value_opt.cu) builds its rows from it; eval_triangulation keeps its own inline copy
+// because routing it through these helpers changes register allocation (and adds spills) in the
+// filter, argmax-tile and rollout kernels that inline it.
+SLB_DEV int tri_locate(const slb_function& f, const double* xin, int64_t* corner_out, double* w) {
+    const slb_grid& g = f.grid;
+    const int d = g.ndim;
+    const double eps = 2.220446049250313e-16;
+    double unit[SLB_MAX_DIM];
+    int64_t corner = 0;
+    int poff = 0;
+    int pattern = 0;
+    bool all_clipped = true;
+    for (int c = 0; c < d; ++c) {
+        const double* pts = g.discrete_points + poff;
+        const int n = (int)g.num_points[c];
+        poff += n;
+        const double xc = xin[c];
+        // np.digitize(x, pts) - 1 clipped to [0, n-2]   (functions.py:771-773)
+        int k = (int)floor((xc - g.offset[c]) / g.unit_maxes[c]);
+        k = k < 0 ? 0 : (k > n - 1 ? n - 1 : k);
+        while (k + 1 <= n - 1 && pts[k + 1] <= xc) ++k;
+        while (k >= 0 && pts[k] > xc) --k;            // k = -1 when x < pts[0]
+        k = k < 0 ? 0 : (k > n - 2 ? n - 2 : k);
+        corner = corner * g.num_points[c] + k;        // rectangle_corner_index (:800-817)
+        // _center_states(clip=True) % unit_maxes          (:691-712, :1120-1123)
+        double cen = f64sub(xc, g.offset[c]);
+        const double lo = 2.0 * eps;
+        const double hi = f64sub(f64sub(g.upper[c], g.offset[c]), 2.0 * eps);
+        if (cen < lo) cen = lo;
+        else if (cen > hi) { cen = hi; pattern |= 1 << c; }
+        else all_clipped = false;
+        unit[c] = fmod_exact_pos(cen, g.unit_maxes[c]);
+    }
+    // simplex inside the unit cell; weights with the ORIGINAL (optionally projected) point
+    const bool tabled = all_clipped && f.corner_simplex != nullptr;
+    const int best = tri_find_simplex(f, unit, tabled ? f.corner_simplex[pattern] : 0, tabled);
+    *corner_out = corner;
+    tri_barycentric(f, xin, corner, best, w);
+    return best;
+}
+
+// The lookup below is restated, operation for operation, by tri_locate / tri_find_simplex /
+// tri_barycentric above (used by the value operator); a change here must be made there too.
 SLB_DEV void eval_triangulation(const slb_function& f, const double* xin, double* out) {
     const slb_grid& g = f.grid;
     const int d = g.ndim;

@@ -5,7 +5,7 @@
 //   GridWorld.index_to_state                    functions.py:714-731
 //   Bellman sweep / argmax / max|dV|            reinforcement_learning.py:65-114,135-140,213-279
 #include "common.cuh"
-#include "gp_mean_staged.cuh"
+#include "bellman.cuh"
 
 #include <stdarg.h>
 #include <stdio.h>
@@ -155,6 +155,45 @@ int slb_validate_gp(const slb_gp_stack* gp) {
         SLB_CHECK(G.factor >= 0 && G.factor < gp->num_factors, "GP output %d: bad factor index", o);
         SLB_CHECK(G.alpha != nullptr, "GP output %d: null alpha", o);
     }
+    return 0;
+}
+
+int slb_validate_bellman(const slb_bellman* cfg, int* m_out) {
+    SLB_CHECK(cfg != nullptr, "bellman: null config");
+    if (slb_validate_grid(&cfg->grid, false)) return 1;
+    const int d = cfg->grid.ndim;
+    int m;
+    if (cfg->fixed_action) {
+        m = cfg->policy.out_dim;
+        SLB_CHECK(m >= 1 && m <= SLB_MAX_ACT, "bellman: fixed action dim %d unsupported", m);
+    } else {
+        if (slb_validate_function(&cfg->policy, "policy", d)) return 1;
+        SLB_CHECK(cfg->policy.kind != SLB_FN_NONE, "bellman: a policy is required");
+        m = cfg->policy.out_dim;
+        SLB_CHECK(m >= 1 && m <= SLB_MAX_ACT, "bellman: policy output dim %d unsupported", m);
+    }
+    if (cfg->gp.num_outputs > 0) {
+        if (slb_validate_gp(&cfg->gp)) return 1;
+        SLB_CHECK(cfg->gp.num_outputs == d && cfg->gp.input_dim == d + m,
+                  "bellman: GP stack shape (%d outputs, %d inputs) does not match state %d + action %d",
+                  cfg->gp.num_outputs, cfg->gp.input_dim, d, m);
+        for (int o = 0; o < cfg->gp.num_outputs; ++o) {
+            const slb_gp_output& G = cfg->gp.outputs[o];
+            const slb_gp_factor& F = cfg->gp.factors[G.factor];
+            SLB_CHECK(F.M == 0 || (G.gamma_f != nullptr && F.Xf != nullptr &&
+                                   (reinterpret_cast<uintptr_t>(G.gamma_f) & 15) == 0 &&
+                                   (reinterpret_cast<uintptr_t>(F.Xf) & 15) == 0),
+                      "bellman: GP output %d lacks the (16-byte aligned) staged tables Xf / gamma_f", o);
+        }
+    } else {
+        if (slb_validate_function(&cfg->dynamics, "dynamics", d + m)) return 1;
+        SLB_CHECK(cfg->dynamics.kind != SLB_FN_NONE, "bellman: no dynamics given");
+    }
+    if (slb_validate_function(&cfg->reward, "reward_function", d + m)) return 1;
+    SLB_CHECK(cfg->reward.kind != SLB_FN_NONE, "bellman: a reward function is required");
+    if (slb_validate_function(&cfg->value, "value_function", d)) return 1;
+    SLB_CHECK(cfg->value.kind != SLB_FN_NONE, "bellman: a value function is required");
+    *m_out = m;
     return 0;
 }
 
@@ -526,42 +565,7 @@ apply_prefix_kernel(const double* __restrict__ values, const uint8_t* __restrict
     }
 }
 
-// ---- Bellman sweep ------------------------------------------------------------------------
-// The mean-only GP runs on the staged pipeline of gp_mean_staged.cuh (training rows and gamma streamed
-// through shared memory by TMA bulk copies, expanded squared distance, the <= 1 ulp table exp).
-struct bellman_smem {
-    mean_pipe P;
-    double* tab512;
-    double* tab64;
-};
-
-template <int DIN>
-SLB_DEV void bellman_setup(bellman_smem& S, unsigned char* smem_raw, const slb_bellman& cfg,
-                           int chunk_rows, int nomax) {
-    mean_pipe_setup(S.P, smem_raw, DIN, chunk_rows, nomax, cfg.gp, &S.tab512, &S.tab64);
-    if (threadIdx.x == 0) mean_pipe_init(S.P, S.tab512);
-    __syncthreads();
-    slb_bulk::mbar_wait(S.P.bar + 2, 0);                       // exp tables have landed
-}
-
-template <int DIN>
-SLB_DEV double bellman_value(const slb_bellman& cfg, const double* x, const double* u, int m,
-                             bellman_smem& S) {
-    const int d = cfg.grid.ndim;
-    double z[SLB_MAX_IN], mu[SLB_MAX_OUT], err[SLB_MAX_OUT], r[SLB_MAX_OUT], v[SLB_MAX_OUT];
-    for (int c = 0; c < d; ++c) z[c] = x[c];
-    for (int c = 0; c < m; ++c) z[d + c] = u[c];
-    if (cfg.gp.num_outputs > 0) {
-        mean_pipe_start<DIN>(cfg.gp, S.P);
-        gp_mean_staged<DIN, false>(cfg.gp, z, mu, err, S.tab512, S.tab64, S.P);
-    } else {
-        eval_fn(cfg.dynamics, z, mu);
-    }
-    eval_fn(cfg.reward, z, r);                               // :95
-    eval_fn(cfg.value, mu, v);                               // :101
-    return f64add(r[0], f64mul(cfg.gamma, v[0]));                // :104
-}
-
+// ---- Bellman sweep (bellman.cuh) ----------------------------------------------------------
 template <int DIN>
 __global__ void __launch_bounds__(LT, 2)
 bellman_kernel(const __grid_constant__ slb_bellman cfg, int64_t idx_begin, int64_t n,
@@ -901,62 +905,10 @@ int slb_index_to_state(void* stream, const slb_grid* grid, int64_t idx_begin, in
     return 0;
 }
 
-// slice size and dynamic shared memory of the Bellman kernels' mean pipeline (< 48 KB: no opt-in)
-static size_t bellman_stage_config(const slb_bellman& cfg, int din, int* chunk_rows, int* nomax) {
-    int most = 1;
-    for (int f = 0; f < cfg.gp.num_factors; ++f) {
-        int no = 0;
-        for (int o = 0; o < cfg.gp.num_outputs; ++o) no += cfg.gp.outputs[o].factor == f;
-        if (no > most) most = no;
-    }
-    *nomax = most;
-    *chunk_rows = mean_chunk_rows(din, most, 24);
-    return mean_smem_bytes(din, most, *chunk_rows);
-}
-
-static int validate_bellman(const slb_bellman* cfg, int* m_out) {
-    SLB_CHECK(cfg != nullptr, "bellman: null config");
-    if (slb_validate_grid(&cfg->grid, false)) return 1;
-    const int d = cfg->grid.ndim;
-    int m;
-    if (cfg->fixed_action) {
-        m = cfg->policy.out_dim;
-        SLB_CHECK(m >= 1 && m <= SLB_MAX_ACT, "bellman: fixed action dim %d unsupported", m);
-    } else {
-        if (slb_validate_function(&cfg->policy, "policy", d)) return 1;
-        SLB_CHECK(cfg->policy.kind != SLB_FN_NONE, "bellman: a policy is required");
-        m = cfg->policy.out_dim;
-        SLB_CHECK(m >= 1 && m <= SLB_MAX_ACT, "bellman: policy output dim %d unsupported", m);
-    }
-    if (cfg->gp.num_outputs > 0) {
-        if (slb_validate_gp(&cfg->gp)) return 1;
-        SLB_CHECK(cfg->gp.num_outputs == d && cfg->gp.input_dim == d + m,
-                  "bellman: GP stack shape (%d outputs, %d inputs) does not match state %d + action %d",
-                  cfg->gp.num_outputs, cfg->gp.input_dim, d, m);
-        for (int o = 0; o < cfg->gp.num_outputs; ++o) {
-            const slb_gp_output& G = cfg->gp.outputs[o];
-            const slb_gp_factor& F = cfg->gp.factors[G.factor];
-            SLB_CHECK(F.M == 0 || (G.gamma_f != nullptr && F.Xf != nullptr &&
-                                   (reinterpret_cast<uintptr_t>(G.gamma_f) & 15) == 0 &&
-                                   (reinterpret_cast<uintptr_t>(F.Xf) & 15) == 0),
-                      "bellman: GP output %d lacks the (16-byte aligned) staged tables Xf / gamma_f", o);
-        }
-    } else {
-        if (slb_validate_function(&cfg->dynamics, "dynamics", d + m)) return 1;
-        SLB_CHECK(cfg->dynamics.kind != SLB_FN_NONE, "bellman: no dynamics given");
-    }
-    if (slb_validate_function(&cfg->reward, "reward_function", d + m)) return 1;
-    SLB_CHECK(cfg->reward.kind != SLB_FN_NONE, "bellman: a reward function is required");
-    if (slb_validate_function(&cfg->value, "value_function", d)) return 1;
-    SLB_CHECK(cfg->value.kind != SLB_FN_NONE, "bellman: a value function is required");
-    *m_out = m;
-    return 0;
-}
-
 int slb_bellman_sweep(void* stream, const slb_bellman* cfg, int64_t idx_begin, int64_t idx_end,
                       double* out_dev) {
     int m;
-    if (validate_bellman(cfg, &m)) return 1;
+    if (slb_validate_bellman(cfg, &m)) return 1;
     SLB_CHECK(idx_begin >= 0 && idx_end >= idx_begin && idx_end <= cfg->grid.nindex,
               "slb_bellman_sweep: range outside the grid");
     const int64_t n = idx_end - idx_begin;
@@ -995,7 +947,7 @@ int slb_bellman_argmax(void* stream, const slb_bellman* cfg, int64_t idx_begin, 
                        int32_t* best_dev, double* best_value_dev, void* workspace_dev) {
     SLB_CHECK(cfg != nullptr && cfg->fixed_action, "slb_bellman_argmax: cfg.fixed_action must be set");
     int m;
-    if (validate_bellman(cfg, &m)) return 1;
+    if (slb_validate_bellman(cfg, &m)) return 1;
     SLB_CHECK(n_actions >= 1 && actions_dev != nullptr, "slb_bellman_argmax: no actions");
     SLB_CHECK(idx_begin >= 0 && idx_end >= idx_begin && idx_end <= cfg->grid.nindex,
               "slb_bellman_argmax: range outside the grid");

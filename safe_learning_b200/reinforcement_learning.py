@@ -3,8 +3,10 @@
 ``value_iteration`` and ``discrete_policy_optimization`` run as fused CUDA sweeps over the
 value function's grid (``slb_bellman_sweep`` / ``slb_bellman_argmax``); ``future_values`` on
 arbitrary state arrays is composed from the eager GPU evaluations of the function objects.
-LP value optimisation (``:142-211``, cvxpy) and ``bellmann_error`` (``:116-133``, autodiff)
-are outside this build's hot path.
+``optimize_value_function`` (``:142-211``) solves the reference's LP as what it is for a
+policy, exact policy evaluation: the fixed point of ``v = r + gamma T v``, assembled and iterated
+to a certified error bound on the GPU (``csrc/value_opt.cu``, DESIGN.md §3.9).
+``bellmann_error`` (``:116-133``, autodiff) is outside this build's hot path.
 """
 
 from __future__ import annotations
@@ -22,6 +24,22 @@ __all__ = ["PolicyIteration", "OptimizationError"]
 
 class OptimizationError(Exception):
     """``reinforcement_learning.py:22-23``."""
+
+
+# cvxpy options of the reference's call (``prob.solve(**solver_options)``) that have no meaning for
+# the fixed-point solve; accepted so that notebook calls run unchanged
+_IGNORED_SOLVER_OPTIONS = ("solver", "verbose", "eps", "warm_start")
+
+
+def _fusable(fn):
+    """True when ``fn`` has a descriptor the CUDA kernels can evaluate."""
+    if not isinstance(fn, Function) or isinstance(fn, UncertainFunction):
+        return False
+    try:
+        fn.descriptor()
+    except (NotImplementedError, TypeError, ValueError):
+        return False
+    return True
 
 
 def _triangulation_of(value_function):
@@ -217,3 +235,108 @@ class PolicyIteration(object):
         full = self._gather(chosen[:, 0].contiguous()).reshape(-1, 1) if m == 1 else chosen
         policy_tri.parameters = full
         return full
+
+    # ------------------------------------------------------------------ exact policy evaluation
+    def optimize_value_function(self, **solver_options):
+        """Evaluate the current policy exactly (``:180-211``) and store the values in the value
+        function; returns them as a numpy array ``[N, 1]``.
+
+        The reference maximises ``sum(v)`` subject to ``v <= r + gamma T v`` with cvxpy, T the value
+        Triangulation's barycentric rows at the mean next states.  For nonnegative rows and
+        ``gamma < 1`` the optimum is the fixed point ``v = r + gamma T v``; it is computed here by
+        iterating that map from the current values until the certified error
+        ``gamma rho / (1 - gamma rho) ||v_k - v_{k-1}||_inf`` is at most ``tol * max(1, ||v||_inf)``.
+
+        Options: ``tol`` (1e-10) and ``max_iters`` (200000); the cvxpy options ``solver``,
+        ``verbose``, ``eps`` and ``warm_start`` are accepted and ignored.  ``last_solve`` holds
+        ``iterations``, ``bound``, ``rho``, ``repaired_rows`` and ``tier`` of the call.
+
+        Raises ``OptimizationError`` when a row extrapolates (a weight < -1e-12: an unprojected
+        next state outside the grid), when ``gamma * rho >= 1``, when a reward, a next state or a
+        value of the current table (the start point) is NaN,
+        or when ``max_iters`` iterations do not reach the bound; ``TypeError`` when the value
+        function is not a plain one-output ``Triangulation``.  Next states on a grid line are looked
+        up in the simplex that contains them (DESIGN.md §3.2 Q6; the reference's lookup can pick a
+        simplex of the wrong side of the cell there, which makes its LP unbounded).
+        """
+        tol = float(solver_options.pop("tol", 1e-10))
+        max_iters = int(solver_options.pop("max_iters", 200000))
+        unknown = set(solver_options) - set(_IGNORED_SOLVER_OPTIONS)
+        if unknown:
+            raise TypeError("optimize_value_function got unexpected options %s" % sorted(unknown))
+        if not 0.0 <= self.gamma < 1.0:
+            raise OptimizationError("Optimization problem is not a contraction: gamma = %r is "
+                                    "outside [0, 1)" % (self.gamma,))
+        values, stats = self._evaluate_policy(tol, max_iters)
+        status = stats["status"]
+        if status == nat.VALUE_NEGATIVE_WEIGHT:
+            raise OptimizationError("Optimization problem is unbounded: the value function "
+                                    "extrapolates (smallest interpolation weight %.3g); use a "
+                                    "projected Triangulation" % stats["min_weight"])
+        if status == nat.VALUE_NOT_CONTRACTIVE:
+            raise OptimizationError("Optimization problem is not a contraction: gamma * rho = %.17g "
+                                    ">= 1" % (self.gamma * stats["rho"]))
+        if status == nat.VALUE_NAN:
+            raise OptimizationError("Optimization problem is infeasible: NaN in the rewards, the "
+                                    "next states or the value function's current table")
+        if status == nat.VALUE_MAX_ITERS:
+            raise OptimizationError("Optimization problem is not solved after %d iterations "
+                                    "(certified error %.3g)" % (stats["iterations"], stats["bound"]))
+        return values
+
+    def _evaluate_policy(self, tol, max_iters):
+        """Assemble the operator and iterate; the table is replaced when the iteration converged.
+        Returns (the last iterate [N, 1] numpy, statistics); the statistics come back with the
+        values in one device-to-host copy."""
+        lib = nat.load()
+        tri = self.value_function
+        if type(tri) is not Triangulation:
+            raise TypeError("optimize_value_function needs a plain Triangulation value function "
+                            "(the reference reaches value_function.tri), got %s" % type(tri).__name__)
+        if tri._param_dev is None or tri._param_dev.shape[1] != 1:
+            raise TypeError("optimize_value_function needs a one-output Triangulation")
+        n, d = self._grid.nindex, self._grid.ndim
+        ncols = d + 1
+        idx = torch.int64 if n > 0x7fffffff else torch.int32
+        cols = dev.empty((n, ncols), idx)
+        weights = dev.empty((n, ncols))
+        stats = dev.zeros((nat.VALUE_STATS,), torch.int64)
+        if all(_fusable(f) for f in (self.policy, self.reward_function)) and (
+                isinstance(self.dynamics, (FunctionStack, GaussianProcess)) or _fusable(self.dynamics)):
+            # every rank assembles and solves the whole system: no collective, identical tables
+            rewards = dev.empty((n,))
+            nat.check(lib.slb_value_operator(dev.stream(), self.bellman_descriptor(), 0, n,
+                                             cols.data_ptr(), weights.data_ptr(), rewards.data_ptr(),
+                                             stats.data_ptr()), "slb_value_operator")
+        else:                                                                 # :197-205 on the host
+            states = self.state_space
+            actions = self.policy(states)
+            next_states = self.dynamics(states, actions)
+            if isinstance(next_states, tuple):
+                next_states = next_states[0]
+            rewards = dev.to_device(np.asarray(self.reward_function(states, actions),
+                                               dtype=np.float64).reshape(n))
+            nxt = dev.to_device(np.asarray(next_states, dtype=np.float64).reshape(n, d))
+            nat.check(lib.slb_value_operator_points(dev.stream(), tri.descriptor(), nxt.data_ptr(), n,
+                                                    cols.data_ptr(), weights.data_ptr(),
+                                                    stats.data_ptr()), "slb_value_operator_points")
+        values = tri._param_dev.reshape(-1).clone()                           # warm start
+        need = int(lib.slb_value_solve_workspace(n, ncols))
+        work = dev.empty((need // 8,)) if need else None
+        nat.check(lib.slb_value_solve(dev.stream(), n, ncols, cols.data_ptr(), weights.data_ptr(),
+                                      rewards.data_ptr(), float(self.gamma), tol, max_iters,
+                                      values.data_ptr(), dev.ptr(work), stats.data_ptr()),
+                  "slb_value_solve")
+        host = torch.cat((values, stats.view(torch.float64))).cpu().numpy()  # the one sync
+        raw = host[n:].view(np.uint64)
+        key = ~raw[0]                                      # order-preserving key of the min weight
+        min_weight = (key & np.uint64(0x7fffffffffffffff)) if key >> np.uint64(63) else ~key
+        info = {"status": int(raw[7]), "iterations": int(raw[4]),
+                "delta": float(host[n + 5]), "bound": float(host[n + 6]),
+                "rho": float(host[n + 1]), "repaired_rows": int(raw[2]), "tier": int(raw[8]),
+                "min_weight": float(np.array([min_weight], dtype=np.uint64).view(np.float64)[0])}
+        self.last_solve = info
+        out = host[:n].reshape(n, 1).copy()
+        if info["status"] == nat.VALUE_CONVERGED:
+            tri._param_dev = values.reshape(-1, 1)
+        return out, info

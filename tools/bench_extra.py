@@ -12,8 +12,13 @@
             pendulum 101^2 with trajectories, cart-pole 51^4 (horizon 2000)
   reward_rollout  reward_rollout of the pendulum loop on 2001x1501 (discount 0.95, horizon 1000,
             tol 1e-2), reporting the stopping step T*
+  value_opt PolicyIteration.optimize_value_function (gamma 0.98, tol 1e-10) with RBF GP-mean dynamics
+            (bench_workloads.make_pendulum) on 55x55 (M=50, the one-CTA solver) and on C3's 512x512
+            (M=500, the cooperative solver):
+            operator assembly, the whole call, iterations; against scipy spsolve on the host and
+            against value_iteration sweeps to the same bound
 
-    python tools/bench_extra.py [bellman] [det] [c5] [shared] [roa] [reward_rollout]
+    python tools/bench_extra.py [bellman] [det] [c5] [shared] [roa] [reward_rollout] [value_opt]
 """
 import json
 import os
@@ -348,6 +353,79 @@ def reward_rollout():
                                                                           np.isfinite(o_sums)))},
                       "note": "point-steps counted up to T*; the chunk holding T* runs twice "
                               "(at most 32 extra steps)", **info}))
+
+
+def value_opt():
+    import time
+    from safe_learning_b200 import _device as dev, _native as nat
+    lib = nat.load()
+    for num, M in ((55, 50), (512, 500)):
+        par = W.make_pendulum(num_points=8, M=M)
+        grid = sl.GridWorld(par["limits"], num)
+        _, dyn = W._build(sl, par, "product")
+        policy = sl.Saturation(sl.LinearSystem(-par["K"]), -1., 1.)
+        reward = sl.QuadraticFunction(-scipy.linalg.block_diag(np.diag([1., 2.]), 1.2 * np.eye(1)))
+        value = sl.Triangulation(grid, np.zeros((grid.nindex, 1)), project=True)
+        rl = sl.PolicyIteration(policy, dyn, reward, value, gamma=0.98)
+        n = grid.nindex
+        cols, w = dev.empty((n, 3), torch.int32), dev.empty((n, 3))
+        r, stats = dev.empty((n,)), dev.zeros((nat.VALUE_STATS,), torch.int64)
+        cfg = rl.bellman_descriptor()
+
+        def assemble():
+            nat.check(lib.slb_value_operator(dev.stream(), cfg, 0, n, cols.data_ptr(), w.data_ptr(),
+                                             r.data_ptr(), stats.data_ptr()), "slb_value_operator")
+
+        ms_assembly = timed(assemble, steps=10)
+        v = dev.empty((n,))
+        need = int(lib.slb_value_solve_workspace(n, 3))
+        work = dev.empty((need // 8,)) if need else None
+
+        def solve():                     # the solver launch alone, from a zero table
+            v.zero_()
+            nat.check(lib.slb_value_solve(dev.stream(), n, 3, cols.data_ptr(), w.data_ptr(),
+                                          r.data_ptr(), 0.98, 1e-10, 200000, v.data_ptr(),
+                                          dev.ptr(work), stats.data_ptr()), "slb_value_solve")
+
+        assemble()
+        ms_solve = timed(solve, steps=5, warmup=1)
+
+        def cold_call():
+            value.parameters = np.zeros((n, 1))
+            rl.optimize_value_function()
+
+        info = _gpu_info(cold_call)
+        ms_call = timed(cold_call, steps=5, warmup=1)
+        it = rl.last_solve["iterations"]
+        ms_warm = timed(rl.optimize_value_function, steps=5, warmup=1)
+        warm_iters = rl.last_solve["iterations"]
+        ms_sweep = timed(rl.value_iteration, steps=10)
+        # host reference: the same operator, scipy's sparse LU
+        assemble()
+        c, wt, rw = cols.cpu().numpy(), w.cpu().numpy(), r.cpu().numpy()
+        t0 = time.perf_counter()
+        import scipy.sparse as sps
+        import scipy.sparse.linalg as spla
+        T = sps.csr_matrix((wt.ravel(), (np.repeat(np.arange(n), 3), c.ravel())), shape=(n, n))
+        exact = spla.spsolve((sps.identity(n) - 0.98 * T).tocsc(), rw)
+        ms_spsolve = (time.perf_counter() - t0) * 1e3
+        value.parameters = np.zeros((n, 1))
+        got = rl.optimize_value_function().ravel()
+        print(json.dumps({"bench": "value_opt", "grid": "%dx%d" % (num, num), "M": M,
+                          "tier": rl.last_solve["tier"], "iterations": it,
+                          "ms_assembly": ms_assembly, "ms_call_cold": ms_call,
+                          "ms_solve": ms_solve, "us_per_iteration": ms_solve * 1e3 / it,
+                          "ms_call_warm": ms_warm, "warm_iterations": warm_iters,
+                          "ms_spsolve_host": ms_spsolve,
+                          "max_abs_diff_vs_spsolve": float(np.max(np.abs(got - exact))),
+                          "bound": rl.last_solve["bound"],
+                          "ms_value_iteration_sweep": ms_sweep,
+                          "ms_value_iteration_same_bound": ms_sweep * it,
+                          "note": "median of CUDA events; ms_solve is the solver launch alone (plus a "
+                                  "table reset), the call includes assembly, solve, the host-side work "
+                                  "and the one device-to-host copy; value iteration to the same bound takes "
+                                  "the same number of sweeps (the same map), timed per sweep",
+                          **info}))
 
 
 if __name__ == "__main__":
