@@ -417,7 +417,8 @@ int slb_bellman_sweep(void* stream, const slb_bellman* cfg, int64_t idx_begin, i
 /* discrete_policy_optimization: actions_dev [n_actions, m]; constraint_dev [n_actions, n] or
  * NULL (value < 0 => -inf, :272-275); best_dev[i] = first argmax over actions (:278, NaN counts as
  * the maximum like np.argmax).  workspace_dev: NULL, or >= slb_bellman_argmax_workspace bytes: with
- * GP dynamics on plain RBF factors the action is then factored out of the exponent (one kernel
+ * GP dynamics on plain RBF factors and a state dimension of 1 or 2 (n_actions >= 2) the action
+ * is then factored out of the exponent (one kernel
  * row per STATE, an [n_actions x M] x [M x states] fp64 tensor-core contraction per output)
  * instead of n_actions sweeps; the workspace size is 0 when that path does not apply. */
 int64_t slb_bellman_argmax_workspace(const slb_bellman* cfg, int32_t n_actions);

@@ -274,6 +274,10 @@ constexpr size_t tile_smem(int ds, int D) {
     return ((size_t)(BCH / 8) * 4 * BKSTR * 2 + (size_t)BCH * ds + 64 + (size_t)ds * BS + 4 * BS) *
                sizeof(double) + 4 * BS * sizeof(int) + (size_t)D * 8 * BMAXRB * BS * sizeof(double);
 }
+// A Bellman GP stack has one output per state dimension (slb_validate_bellman), so the means of a
+// pass take D = d slices of Cm: from d = 3 on the tile no longer fits, and only DS = 1, 2 exist.
+static_assert(tile_smem(2, 2) <= 227 * 1024 && tile_smem(3, 3) > 227 * 1024,
+              "factored argmax: state dimensions 1..2 fit the CTA, 3 does not");
 
 template <int DS>
 int launch_argmax_tile(cudaStream_t st, const slb_bellman& cfg, const argmax_args& a) {
@@ -298,7 +302,7 @@ int launch_argmax_tile(cudaStream_t st, const slb_bellman& cfg, const argmax_arg
 bool slb_argmax_factorable(const slb_bellman& cfg, int m, int n_actions) {
     if (cfg.gp.num_outputs <= 0 || n_actions < 2) return false;
     const int d = cfg.grid.ndim;
-    if (d < 1 || d > 4 || m < 1) return false;
+    if (d < 1 || d > 2 || m < 1) return false;
     for (int f = 0; f < cfg.gp.num_factors; ++f)
         if (cfg.gp.factors[f].kernel.num_prims > 0 || cfg.gp.factors[f].M == 0) return false;
     for (int o = 0; o < cfg.gp.num_outputs; ++o)
@@ -339,10 +343,8 @@ int slb_launch_argmax_factored(cudaStream_t st, const slb_bellman& cfg, int64_t 
     switch (d) {
     case 1: return launch_argmax_tile<1>(st, cfg, a);
     case 2: return launch_argmax_tile<2>(st, cfg, a);
-    case 3: return launch_argmax_tile<3>(st, cfg, a);
-    case 4: return launch_argmax_tile<4>(st, cfg, a);
     default:
-        slb_set_error("factored argmax: state dimension %d not compiled (1..4)", d);
+        slb_set_error("factored argmax: state dimension %d not compiled (1..2)", d);
         return 1;
     }
 }
