@@ -69,7 +69,7 @@ enum slb_fn_kind {
     SLB_FN_PENDULUM = 5,       /* InvertedPendulum            examples/utilities.py:144-289 */
     SLB_FN_CARTPOLE = 6,       /* CartPole                    examples/utilities.py:292-437 */
     SLB_FN_LYAPUNOV_NN = 7,    /* LyapunovNetwork             examples/utilities.py:48-104  */
-    SLB_FN_MLP = 8             /* NeuralNetwork (inference)   functions.py:1702-1729        */
+    SLB_FN_MLP = 8             /* NeuralNetwork               functions.py:1702-1729        */
 };
 /* post-ops, applied in this order: saturate -> abs -> norm1 | maxabs -> out_scale */
 #define SLB_FLAG_SATURATE 1u   /* Saturation  functions.py:349-354                     */
@@ -486,6 +486,26 @@ int64_t slb_value_solve_workspace(int64_t n, int32_t ncols);
 int slb_value_solve(void* stream, int64_t n, int32_t ncols, const void* cols_dev, const double* weights_dev,
                     const double* rewards_dev, double gamma, double tol, int64_t max_iters,
                     double* v_inout_dev, void* workspace_dev, uint64_t* stats_dev);
+
+/* ---- reverse mode of the fused networks and plants (the reference's tf.gradients through
+ *      NeuralNetwork functions.py:1702-1729, LyapunovNetwork and the plants examples/utilities.py:48-104,
+ *      242-289, 387-437): for a cotangent grad_out_dev [n, out] (out = 1 for LYAPUNOV_NN)
+ *        grad_in_dev     [n, in]  = grad_out^T d out / d points               (or NULL)
+ *        grad_params_dev          = sum over the n points of grad_out^T d out / d params, OVERWRITTEN,
+ *                                   in the layout of fn->matrix (MLP: packed weights and biases; LYAPUNOV_NN:
+ *                                   the packed layer kernels [W^T W + eps I; W_extra]); NULL, and NULL for
+ *                                   the plants, which have no parameters
+ *        out_dev         [n, out] = the forward pass recomputed by the gradient kernel, bit-identical to
+ *                                   slb_eval_function (or NULL)
+ *      Kinds MLP, LYAPUNOV_NN, PENDULUM and CARTPOLE without post-op flags.  Gradient conventions: ReLU' = 0
+ *      at 0, tanh' = 1 - tanh^2.  The parameter gradient is reduced in a fixed order without atomics: two
+ *      calls with the same inputs give bit-identical results.  n == 0 zeroes grad_params and launches
+ *      nothing.  workspace_dev: >= slb_function_vjp_workspace(fn, n) bytes when grad_params_dev is
+ *      given (0 for the plants and for n <= 32); the size function returns -1 for a descriptor it rejects. */
+int64_t slb_function_vjp_workspace(const slb_function* fn, int64_t n);
+int slb_function_vjp(void* stream, const slb_function* fn, const double* points_dev, int64_t n,
+                     const double* grad_out_dev, double* grad_in_dev, double* grad_params_dev,
+                     double* out_dev, void* workspace_dev);
 
 #ifdef __cplusplus
 }

@@ -173,6 +173,8 @@ SIGNATURES = {
     "slb_value_solve_workspace": (C.c_int64, [_i64, _i32]),
     "slb_value_solve": (C.c_int, [_vp, _i64, _i32, _vp, _dp, _dp, C.c_double, C.c_double, _i64, _dp,
                                   _vp, _vp]),
+    "slb_function_vjp_workspace": (C.c_int64, [C.POINTER(SlbFunction), _i64]),
+    "slb_function_vjp": (C.c_int, [_vp, C.POINTER(SlbFunction), _dp, _i64, _dp, _dp, _dp, _dp, _vp]),
 }
 
 _lib = None

@@ -245,8 +245,45 @@ class _FusedApply(torch.autograd.Function):
     @staticmethod
     def backward(ctx, grad_out):
         (points,) = ctx.saved_tensors
+        if isinstance(ctx.fun, (InvertedPendulum, CartPole)):      # one slb_function_vjp call
+            return _function_vjp(ctx.fun, points, grad_out)[0], None
         jac = ctx.fun.jacobian_device(points)                       # [n, out, in]
         return torch.einsum("no,noi->ni", grad_out.contiguous(), jac), None
+
+
+def _function_vjp(fun, points, grad_out, want_in=True, nparams=0, want_out=False):
+    """One ``slb_function_vjp`` call: (grad_in [n, in] or None, grad_params [nparams] or None,
+    recomputed forward [n, out] or None), device tensors."""
+    lib = nat.load()
+    desc = fun.descriptor()
+    pts = dev.to_device(points)
+    n = pts.shape[0]
+    ncols = 1 if desc.kind == nat.FN_LYAPUNOV_NN else desc.out_dim
+    gout = dev.to_device(grad_out).reshape(n, ncols).contiguous()
+    gin = dev.empty((n, desc.in_dim)) if want_in else None
+    gpar = dev.empty((nparams,)) if nparams else None
+    out = dev.empty((n, ncols)) if want_out else None
+    ws = None
+    if gpar is not None:
+        size = lib.slb_function_vjp_workspace(desc, n)
+        if size < 0:
+            raise nat.NativeLibraryError("slb_function_vjp_workspace: %s" % nat.last_error())
+        ws = torch.empty(size, dtype=torch.uint8, device=pts.device) if size else None
+    nat.check(lib.slb_function_vjp(dev.stream(), desc, pts.data_ptr(), n, gout.data_ptr(), dev.ptr(gin),
+                                   dev.ptr(gpar), dev.ptr(out), dev.ptr(ws)), "slb_function_vjp")
+    return gin, gpar, out
+
+
+def _unit_vjp_jacobian(fun, points):
+    """[n, out, in] from out_dim VJPs with unit cotangents."""
+    pts = dev.to_device(points)
+    n, nout = pts.shape[0], fun.output_dim
+    rows = []
+    for o in range(nout):
+        cot = dev.zeros((n, nout))
+        cot[:, o] = 1.0
+        rows.append(_function_vjp(fun, pts, cot)[0])
+    return torch.stack(rows, dim=1)
 
 
 class DeterministicFunction(Function):
@@ -347,7 +384,12 @@ class _PostOp(DeterministicFunction):
                 "%s around %s: post-operations fuse only in the order "
                 "saturate -> abs -> norm1 -> scale" % (type(self).__name__, type(fun).__name__))
         self.fun = fun
-        self.input_dim = fun.input_dim
+
+    @property
+    def input_dim(self):
+        # read through, so that a wrapped network in the reference's convention reports the width
+        # its first evaluation gives it
+        return self.fun.input_dim
 
     @property
     def parameters(self):
@@ -706,6 +748,10 @@ class InvertedPendulum(DeterministicFunction):
         cp[10] = 1.0 if self.friction > 0 else 0.0
         return d
 
+    def jacobian_device(self, points):
+        """d x+ / d [x, u] through the ten Euler sub-steps, [n, 2, 3] (``slb_function_vjp``)."""
+        return _unit_vjp_jacobian(self, points)
+
 
 class CartPole(DeterministicFunction):
     """Cart-pole (``examples/utilities.py:292-437``)."""
@@ -746,15 +792,137 @@ class CartPole(DeterministicFunction):
         cp[15] = _pack_norm(cp, self.normalization, 4, 6)    # [6..9] Tx, [10] Tu, [11..14] 1/Tx
         return d
 
+    def jacobian_device(self, points):
+        """d x+ / d [x, u] through the ten Euler sub-steps, [n, 4, 5] (``slb_function_vjp``)."""
+        return _unit_vjp_jacobian(self, points)
 
-class LyapunovNetwork(DeterministicFunction):
-    """Positive-definite network ``V(x) = |phi(x)|^2`` (``examples/utilities.py:48-104``),
-    inference only: layer i applies ``act(net . [W_i^T W_i + eps I; W_i'']^T)``.
+
+def _param_device():
+    """Where network parameters live: the library's device when torch sees one (every evaluation
+    needs it), otherwise the CPU, so that a network can be built and inspected on a host without a
+    GPU."""
+    return dev.device() if torch.cuda.is_available() else torch.device("cpu")
+
+
+def _leaf(value):
+    """A float64 leaf tensor with requires_grad on the parameter device (copies its input)."""
+    if isinstance(value, torch.Tensor):
+        t = value.detach().to(device=_param_device(), dtype=torch.float64).clone()
+    else:
+        t = torch.tensor(np.asarray(value, dtype=np.float64), device=_param_device())
+    return t.requires_grad_(True)
+
+
+class _TrainableNetwork(DeterministicFunction):
+    """Parameters as torch leaf tensors (``parameters``), a descriptor rebuilt whenever one of them
+    changes (``version`` follows ``torch.Tensor._version``, so in-place optimizer steps count), and
+    ``torch(points)`` as one autograd node whose backward is one ``slb_function_vjp`` call for the
+    points and every parameter."""
+
+    def _init_params(self):
+        self._params = []
+        self._names = []
+        self._set_count = 0
+        self._packed = None
+        self._packed_version = None
+
+    @property
+    def parameters(self):
+        return list(self._params)
+
+    @parameters.setter
+    def parameters(self, values):
+        values = list(values)
+        if len(values) != len(self._params):
+            raise ValueError("%s has %d parameter tensors, got %d"
+                             % (type(self).__name__, len(self._params), len(values)))
+        new = []
+        for old, v in zip(self._params, values):
+            t = _leaf(v)
+            if tuple(t.shape) != tuple(old.shape):
+                raise DimensionError("parameter shape %s, expected %s" % (tuple(t.shape), tuple(old.shape)))
+            new.append(t)
+        self._set_params(new)
+
+    @property
+    def parameter_names(self):
+        """TF variable names of ``parameters``, in the reference's creation order."""
+        return list(self._names)
+
+    def _set_params(self, tensors):
+        self._params = tensors
+        self._set_count += 1
+
+    @property
+    def version(self):
+        return (self._set_count,) + tuple(t._version for t in self._params)
+
+    def _packed_device(self):
+        """The descriptor's parameter buffer for the current parameter version."""
+        v = self.version
+        if self._packed is None or self._packed_version != v:
+            self._packed = self._pack()
+            self._packed_version = v
+        return self._packed
+
+    def torch(self, points):
+        """``fun(points)`` on a device tensor [n, in] as one autograd node: forward = the fused
+        evaluation, backward = one ``slb_function_vjp`` call giving the gradients of ``points`` and
+        of every tensor in ``parameters``."""
+        return _NetworkApply.apply(points, self, *self._params)
+
+    def jacobian_device(self, points):
+        return _unit_vjp_jacobian(self, points)
+
+    def vjp(self, points, grad_out, want_out=False):
+        """(grad_in [n, in], [grad of each parameter], recomputed forward or None) for the cotangent
+        ``grad_out`` [n, out] (device tensors)."""
+        gin, gflat, out = _function_vjp(self, points, grad_out, True, self._packed_device().numel(),
+                                        want_out)
+        return gin, self._grads_like(gflat, self._params), out
+
+    def _grads_like(self, gflat, params):
+        """The flat parameter gradient as one tensor per parameter, each on its parameter's device
+        (a network built before ``torch.cuda.set_device`` keeps its leaves where they were made)."""
+        return [g.to(p.device) for g, p in zip(self._unpack_grads(gflat), params)]
+
+
+class _NetworkApply(torch.autograd.Function):
+    """A NeuralNetwork / LyapunovNetwork in torch's autograd graph with its parameters as inputs."""
+
+    @staticmethod
+    def forward(ctx, points, fun, *params):
+        points = points.detach().contiguous()
+        ctx.fun = fun
+        ctx.save_for_backward(points, *params)       # torch refuses backward after an in-place update
+        return fun.evaluate_device(points)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_out):
+        # the VJP kernel is not itself differentiable: double backward raises instead of treating
+        # the gradient as a constant
+        points, params = ctx.saved_tensors[0], ctx.saved_tensors[1:]
+        fun = ctx.fun
+        want_params = any(ctx.needs_input_grad[2:])
+        gin, gflat, _ = _function_vjp(fun, points, grad_out, ctx.needs_input_grad[0],
+                                      fun._packed_device().numel() if want_params else 0)
+        if gin is not None:
+            gin = gin.to(points.device)
+        grads = fun._grads_like(gflat, params) if want_params else [None] * len(params)
+        return (gin, None) + tuple(grads)
+
+
+class LyapunovNetwork(_TrainableNetwork):
+    """Positive-definite network ``V(x) = |phi(x)|^2`` (``examples/utilities.py:48-104``):
+    layer i applies ``act(net . [W_i^T W_i + eps I; W_i'']^T)``.
 
     ``weights[i] = (W_posdef, W_extra or None)`` with the reference's shapes
     (``[ceil((in+1)/2), in]`` and ``[out - in, in]``); when omitted they are drawn Xavier-uniform
     from ``seed`` (the reference uses ``tf.contrib.layers.xavier_initializer``).  ``activations``
-    are 'tanh' | 'relu' | 'linear' (or ``numpy.tanh``).
+    are 'tanh' | 'relu' | 'linear' (or ``numpy.tanh``).  ``parameters`` holds the same matrices as
+    trainable tensors, in the reference's variable order ``weights_posdef_i``, ``weights_i``; the
+    layer kernels are formed from them on the host once per parameter version.
     """
 
     _ACT = {"tanh": 0, "relu": 1, "linear": 2, "identity": 2}
@@ -791,40 +959,107 @@ class LyapunovNetwork(DeterministicFunction):
                 extra = self.output_dims[i] - din
                 weights.append((xavier(self.hidden_dims[i], din),
                                 xavier(extra, din) if extra > 0 else None))
+        self._init_params()
         self.weights = weights
-        self._kernel_dev = None
+
+    def _layer_in(self, i):
+        return self.input_dim if i == 0 else self.output_dims[i - 1]
+
+    @property
+    def weights(self):
+        """``[(W_posdef, W_extra or None)]`` per layer, numpy copies of the current parameters."""
+        out, it = [], iter(self._params)
+        for i in range(self.num_layers):
+            w0 = next(it).detach().cpu().numpy()
+            w1 = next(it).detach().cpu().numpy() if self.output_dims[i] > self._layer_in(i) else None
+            out.append((w0, w1))
+        return out
+
+    @weights.setter
+    def weights(self, weights):
+        params, names = [], []
+        for i, (w0, w1) in enumerate(weights):
+            din = self._layer_in(i)
+            w0 = np.asarray(w0.detach().cpu().numpy() if isinstance(w0, torch.Tensor) else w0,
+                            dtype=np.float64)
+            if w0.ndim != 2 or w0.shape[1] != din:
+                raise DimensionError("weights_posdef_%d must have %d columns, got shape %s"
+                                     % (i, din, w0.shape))
+            params.append(_leaf(w0))
+            names.append("weights_posdef_%d" % i)
+            if self.output_dims[i] > din:
+                if w1 is None or tuple(np.shape(w1) if not hasattr(w1, "shape") else w1.shape) != \
+                        (self.output_dims[i] - din, din):
+                    raise DimensionError("weights_%d must have shape %s"
+                                         % (i, (self.output_dims[i] - din, din)))
+                params.append(_leaf(w1))
+                names.append("weights_%d" % i)
+        if len(weights) != self.num_layers:
+            raise DimensionError("%d layers need %d weight pairs" % (self.num_layers, len(weights)))
+        self._names = names
+        self._set_params(params)
 
     def kernels(self):
         """Layer kernels ``[W^T W + eps I; W_extra]`` ([out_i, in_i])."""
         out = []
         for i, (w0, w1) in enumerate(self.weights):
-            din = self.input_dim if i == 0 else self.output_dims[i - 1]
+            din = self._layer_in(i)
             k = w0.T.dot(w0) + self.eps * np.eye(din)
             if w1 is not None:
                 k = np.concatenate([k, w1], axis=0)
             out.append(k)
         return out
 
+    def _pack(self):
+        return dev.to_device(np.concatenate([k.ravel() for k in self.kernels()]))
+
     def descriptor(self):
-        if self._kernel_dev is None:
-            self._kernel_dev = dev.to_device(np.concatenate([k.ravel() for k in self.kernels()]))
         d = nat.SlbFunction()
         d.kind, d.in_dim, d.out_dim = nat.FN_LYAPUNOV_NN, self.input_dim, 1
         d.cparams[0] = self.num_layers
         for i, (od, act) in enumerate(zip(self.output_dims, self.activations)):
             d.cparams[1 + i] = od
             d.cparams[9 + i] = self._ACT[act]
-        d.matrix = self._kernel_dev.data_ptr()
+        d.matrix = self._packed_device().data_ptr()
         return d
 
+    def _unpack_grads(self, gflat):
+        """dL/dK_i -> the leaves: dW_posdef = W (G + G^T) over the top in_i rows, dW_extra = G below."""
+        grads, off, it = [], 0, iter(self._params)
+        for i in range(self.num_layers):
+            din, dout = self._layer_in(i), self.output_dims[i]
+            G = gflat[off:off + dout * din].view(dout, din)
+            off += dout * din
+            top = G[:din]
+            grads.append(next(it).detach() @ (top + top.T))
+            if dout > din:
+                next(it)
+                grads.append(G[din:].clone())
+        return grads
 
-class NeuralNetwork(DeterministicFunction):
-    """Dense MLP, inference only (``functions.py:1665-1729``): bias in the hidden layers only,
-    no bias in the output layer, output multiplied by ``output_scale``.  ``layers`` =
-    [in, h1, ..., out]; ``nonlinearities`` one per layer after the input ('tanh' | 'relu' | None).
+    def gradient(self, points):
+        """dV/dx at the points, numpy ``[n, d]`` (``tf.gradients(V(x), x)`` of the notebooks)."""
+        pts = dev.to_device(concatenate_inputs([points]) if not isinstance(points, torch.Tensor)
+                            else points)
+        gin, _, _ = _function_vjp(self, pts, torch.ones((pts.shape[0], 1), dtype=torch.float64,
+                                                          device=pts.device))
+        return gin.cpu().numpy()
+
+
+class NeuralNetwork(_TrainableNetwork):
+    """Dense MLP (``functions.py:1665-1729``): bias in the hidden layers only, no bias in the output
+    layer, output multiplied by ``output_scale``; ``nonlinearities`` one per layer ('tanh' | 'relu' |
+    None).
+
+    Two conventions for ``layers``:
+      - ``[in, h1, ..., out]`` with one nonlinearity per layer after the input: built at once;
+      - the reference's ``[h1, ..., out]`` with as many nonlinearities as entries: every entry is a
+        layer width, and the input width and the parameters are created at the first evaluation, as
+        the reference's TF variables are (``parameters`` is ``[]`` before that).
     ``weights[i]`` has the TF layout ``[in_i, out_i]``, ``biases[i]`` ``[out_i]`` (hidden layers);
-    both are drawn Xavier-uniform / zero from ``seed`` when omitted.  Training (the reference
-    optimises these with TF optimisers) is outside this build.
+    both are drawn Xavier-uniform / zero from ``seed`` when omitted.  ``parameters`` holds them as
+    trainable tensors in the reference's variable order (``layer_i/kernel``, ``layer_i/bias``, ...,
+    ``output/kernel``).
     """
 
     def __init__(self, layers, nonlinearities, output_scale=1., use_bias=True,
@@ -838,43 +1073,167 @@ class NeuralNetwork(DeterministicFunction):
             if key not in LyapunovNetwork._ACT:
                 raise NotImplementedError("nonlinearity %r is not fused (tanh/relu/None)" % (act,))
             self.nonlinearities.append(key)
-        if len(self.nonlinearities) != len(self.layers) - 1:
+        if len(self.nonlinearities) == len(self.layers):
+            widths = list(self.layers)                       # reference convention: input inferred
+        elif len(self.nonlinearities) == len(self.layers) - 1:
+            widths = self.layers[1:]
+        else:
             raise ValueError("one nonlinearity per layer after the input is required")
         self.output_scale = float(output_scale)
         self.use_bias = bool(use_bias)
-        self.input_dim, self.output_dim = self.layers[0], self.layers[-1]
-        if max(self.layers[1:]) > 64 or len(self.layers) - 1 > 8 or self.output_dim > nat.SLB_MAX_OUT:
+        self.output_dim = widths[-1]
+        if max(widths) > 64 or len(widths) > 8 or self.output_dim > nat.SLB_MAX_OUT:
             raise DimensionError("NeuralNetwork: at most 8 layers of width <= 64 are fused")
-        rng = np.random.default_rng(seed)
+        self._widths = widths
+        self._seed = seed
+        self._init_params()
+        self._biases_unused = None
+        self.input_dim = None
+        if len(self.nonlinearities) == len(self.layers) - 1:
+            self._create(self.layers[0], weights, biases)
+        elif weights is not None:
+            self._create(int(np.shape(weights[0])[0]), weights, biases)
+        elif biases is not None:
+            raise ValueError("biases without weights need the [in, h1, ..., out] convention")
+
+    @property
+    def built(self):
+        return self.input_dim is not None
+
+    def _create(self, input_dim, weights=None, biases=None):
+        """Create the parameters for input width ``input_dim`` (drawn from ``seed`` when omitted)."""
+        self.input_dim = int(input_dim)
+        if self.input_dim > nat.SLB_MAX_IN:
+            raise DimensionError("NeuralNetwork: input width above %d" % nat.SLB_MAX_IN)
+        dims = [self.input_dim] + self._widths
+        rng = np.random.default_rng(self._seed)
         if weights is None:
             weights = []
-            for din, dout in zip(self.layers[:-1], self.layers[1:]):
+            for din, dout in zip(dims[:-1], dims[1:]):
                 lim = np.sqrt(6.0 / (din + dout))
                 weights.append(rng.uniform(-lim, lim, size=(din, dout)))
         if biases is None:
-            biases = [np.zeros(d) for d in self.layers[1:-1]]
-        self.weights = [np.asarray(w, dtype=np.float64) for w in weights]
-        self.biases = [np.asarray(b, dtype=np.float64) for b in biases]
-        self._param_dev = None
+            biases = [np.zeros(d) for d in dims[1:-1]]
+        self._dims = dims
+        self._set_weights_biases(weights, biases)
+
+    def build(self, input_dim):
+        """Create the parameters for input width ``input_dim`` unless they exist (what the first
+        evaluation does with its points' width).  A network in the reference's convention needs this,
+        or one evaluation, before it is handed to a fused consumer (Lyapunov, PolicyIteration,
+        ClosedLoop), which reads its descriptor."""
+        if not self.built:
+            self._create(input_dim)
+
+    def _set_weights_biases(self, weights, biases):
+        dims = self._dims
+        weights = [np.asarray(w.detach().cpu().numpy() if isinstance(w, torch.Tensor) else w,
+                              dtype=np.float64) for w in weights]
+        biases = [np.asarray(b.detach().cpu().numpy() if isinstance(b, torch.Tensor) else b,
+                             dtype=np.float64) for b in biases]
+        if len(weights) != len(dims) - 1 or any(w.shape != (a, b) for w, a, b in
+                                               zip(weights, dims[:-1], dims[1:])):
+            raise DimensionError("weights must have shapes %s"
+                                 % [(a, b) for a, b in zip(dims[:-1], dims[1:])])
+        if len(biases) != len(dims) - 2 or any(b.shape != (d,) for b, d in zip(biases, dims[1:-1])):
+            raise DimensionError("biases must have shapes %s" % [(d,) for d in dims[1:-1]])
+        params, names = [], []
+        for i, w in enumerate(weights[:-1]):
+            params.append(_leaf(w))
+            names.append("layer_%d/kernel" % i)
+            if self.use_bias:
+                params.append(_leaf(biases[i]))
+                names.append("layer_%d/bias" % i)
+        params.append(_leaf(weights[-1]))
+        names.append("output/kernel")
+        self._biases_unused = None if self.use_bias else biases
+        self._names = names
+        self._set_params(params)
+
+    def _kernel_tensors(self):
+        step = 2 if self.use_bias else 1
+        return self._params[0:-1:step] + [self._params[-1]]
+
+    @property
+    def weights(self):
+        """Layer kernels ``[in_i, out_i]``, numpy copies of the current parameters."""
+        return [t.detach().cpu().numpy() for t in self._kernel_tensors()] if self.built else []
+
+    @weights.setter
+    def weights(self, weights):
+        if not self.built:
+            self._create(int(np.shape(weights[0])[0]), weights)
+        else:
+            self._set_weights_biases(weights, self.biases)
+
+    @property
+    def biases(self):
+        """Hidden-layer biases ``[out_i]``, numpy copies of the current parameters."""
+        if not self.built:
+            return []
+        if not self.use_bias:
+            return [np.array(b) for b in self._biases_unused]
+        return [t.detach().cpu().numpy() for t in self._params[1:-1:2]]
+
+    @biases.setter
+    def biases(self, biases):
+        if not self.built:
+            raise ValueError("the network creates its parameters at the first evaluation")
+        self._set_weights_biases(self.weights, biases)
+
+    def lipschitz(self):
+        """Product over the layer kernels of their largest singular value (``functions.py:1742-1761``).
+        Every kernel enters, also with ``use_bias=False`` (where the reference's pairing of
+        parameters skips every second one)."""
+        out = 1.0
+        for w in self.weights:
+            out *= float(np.linalg.svd(w, compute_uv=False).max())
+        return out
+
+    def _pack(self):
+        parts = []
+        for i, t in enumerate(self._params):
+            name = self._names[i]
+            parts.append(t.detach().T.reshape(-1) if name.endswith("kernel") else t.detach().reshape(-1))
+        return torch.cat(parts).to(dev.device()).contiguous()
+
+    def _unpack_grads(self, gflat):
+        grads, off = [], 0
+        for t, name in zip(self._params, self._names):
+            if name.endswith("kernel"):
+                din, dout = t.shape
+                grads.append(gflat[off:off + din * dout].view(dout, din).T.contiguous())
+                off += din * dout
+            else:
+                grads.append(gflat[off:off + t.shape[0]].clone())
+                off += t.shape[0]
+        return grads
 
     def descriptor(self):
-        if self._param_dev is None:
-            parts = []
-            for i, w in enumerate(self.weights):
-                parts.append(w.T.ravel())                       # [out, in] rows
-                if self.use_bias and i + 1 < len(self.weights):
-                    parts.append(self.biases[i].ravel())
-            self._param_dev = dev.to_device(np.concatenate(parts))
+        if not self.built:
+            raise DimensionError("NeuralNetwork(%s): the input width is set by the first evaluation;"
+                                 " call build(input_dim) or evaluate it once before fusing it"
+                                 % self.layers)
         d = nat.SlbFunction()
         d.kind, d.in_dim, d.out_dim = nat.FN_MLP, self.input_dim, self.output_dim
-        d.cparams[0] = len(self.weights)
-        for i, (od, act) in enumerate(zip(self.layers[1:], self.nonlinearities)):
+        d.cparams[0] = len(self._widths)
+        for i, (od, act) in enumerate(zip(self._widths, self.nonlinearities)):
             d.cparams[1 + i] = od
             d.cparams[9 + i] = LyapunovNetwork._ACT[act]
         d.cparams[17] = self.output_scale
         d.cparams[18] = 1.0 if self.use_bias else 0.0
-        d.matrix = self._param_dev.data_ptr()
+        d.matrix = self._packed_device().data_ptr()
         return d
+
+    def evaluate_device(self, points):
+        pts = dev.to_device(points)
+        if pts.dim() == 2:
+            self.build(pts.shape[1])
+        return super().evaluate_device(pts)
+
+    def torch(self, points):
+        self.build(points.shape[1])
+        return super().torch(points)
 
 
 # =============================================================================== Gaussian processes

@@ -17,8 +17,12 @@
             (M=500, the cooperative solver):
             operator assembly, the whole call, iterations; against scipy spsolve on the host and
             against value_iteration sweeps to the same bound
+  train     slb_function_vjp (gradients of the points and of every parameter) for
+            LyapunovNetwork(2, [64, 64, 64], tanh) and the 2-64-64-1 ReLU MLP on 100, 1000 and 251^2
+            points, against torch's autograd of the same network on the same GPU (fp64 cuBLAS), and the
+            per-step time of three notebook training loops (value net, policy net, Lyapunov pre-training)
 
-    python tools/bench_extra.py [bellman] [det] [c5] [shared] [roa] [reward_rollout] [value_opt]
+    python tools/bench_extra.py [bellman] [det] [c5] [shared] [roa] [reward_rollout] [value_opt] [train]
 """
 import json
 import os
@@ -425,6 +429,98 @@ def value_opt():
                                   "table reset), the call includes assembly, solve, the host-side work "
                                   "and the one device-to-host copy; value iteration to the same bound takes "
                                   "the same number of sweeps (the same map), timed per sweep",
+                          **info}))
+
+
+def _torch_mlp(x, params, use_bias=True):
+    """The 2-64-64-1 ReLU MLP as plain torch operations (autograd through cuBLAS fp64)."""
+    k = params[0:-1:2] if use_bias else params[:-1]
+    b = params[1:-1:2] if use_bias else []
+    net = x
+    for i, w in enumerate(k):
+        net = torch.relu(net @ w + b[i] if use_bias else net @ w)
+    return net @ params[-1]
+
+
+def _torch_lnn(x, params, net_obj):
+    it, din, net = iter(params), net_obj.input_dim, x
+    for dout in net_obj.output_dims:
+        w0 = next(it)
+        k = w0.T @ w0 + net_obj.eps * torch.eye(din, dtype=torch.float64, device=x.device)
+        if dout > din:
+            k = torch.cat([k, next(it)], dim=0)
+        net = torch.tanh(net @ k.T)
+        din = dout
+    return torch.sum(net * net, dim=1, keepdim=True)
+
+
+def train():
+    """Gradient kernel against torch autograd, and per-step times of three notebook loops.  FLOPs per
+    point of one VJP: 6 sum_l in_l out_l (forward, weight gradient and input gradient, 2 each)."""
+    rng = np.random.default_rng(0)
+    lnn = sl.LyapunovNetwork(2, [64, 64, 64], ["tanh"] * 3, seed=1)
+    mlp = sl.NeuralNetwork([2, 64, 64, 1], ["relu", "relu", None], seed=1)
+    info = _gpu_info(lambda: mlp.vjp(torch.zeros((1000, 2), dtype=torch.float64, device="cuda"),
+                                     torch.ones((1000, 1), dtype=torch.float64, device="cuda")))
+    for name, net, ref in (("lyapunov_2x64x64x64_tanh", lnn, lambda x, p: _torch_lnn(x, p, lnn)),
+                           ("mlp_2x64x64x1_relu", mlp, _torch_mlp)):
+        if isinstance(net, sl.LyapunovNetwork):
+            dims = [2, 64, 64, 64]
+        else:
+            dims = [2, 64, 64, 1]
+        flops_pt = 6 * sum(a * b for a, b in zip(dims[:-1], dims[1:]))
+        for n in (100, 1000, 251 ** 2):
+            x = torch.tensor(rng.uniform(-1, 1, (n, 2)), device="cuda")
+            cot = torch.ones((n, 1), dtype=torch.float64, device="cuda")
+            ms_vjp = timed(lambda: net.vjp(x, cot), steps=50, warmup=5)
+            params = [p.detach().clone().requires_grad_(True) for p in net.parameters]
+            xr = x.clone().requires_grad_(True)
+
+            def torch_grad():
+                torch.autograd.grad(ref(xr, params).sum(), [xr] + params)
+            ms_torch = timed(torch_grad, steps=50, warmup=5)
+            print(json.dumps({"bench": "train_vjp", "network": name, "points": n,
+                              "ms_slb_function_vjp": ms_vjp, "ms_torch_autograd": ms_torch,
+                              "flops_per_point": flops_pt,
+                              "gflops_slb": flops_pt * n / ms_vjp / 1e6, **info}))
+    # the three loops of test_gpu_network_grad.py, one SGD step each
+    pend = sl.InvertedPendulum(0.15, 0.5, 0.1, 0.01, [(np.deg2rad(30), np.sqrt(9.81 / 0.5)),
+                                                      (9.81 * 0.15 * 0.5 * 0.5,)])
+    lqr, reward = sl.LinearSystem(np.array([[-0.7, -0.4]])), sl.QuadraticFunction(-0.1 * np.eye(3))
+    vf = sl.NeuralNetwork([64, 64, 1], ["relu", "relu", None], seed=2)
+    pol = sl.NeuralNetwork([64, 64, 1], ["relu", "relu", None], use_bias=False, seed=3)
+    xb = torch.tensor(rng.uniform(-1, 1, (100, 2)), device="cuda")
+    vf.torch(xb), pol.torch(xb)
+    opt_v, opt_p = torch.optim.SGD(vf.parameters, lr=0.005), torch.optim.SGD(pol.parameters, lr=0.6)
+    opt_l = torch.optim.SGD(lnn.parameters, lr=0.1)
+    xl = torch.tensor(rng.uniform(-0.07, 0.07, (1000, 2)), device="cuda")
+
+    def value_step():
+        z = torch.cat([xb, lqr.torch(xb)], dim=1)
+        target = (reward.torch(z) + 0.95 * vf.torch(pend.torch(z))).detach()
+        obj = torch.mean(torch.abs(vf.torch(xb) - target)) / 0.3
+        opt_v.zero_grad()
+        obj.backward()
+        opt_v.step()
+
+    def policy_step():
+        z = torch.cat([xb, pol.torch(xb)], dim=1)
+        obj = -0.25 * torch.mean(reward.torch(z) + 0.95 * vf.torch(pend.torch(z)))
+        opt_p.zero_grad()
+        obj.backward()
+        opt_p.step()
+
+    def pretrain_step():
+        obj = torch.mean(torch.abs(lnn.torch(xl) - 0.1 * torch.sum(xl * xl, dim=1, keepdim=True)))
+        opt_l.zero_grad()
+        obj.backward()
+        opt_l.step()
+
+    for name, step in (("value_net_batch100", value_step), ("policy_net_batch100", policy_step),
+                       ("lyapunov_pretrain_batch1000", pretrain_step)):
+        print(json.dumps({"bench": "train_loop", "loop": name, "ms_per_step": timed(step, steps=50),
+                          "note": "median of CUDA events around one SGD step (forward, backward, "
+                                  "update; the LyapunovNetwork forms its kernels on the host each step)",
                           **info}))
 
 
