@@ -205,7 +205,17 @@ typedef struct slb_gp_stack {
     slb_gp_output outputs[SLB_MAX_OUT];
 } slb_gp_stack;
 
-/* ---- one Lyapunov sweep: the graph of lyapunov.py:433-441 ----------------------------- */
+/* ---- one Lyapunov sweep: the graph of lyapunov.py:433-441 -----------------------------
+ * Shapes.  A function's COLUMNS are what it returns after its post-ops: out_dim, except 1 for
+ * QUADRATIC and LYAPUNOV_NN, 2 for PENDULUM, 4 for CARTPOLE, and 1 after NORM1 or MAXABS.  With
+ * d = grid.ndim and m = the policy's columns:
+ *   policy        d inputs, m = 1..SLB_MAX_ACT columns
+ *   dynamics      d + m inputs, d columns                   (gp.num_outputs == 0)
+ *   gp            d outputs, input_dim = d + m              (gp.num_outputs > 0)
+ *   lyapunov      d inputs
+ *   lipschitz_v   d inputs, 1 or d columns                  (or kind NONE)
+ *   lipschitz_f   d inputs; L_f is its first column         (or kind NONE)
+ * Every sweep entry point rejects a descriptor that breaks them, also for an empty index range. */
 typedef struct slb_sweep {
     slb_grid     grid;          /* discretization                                       */
     slb_function policy;        /* x -> u                       lyapunov.py:436         */
@@ -225,7 +235,16 @@ typedef struct slb_sweep {
     int64_t lf_index_base;
 } slb_sweep;
 
-/* ---- one Bellman sweep: PolicyIteration.future_values (reinforcement_learning.py:65-114) */
+/* ---- one Bellman sweep: PolicyIteration.future_values (reinforcement_learning.py:65-114)
+ * Shapes (columns as for slb_sweep), with d = grid.ndim and m = the policy's columns, or
+ * m = policy.out_dim with fixed_action (the action dimension; the rest of the policy is ignored):
+ *   policy        d inputs, m = 1..SLB_MAX_ACT columns
+ *   dynamics      d + m inputs, d columns                   (gp.num_outputs == 0)
+ *   gp            d outputs, input_dim = d + m              (gp.num_outputs > 0)
+ *   reward        d + m inputs, 1 column
+ *   value         d inputs, 1 column
+ * slb_bellman_sweep, slb_bellman_argmax and slb_value_operator reject a descriptor that breaks them
+ * before any work.  The rollouts check their own subset (see slb_rollout). */
 typedef struct slb_bellman {
     slb_grid     grid;          /* value_function.discretization (state space, :58-59)  */
     slb_function policy;        /* ignored when fixed_action != 0                       */

@@ -45,8 +45,14 @@ void slb_count_launch();
     } while (0)
 
 int slb_validate_function(const slb_function* f, const char* what, int expect_in /* <=0: any */);
+int slb_fn_columns(const slb_function& f);
+int slb_validate_dynamics(const slb_function* f, const char* who, int d, int m);
 int slb_validate_gp(const slb_gp_stack* gp);
+int slb_validate_staged_tables(const slb_gp_stack* gp, const char* who);
 int slb_validate_grid(const slb_grid* g, bool need_points);
+int slb_validate_range(const char* who, int64_t idx_begin, int64_t idx_end, int64_t nindex);
+// validates an slb_sweep descriptor (explicit_states: a sweep of a state list), *m_out = action dimension
+int slb_validate_sweep(const slb_sweep* cfg, bool explicit_states, int* m_out);
 
 // ----------------------------------------------------------------------------- device side
 #define SLB_DEV __device__ __forceinline__
@@ -637,7 +643,9 @@ SLB_DEV void eval_mlp(const slb_function& f, const double* in, double* out) {
 }
 
 // Evaluate a fused function object. `in` has f.in_dim entries, `out` receives the result
-// columns; returns the number of columns (1 after NORM1).  In gp_sweep.cu (SLB_EVAL_NOINLINE) it
+// columns; returns the number of columns (1 after NORM1 / MAXABS).  slb_fn_columns (light.cu) states
+// that number on the host, where it sizes the kernels and checks shapes: a change to one must be
+// made to the other.  In gp_sweep.cu (SLB_EVAL_NOINLINE) it
 // is deliberately NOT inlined: the tile kernel calls it five times per point (policy, V twice,
 // L_V twice) in cold prologue / epilogue code, and one shared copy keeps the kernel text small.
 // The thread-per-point kernels of light.cu inline it (the call overhead would cost them more).

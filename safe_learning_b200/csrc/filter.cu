@@ -900,56 +900,33 @@ int64_t slb_filter_workspace(int64_t n) {
 int slb_lyapunov_sweep_filtered(void* stream, const slb_sweep* cfg, int64_t idx_begin,
                                 int64_t idx_end, uint8_t* negative_dev, double* values_dev,
                                 void* workspace_dev, int64_t* stats_dev) {
-    SLB_CHECK(cfg != nullptr, "slb_lyapunov_sweep_filtered: null config");
-    SLB_CHECK(idx_begin >= 0 && idx_end >= idx_begin && idx_end <= cfg->grid.nindex,
-              "slb_lyapunov_sweep_filtered: index range [%lld, %lld) outside the grid (nindex %lld)",
-              (long long)idx_begin, (long long)idx_end, (long long)cfg->grid.nindex);
-    const int64_t n_all = idx_end - idx_begin;
-    if (n_all == 0) return 0;
-    SLB_CHECK(negative_dev != nullptr && workspace_dev != nullptr,
-              "slb_lyapunov_sweep_filtered: negative_dev and workspace_dev are required");
-    if (slb_validate_grid(&cfg->grid, false)) return 1;
-    const int d = cfg->grid.ndim;
-    if (slb_validate_function(&cfg->policy, "policy", d)) return 1;
-    SLB_CHECK(cfg->policy.kind != SLB_FN_NONE, "lyapunov sweep: a policy is required");
-    if (slb_validate_function(&cfg->lyapunov, "lyapunov_function", d)) return 1;
-    SLB_CHECK(cfg->lyapunov.kind != SLB_FN_NONE, "lyapunov sweep: a Lyapunov function is required");
-    if (slb_validate_function(&cfg->lipschitz_v, "lipschitz_lyapunov", d)) return 1;
-    if (slb_validate_function(&cfg->lipschitz_f, "lipschitz_dynamics", d)) return 1;
-    const int m = (cfg->policy.flags & SLB_FLAG_NORM1) ? 1 : cfg->policy.out_dim;
-    SLB_CHECK(m >= 1 && m <= SLB_MAX_ACT, "policy output dim %d unsupported", m);
+    int m;
+    if (slb_validate_sweep(cfg, false, &m)) return 1;
+    if (slb_validate_range("slb_lyapunov_sweep_filtered", idx_begin, idx_end, cfg->grid.nindex)) return 1;
     SLB_CHECK(cfg->gp.num_outputs > 0, "slb_lyapunov_sweep_filtered needs GP dynamics "
               "(deterministic dynamics have nothing to filter: use slb_lyapunov_sweep)");
-    if (slb_validate_gp(&cfg->gp)) return 1;
-    SLB_CHECK(cfg->gp.num_outputs == d, "GP stack has %d outputs but the state has %d dims",
-              cfg->gp.num_outputs, d);
-    SLB_CHECK(cfg->gp.input_dim == d + m, "GP input_dim %d != state %d + action %d",
-              cfg->gp.input_dim, d, m);
+    if (slb_validate_staged_tables(&cfg->gp, "filtered sweep")) return 1;
     int nomax = 1;
     for (int f = 0; f < cfg->gp.num_factors; ++f) {
         const slb_gp_factor& F = cfg->gp.factors[f];
-        SLB_CHECK(F.M == 0 || (F.Xf != nullptr && F.Whead != nullptr && F.Wheadp != nullptr &&
-                               F.Xhead != nullptr),
-                  "filtered sweep: GP factor %d lacks the filter tables (Xf / Whead / Wheadp / Xhead)", f);
+        SLB_CHECK(F.M == 0 || (F.Whead != nullptr && F.Wheadp != nullptr && F.Xhead != nullptr),
+                  "filtered sweep: GP factor %d lacks the filter tables (Whead / Wheadp / Xhead)", f);
         SLB_CHECK(F.M == 0 || ((reinterpret_cast<uintptr_t>(F.Wheadp) & 15) == 0 &&
                                (reinterpret_cast<uintptr_t>(F.Xhead) & 15) == 0),
                   "filtered sweep: GP factor %d: Wheadp / Xhead must be 16-byte aligned", f);
         SLB_CHECK(F.head_rows >= 0 && F.head_rows <= SLB_HEAD_RANK && F.head_rows <= F.M,
                   "filtered sweep: GP factor %d has %d head rows (0..min(M, %d))", f, F.head_rows,
                   SLB_HEAD_RANK);
-        SLB_CHECK((reinterpret_cast<uintptr_t>(F.Xf) & 15) == 0,
-                  "filtered sweep: GP factor %d: Xf must be 16-byte aligned", f);
         int no = 0;
         for (int o = 0; o < cfg->gp.num_outputs; ++o) no += cfg->gp.outputs[o].factor == f;
         if (no > nomax) nomax = no;
     }
-    for (int o = 0; o < cfg->gp.num_outputs; ++o) {
-        const slb_gp_output& G = cfg->gp.outputs[o];
-        SLB_CHECK(cfg->gp.factors[G.factor].M == 0 ||
-                  (G.gamma_f != nullptr && (reinterpret_cast<uintptr_t>(G.gamma_f) & 15) == 0),
-                  "filtered sweep: GP output %d has no (16-byte aligned) gamma_f", o);
-        SLB_CHECK(G.gamma_l1 >= 0.0, "filtered sweep: GP output %d has no gamma_l1", o);
-    }
+    for (int o = 0; o < cfg->gp.num_outputs; ++o)
+        SLB_CHECK(cfg->gp.outputs[o].gamma_l1 >= 0.0, "filtered sweep: GP output %d has no gamma_l1", o);
+    const int64_t n_all = idx_end - idx_begin;
+    if (n_all == 0) return 0;
+    SLB_CHECK(negative_dev != nullptr && workspace_dev != nullptr,
+              "slb_lyapunov_sweep_filtered: negative_dev and workspace_dev are required");
     cudaStream_t st = (cudaStream_t)stream;
     char* ws = static_cast<char*>(workspace_dev);
     const int64_t cap = n_all < CHUNK ? n_all : CHUNK;

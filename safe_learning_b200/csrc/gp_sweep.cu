@@ -218,28 +218,12 @@ int slb_gp_predict(void* stream, const slb_gp_stack* gp, const double* points_de
 static int sweep_common(void* stream, const slb_sweep* cfg, const double* states, int64_t n,
                         int64_t idx_begin, uint8_t* negative, double* values, double* decrease,
                         double* threshold, double* mean, double* err) {
-    SLB_CHECK(cfg != nullptr, "lyapunov sweep: null config");
+    int m;
+    if (slb_validate_sweep(cfg, states != nullptr, &m)) return 1;
     SLB_CHECK(n >= 0, "lyapunov sweep: negative point count");
     if (n == 0) return 0;
     SLB_CHECK(negative != nullptr, "lyapunov sweep: negative_dev is required");
-    if (slb_validate_grid(&cfg->grid, false)) return 1;
-    const int d = cfg->grid.ndim;
-    if (slb_validate_function(&cfg->policy, "policy", d)) return 1;
-    SLB_CHECK(cfg->policy.kind != SLB_FN_NONE, "lyapunov sweep: a policy is required");
-    if (slb_validate_function(&cfg->lyapunov, "lyapunov_function", d)) return 1;
-    SLB_CHECK(cfg->lyapunov.kind != SLB_FN_NONE, "lyapunov sweep: a Lyapunov function is required");
-    if (slb_validate_function(&cfg->lipschitz_v, "lipschitz_lyapunov", d)) return 1;
-    if (slb_validate_function(&cfg->lipschitz_f, "lipschitz_dynamics", d)) return 1;
-    SLB_CHECK(cfg->lf_values == nullptr || states == nullptr,
-              "lf_values (L_f tabulated per grid index) needs an index-range sweep");
-    const int m = (cfg->policy.flags & SLB_FLAG_NORM1) ? 1 : cfg->policy.out_dim;
-    SLB_CHECK(m >= 1 && m <= SLB_MAX_ACT, "policy output dim %d unsupported", m);
     if (cfg->gp.num_outputs > 0) {
-        if (slb_validate_gp(&cfg->gp)) return 1;
-        SLB_CHECK(cfg->gp.num_outputs == d,
-                  "GP stack has %d outputs but the state has %d dims", cfg->gp.num_outputs, d);
-        SLB_CHECK(cfg->gp.input_dim == d + m, "GP input_dim %d != state %d + action %d",
-                  cfg->gp.input_dim, d, m);
         slb_gp_args a;
         memset(&a, 0, sizeof(a));
         a.points = states; a.n = n; a.idx_begin = idx_begin;
@@ -249,8 +233,6 @@ static int sweep_common(void* stream, const slb_sweep* cfg, const double* states
         a.timing = g_timing_buffer;
         return dispatch_gp_tile((cudaStream_t)stream, *cfg, a);
     }
-    if (slb_validate_function(&cfg->dynamics, "dynamics", d + m)) return 1;
-    SLB_CHECK(cfg->dynamics.kind != SLB_FN_NONE, "lyapunov sweep: no dynamics given");
     SLB_CHECK(err == nullptr, "deterministic dynamics have no error bounds (err_dev must be NULL)");
     return slb_launch_det_sweep((cudaStream_t)stream, *cfg, states, n, idx_begin, negative, values,
                                 decrease, threshold, mean);
@@ -260,9 +242,7 @@ int slb_lyapunov_sweep(void* stream, const slb_sweep* cfg, int64_t idx_begin, in
                        uint8_t* negative_dev, double* values_dev, double* decrease_dev,
                        double* threshold_dev, double* mean_dev, double* err_dev) {
     SLB_CHECK(cfg != nullptr, "slb_lyapunov_sweep: null config");
-    SLB_CHECK(idx_begin >= 0 && idx_end >= idx_begin && idx_end <= cfg->grid.nindex,
-              "slb_lyapunov_sweep: index range [%lld, %lld) outside the grid (nindex %lld)",
-              (long long)idx_begin, (long long)idx_end, (long long)cfg->grid.nindex);
+    if (slb_validate_range("slb_lyapunov_sweep", idx_begin, idx_end, cfg->grid.nindex)) return 1;
     return sweep_common(stream, cfg, nullptr, idx_end - idx_begin, idx_begin, negative_dev,
                         values_dev, decrease_dev, threshold_dev, mean_dev, err_dev);
 }

@@ -41,6 +41,13 @@ int slb_validate_grid(const slb_grid* g, bool need_points) {
     return 0;
 }
 
+int slb_validate_range(const char* who, int64_t idx_begin, int64_t idx_end, int64_t nindex) {
+    SLB_CHECK(idx_begin >= 0 && idx_end >= idx_begin && idx_end <= nindex,
+              "%s: index range [%lld, %lld) outside the grid (nindex %lld)", who, (long long)idx_begin,
+              (long long)idx_end, (long long)nindex);
+    return 0;
+}
+
 int slb_validate_function(const slb_function* f, const char* what, int expect_in) {
     SLB_CHECK(!(f->flags & SLB_FLAG_GRADIENT) || f->kind == SLB_FN_TRIANGULATION,
               "%s: the gradient flag is only defined for Triangulation", what);
@@ -115,6 +122,28 @@ int slb_validate_function(const slb_function* f, const char* what, int expect_in
     return 0;
 }
 
+// The columns eval_fn (common.cuh) returns for f: the kind's count, then 1 after NORM1 / MAXABS.
+// Host code sizes kernels and checks shapes with this number and never with out_dim: a change to
+// eval_fn's return value must be made here too.
+int slb_fn_columns(const slb_function& f) {
+    if (f.flags & (SLB_FLAG_NORM1 | SLB_FLAG_MAXABS)) return 1;
+    switch (f.kind) {
+    case SLB_FN_QUADRATIC: case SLB_FN_LYAPUNOV_NN: return 1;
+    case SLB_FN_PENDULUM: return 2;
+    case SLB_FN_CARTPOLE: return 4;
+    default: return f.out_dim;
+    }
+}
+
+// deterministic dynamics: [x, u] (d + m inputs) -> the next state (d columns)
+int slb_validate_dynamics(const slb_function* f, const char* who, int d, int m) {
+    if (slb_validate_function(f, "dynamics", d + m)) return 1;
+    SLB_CHECK(f->kind != SLB_FN_NONE, "%s: no dynamics given", who);
+    SLB_CHECK(slb_fn_columns(*f) == d, "%s: dynamics return %d columns, the state has %d", who,
+              slb_fn_columns(*f), d);
+    return 0;
+}
+
 int slb_validate_gp(const slb_gp_stack* gp) {
     if (gp->num_outputs == 0) return 0;
     SLB_CHECK(gp->num_outputs >= 1 && gp->num_outputs <= SLB_MAX_OUT, "GP outputs %d outside 1..%d",
@@ -158,6 +187,49 @@ int slb_validate_gp(const slb_gp_stack* gp) {
     return 0;
 }
 
+// The staged GP mean (gp_mean_staged.cuh) copies Xf of every factor and gamma_f of every output by
+// TMA bulk copies: wherever a factor has training points they must be present and 16-byte aligned.
+int slb_validate_staged_tables(const slb_gp_stack* gp, const char* who) {
+    auto aligned = [](const double* p) { return p != nullptr && (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
+    for (int f = 0; f < gp->num_factors; ++f)
+        SLB_CHECK(gp->factors[f].M == 0 || aligned(gp->factors[f].Xf),
+                  "%s: GP factor %d lacks the (16-byte aligned) staged table Xf", who, f);
+    for (int o = 0; o < gp->num_outputs; ++o)
+        SLB_CHECK(gp->factors[gp->outputs[o].factor].M == 0 || aligned(gp->outputs[o].gamma_f),
+                  "%s: GP output %d lacks the (16-byte aligned) staged table gamma_f", who, o);
+    return 0;
+}
+
+int slb_validate_sweep(const slb_sweep* cfg, bool explicit_states, int* m_out) {
+    SLB_CHECK(cfg != nullptr, "lyapunov sweep: null config");
+    if (slb_validate_grid(&cfg->grid, false)) return 1;
+    const int d = cfg->grid.ndim;
+    if (slb_validate_function(&cfg->policy, "policy", d)) return 1;
+    SLB_CHECK(cfg->policy.kind != SLB_FN_NONE, "lyapunov sweep: a policy is required");
+    if (slb_validate_function(&cfg->lyapunov, "lyapunov_function", d)) return 1;
+    SLB_CHECK(cfg->lyapunov.kind != SLB_FN_NONE, "lyapunov sweep: a Lyapunov function is required");
+    if (slb_validate_function(&cfg->lipschitz_v, "lipschitz_lyapunov", d)) return 1;
+    const int nl = slb_fn_columns(cfg->lipschitz_v);
+    SLB_CHECK(cfg->lipschitz_v.kind == SLB_FN_NONE || nl == 1 || nl == d,
+              "lyapunov sweep: lipschitz_lyapunov returns %d columns, expected 1 or the state's %d", nl, d);
+    if (slb_validate_function(&cfg->lipschitz_f, "lipschitz_dynamics", d)) return 1;
+    SLB_CHECK(cfg->lf_values == nullptr || !explicit_states,
+              "lf_values (L_f tabulated per grid index) needs an index-range sweep");
+    const int m = slb_fn_columns(cfg->policy);
+    SLB_CHECK(m >= 1 && m <= SLB_MAX_ACT, "policy output dim %d unsupported", m);
+    if (cfg->gp.num_outputs > 0) {
+        if (slb_validate_gp(&cfg->gp)) return 1;
+        SLB_CHECK(cfg->gp.num_outputs == d,
+                  "GP stack has %d outputs but the state has %d dims", cfg->gp.num_outputs, d);
+        SLB_CHECK(cfg->gp.input_dim == d + m, "GP input_dim %d != state %d + action %d",
+                  cfg->gp.input_dim, d, m);
+    } else if (slb_validate_dynamics(&cfg->dynamics, "lyapunov sweep", d, m)) {
+        return 1;
+    }
+    *m_out = m;
+    return 0;
+}
+
 int slb_validate_bellman(const slb_bellman* cfg, int* m_out) {
     SLB_CHECK(cfg != nullptr, "bellman: null config");
     if (slb_validate_grid(&cfg->grid, false)) return 1;
@@ -169,7 +241,7 @@ int slb_validate_bellman(const slb_bellman* cfg, int* m_out) {
     } else {
         if (slb_validate_function(&cfg->policy, "policy", d)) return 1;
         SLB_CHECK(cfg->policy.kind != SLB_FN_NONE, "bellman: a policy is required");
-        m = cfg->policy.out_dim;
+        m = slb_fn_columns(cfg->policy);
         SLB_CHECK(m >= 1 && m <= SLB_MAX_ACT, "bellman: policy output dim %d unsupported", m);
     }
     if (cfg->gp.num_outputs > 0) {
@@ -177,22 +249,18 @@ int slb_validate_bellman(const slb_bellman* cfg, int* m_out) {
         SLB_CHECK(cfg->gp.num_outputs == d && cfg->gp.input_dim == d + m,
                   "bellman: GP stack shape (%d outputs, %d inputs) does not match state %d + action %d",
                   cfg->gp.num_outputs, cfg->gp.input_dim, d, m);
-        for (int o = 0; o < cfg->gp.num_outputs; ++o) {
-            const slb_gp_output& G = cfg->gp.outputs[o];
-            const slb_gp_factor& F = cfg->gp.factors[G.factor];
-            SLB_CHECK(F.M == 0 || (G.gamma_f != nullptr && F.Xf != nullptr &&
-                                   (reinterpret_cast<uintptr_t>(G.gamma_f) & 15) == 0 &&
-                                   (reinterpret_cast<uintptr_t>(F.Xf) & 15) == 0),
-                      "bellman: GP output %d lacks the (16-byte aligned) staged tables Xf / gamma_f", o);
-        }
-    } else {
-        if (slb_validate_function(&cfg->dynamics, "dynamics", d + m)) return 1;
-        SLB_CHECK(cfg->dynamics.kind != SLB_FN_NONE, "bellman: no dynamics given");
+        if (slb_validate_staged_tables(&cfg->gp, "bellman")) return 1;
+    } else if (slb_validate_dynamics(&cfg->dynamics, "bellman", d, m)) {
+        return 1;
     }
     if (slb_validate_function(&cfg->reward, "reward_function", d + m)) return 1;
     SLB_CHECK(cfg->reward.kind != SLB_FN_NONE, "bellman: a reward function is required");
+    SLB_CHECK(slb_fn_columns(cfg->reward) == 1, "bellman: reward_function returns %d columns, expected 1",
+              slb_fn_columns(cfg->reward));
     if (slb_validate_function(&cfg->value, "value_function", d)) return 1;
     SLB_CHECK(cfg->value.kind != SLB_FN_NONE, "bellman: a value function is required");
+    SLB_CHECK(slb_fn_columns(cfg->value) == 1, "bellman: value_function returns %d columns, expected 1",
+              slb_fn_columns(cfg->value));
     *m_out = m;
     return 0;
 }
@@ -881,10 +949,8 @@ int slb_eval_function(void* stream, const slb_function* fn, const double* points
     SLB_CHECK(n >= 0, "slb_eval_function: negative n");
     if (n == 0) return 0;
     SLB_CHECK(points_dev && out_dev, "slb_eval_function: null buffer");
-    int ncols = (fn->flags & (SLB_FLAG_NORM1 | SLB_FLAG_MAXABS)) ? 1 : fn->out_dim;
-    if (fn->kind == SLB_FN_QUADRATIC || fn->kind == SLB_FN_LYAPUNOV_NN) ncols = 1;
     eval_function_kernel<<<blocks_for(n), LT, 0, (cudaStream_t)stream>>>(*fn, points_dev, n, out_dev,
-                                                                        ncols);
+                                                                        slb_fn_columns(*fn));
     SLB_LAUNCH_CHECK();
     return 0;
 }
@@ -893,9 +959,7 @@ int slb_index_to_state(void* stream, const slb_grid* grid, int64_t idx_begin, in
                        double* states_dev) {
     SLB_CHECK(grid != nullptr, "slb_index_to_state: null grid");
     if (slb_validate_grid(grid, false)) return 1;
-    SLB_CHECK(idx_begin >= 0 && idx_end >= idx_begin && idx_end <= grid->nindex,
-              "slb_index_to_state: range [%lld, %lld) outside the grid", (long long)idx_begin,
-              (long long)idx_end);
+    if (slb_validate_range("slb_index_to_state", idx_begin, idx_end, grid->nindex)) return 1;
     const int64_t n = idx_end - idx_begin;
     if (n == 0) return 0;
     SLB_CHECK(states_dev != nullptr, "slb_index_to_state: null output");
@@ -909,8 +973,7 @@ int slb_bellman_sweep(void* stream, const slb_bellman* cfg, int64_t idx_begin, i
                       double* out_dev) {
     int m;
     if (slb_validate_bellman(cfg, &m)) return 1;
-    SLB_CHECK(idx_begin >= 0 && idx_end >= idx_begin && idx_end <= cfg->grid.nindex,
-              "slb_bellman_sweep: range outside the grid");
+    if (slb_validate_range("slb_bellman_sweep", idx_begin, idx_end, cfg->grid.nindex)) return 1;
     const int64_t n = idx_end - idx_begin;
     if (n == 0) return 0;
     SLB_CHECK(out_dev != nullptr, "slb_bellman_sweep: null output");
@@ -949,8 +1012,7 @@ int slb_bellman_argmax(void* stream, const slb_bellman* cfg, int64_t idx_begin, 
     int m;
     if (slb_validate_bellman(cfg, &m)) return 1;
     SLB_CHECK(n_actions >= 1 && actions_dev != nullptr, "slb_bellman_argmax: no actions");
-    SLB_CHECK(idx_begin >= 0 && idx_end >= idx_begin && idx_end <= cfg->grid.nindex,
-              "slb_bellman_argmax: range outside the grid");
+    if (slb_validate_range("slb_bellman_argmax", idx_begin, idx_end, cfg->grid.nindex)) return 1;
     const int64_t n = idx_end - idx_begin;
     if (n == 0) return 0;
     SLB_CHECK(best_dev != nullptr, "slb_bellman_argmax: null output");

@@ -256,17 +256,6 @@ int rollout_block(int64_t n) {
     return bs;
 }
 
-// columns a fused function returns (eval_fn's return value)
-int fn_columns(const slb_function& f) {
-    if (f.flags & (SLB_FLAG_NORM1 | SLB_FLAG_MAXABS)) return 1;
-    switch (f.kind) {
-    case SLB_FN_QUADRATIC: case SLB_FN_LYAPUNOV_NN: return 1;
-    case SLB_FN_PENDULUM: return 2;
-    case SLB_FN_CARTPOLE: return 4;
-    default: return f.out_dim;
-    }
-}
-
 int validate_rollout(const char* who, const slb_bellman* cfg, const double* states_dev, int64_t idx_begin,
                      int64_t n, int32_t horizon, bool reward) {
     SLB_CHECK(cfg != nullptr, "%s: null config", who);
@@ -278,23 +267,18 @@ int validate_rollout(const char* who, const slb_bellman* cfg, const double* stat
     SLB_CHECK(horizon >= 0, "%s: negative horizon %d", who, horizon);
     if (states_dev == nullptr) {
         if (slb_validate_grid(&cfg->grid, false)) return 1;
-        SLB_CHECK(idx_begin >= 0 && idx_begin + n <= cfg->grid.nindex,
-                  "%s: index range [%lld, %lld) outside the grid", who, (long long)idx_begin,
-                  (long long)(idx_begin + n));
+        if (slb_validate_range(who, idx_begin, idx_begin + n, cfg->grid.nindex)) return 1;
     }
     if (slb_validate_function(&cfg->policy, "policy", d)) return 1;
     SLB_CHECK(cfg->policy.kind != SLB_FN_NONE, "%s: a policy is required", who);
-    const int m = fn_columns(cfg->policy);
+    const int m = slb_fn_columns(cfg->policy);
     SLB_CHECK(m >= 1 && d + m <= SLB_MAX_IN, "%s: state %d + action %d exceeds %d inputs", who, d, m,
               SLB_MAX_IN);
-    if (slb_validate_function(&cfg->dynamics, "dynamics", d + m)) return 1;
-    SLB_CHECK(cfg->dynamics.kind != SLB_FN_NONE, "%s: no dynamics given", who);
-    SLB_CHECK(fn_columns(cfg->dynamics) == d, "%s: dynamics return %d columns, the state has %d", who,
-              fn_columns(cfg->dynamics), d);
+    if (slb_validate_dynamics(&cfg->dynamics, who, d, m)) return 1;
     if (reward) {
         if (slb_validate_function(&cfg->reward, "reward_function", d + m)) return 1;
         SLB_CHECK(cfg->reward.kind != SLB_FN_NONE, "%s: a reward function is required", who);
-        SLB_CHECK(fn_columns(cfg->reward) == 1, "%s: the reward must return one column", who);
+        SLB_CHECK(slb_fn_columns(cfg->reward) == 1, "%s: the reward must return one column", who);
     }
     return 0;
 }

@@ -352,6 +352,13 @@ value_solve_coop_kernel(const solve_args a, const IDX* __restrict__ cols, const 
 
 static bool wide_index(int64_t nindex) { return nindex > 0x7fffffffll; }
 
+// the rows of T are the barycentric weights of a one-output Triangulation (projection allowed)
+static int validate_value_table(const slb_function& value, const char* who) {
+    SLB_CHECK(value.kind == SLB_FN_TRIANGULATION && value.out_dim == 1 && !(value.flags & ~SLB_FLAG_PROJECT),
+              "%s: the value function must be a plain one-output Triangulation", who);
+    return 0;
+}
+
 template <typename IDX>
 static int launch_solve(cudaStream_t st, const solve_args& a, const void* cols, const double* W,
                         const double* R, double* v, void* workspace, unsigned long long* stats) {
@@ -392,11 +399,8 @@ int slb_value_operator(void* stream, const slb_bellman* cfg, int64_t idx_begin, 
     int m;
     if (slb_validate_bellman(cfg, &m)) return 1;
     SLB_CHECK(!cfg->fixed_action, "slb_value_operator: the policy is evaluated, fixed_action must be 0");
-    SLB_CHECK(cfg->value.kind == SLB_FN_TRIANGULATION && cfg->value.out_dim == 1 &&
-              !(cfg->value.flags & ~SLB_FLAG_PROJECT),
-              "slb_value_operator: the value function must be a plain one-output Triangulation");
-    SLB_CHECK(idx_begin >= 0 && idx_end >= idx_begin && idx_end <= cfg->grid.nindex,
-              "slb_value_operator: range outside the grid");
+    if (validate_value_table(cfg->value, "slb_value_operator")) return 1;
+    if (slb_validate_range("slb_value_operator", idx_begin, idx_end, cfg->grid.nindex)) return 1;
     SLB_CHECK(stats_dev != nullptr, "slb_value_operator: null stats");
     const int64_t n = idx_end - idx_begin;
     cudaStream_t st = (cudaStream_t)stream;
@@ -431,9 +435,7 @@ int slb_value_operator_points(void* stream, const slb_function* value, const dou
                               int64_t n, void* cols_dev, double* weights_dev, uint64_t* stats_dev) {
     SLB_CHECK(value != nullptr, "slb_value_operator_points: null value function");
     if (slb_validate_function(value, "value_function", 0)) return 1;
-    SLB_CHECK(value->kind == SLB_FN_TRIANGULATION && value->out_dim == 1 &&
-              !(value->flags & ~SLB_FLAG_PROJECT),
-              "slb_value_operator_points: the value function must be a plain one-output Triangulation");
+    if (validate_value_table(*value, "slb_value_operator_points")) return 1;
     SLB_CHECK(n >= 0, "slb_value_operator_points: negative n");
     SLB_CHECK(stats_dev != nullptr, "slb_value_operator_points: null stats");
     cudaStream_t st = (cudaStream_t)stream;
