@@ -18,7 +18,7 @@ OBJDIR = os.path.join(CSRC, "build")
 OUTPUT = os.path.join(HERE, "libslb200.so")
 HEADER = os.path.join(HERE, "..", "include", "slb200.h")
 
-# (object name, source, extra flags, headers it depends on besides common.cuh / slb200.h)
+# (object name, source, extra flags, headers it depends on besides common.cuh / exp2_tab64.h / slb200.h)
 UNITS = [("gp_tile_%d_%d.o" % (d, tp), "gp_tile_inst.cu", ["-DSLB_TILE_DIN=%d" % d, "-DSLB_TP=%d" % tp],
           ["gp_tile.cuh", "gp_args.h"]) for d in range(1, 7) for tp in (64, 32)]
 UNITS += [("gp_sweep.o", "gp_sweep.cu", [], ["gp_args.h"]),
@@ -42,7 +42,8 @@ def _mtime(path):
 def _unit_stale(unit):
     obj, src, _, headers = unit
     built = _mtime(os.path.join(OBJDIR, obj))
-    deps = [os.path.join(CSRC, src), os.path.join(CSRC, "common.cuh"), HEADER, os.path.abspath(__file__)]
+    deps = [os.path.join(CSRC, src), os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "exp2_tab64.h"),
+            HEADER, os.path.abspath(__file__)]
     deps += [os.path.join(CSRC, h) for h in headers]
     return built == 0.0 or any(_mtime(d) > built for d in deps)
 

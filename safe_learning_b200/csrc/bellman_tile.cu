@@ -340,11 +340,7 @@ int slb_launch_argmax_factored(cudaStream_t st, const slb_bellman& cfg, int64_t 
         a.gpack[o] = ws;
         ws += total;
     }
-    switch (d) {
-    case 1: return launch_argmax_tile<1>(st, cfg, a);
-    case 2: return launch_argmax_tile<2>(st, cfg, a);
-    default:
-        slb_set_error("factored argmax: state dimension %d not compiled (1..2)", d);
-        return 1;
-    }
+    return slb_dispatch_dim<1, 2>(d, "factored argmax: state dimension", [&](auto D) {
+        return launch_argmax_tile<D>(st, cfg, a);
+    });
 }

@@ -13,7 +13,10 @@
 #include <stdint.h>
 #include <math.h>
 
+#include <type_traits>
+
 #include "../../include/slb200.h"
+#include "exp2_tab64.h"
 
 // SMs of the target GPU (H100 SXM, sm_90a): the CTA count of one full wave of the one-CTA-per-SM
 // launches (head stage, persistent refine tiles, L2 prefetch of the packed factors)
@@ -54,6 +57,17 @@ int slb_validate_range(const char* who, int64_t idx_begin, int64_t idx_end, int6
 // validates an slb_sweep descriptor (explicit_states: a sweep of a state list), *m_out = action dimension
 int slb_validate_sweep(const slb_sweep* cfg, bool explicit_states, int* m_out);
 
+// Runs the kernel instantiation of a runtime dimension d: returns launch(std::integral_constant<int,
+// d>{}) for d in the compiled range [LO, HI], else the error "<what> <d> not compiled (LO..HI)".
+template <int LO, int HI, class F>
+int slb_dispatch_dim(int d, const char* what, F&& launch) {
+    SLB_CHECK(d >= LO && d <= HI, "%s %d not compiled (%d..%d)", what, d, LO, HI);
+    if constexpr (LO < HI) {
+        if (d > LO) return slb_dispatch_dim<LO + 1, HI>(d, what, launch);
+    }
+    return launch(std::integral_constant<int, LO>{});
+}
+
 // ----------------------------------------------------------------------------- device side
 #define SLB_DEV __device__ __forceinline__
 
@@ -73,57 +87,11 @@ SLB_DEV double key_value(uint64_t k) {
     return __longlong_as_double((long long)b);
 }
 
-// exp(x) for x <= 0, <= 1 ulp (checked against glibc on 2e7 points, tools/exp_neg_check.c):
-// Cody-Waite reduction x = k ln2 + r, |r| <= ln2/2, degree-13 Taylor polynomial, 2^k by exponent
-// add.  Branch-free so four evaluations interleave in the k-row generation loop; anything
-// below exp(-700) flushes to 0 (it only ever multiplies finite L^-1 entries).
-SLB_DEV double exp_neg(double x) {
-    const double MAGIC = 6755399441055744.0;             // 1.5 * 2^52
-    const double t = fma(x, 1.4426950408889634074, MAGIC);
-    const int k = __double2loint(t);
-    const double kd = t - MAGIC;
-    double r = fma(kd, -6.93147180369123816490e-01, x);
-    r = fma(kd, -1.90821492927058770002e-10, r);
-    double p = 1.0 / 6227020800.0;
-    p = fma(p, r, 1.0 / 479001600.0);
-    p = fma(p, r, 1.0 / 39916800.0);
-    p = fma(p, r, 1.0 / 3628800.0);
-    p = fma(p, r, 1.0 / 362880.0);
-    p = fma(p, r, 1.0 / 40320.0);
-    p = fma(p, r, 1.0 / 5040.0);
-    p = fma(p, r, 1.0 / 720.0);
-    p = fma(p, r, 1.0 / 120.0);
-    p = fma(p, r, 1.0 / 24.0);
-    p = fma(p, r, 1.0 / 6.0);
-    p = fma(p, r, 0.5);
-    p = fma(p, r, 1.0);
-    p = fma(p, r, 1.0);
-    p = __hiloint2double(__double2hiint(p) + (k << 20), __double2loint(p));
-    return x < -700.0 ? 0.0 : p;
-}
-
-// Table-driven exp(x) for x <= 0 (<= 1 ulp against glibc on 2e7 points, tools/exp_neg_check.c):
+// Table-driven exp(x) for x <= 0 (<= 1 ulp against glibc on 2e7 points, tools/exp_neg_tab_check.c):
 // x = (64 k + j) ln2/64 + r, |r| <= ln2/128;  exp(x) = 2^k * T[j] * (1 + r + ... + r^5/120).
-// 10 fp64 operations instead of 17; T (64 correctly rounded doubles) is read from a shared-memory
+// 10 fp64 operations; T (64 correctly rounded doubles) is read from a shared-memory
 // copy because the index differs per lane (constant memory would serialise).
-__constant__ double c_exp2_tab[64] = {
-    1.0, 1.0108892860517005, 1.0218971486541166, 1.0330248790212284,
-    1.0442737824274138, 1.0556451783605572, 1.0671404006768237, 1.0787607977571199,
-    1.0905077326652577, 1.102382583307841, 1.1143867425958924, 1.1265216186082418,
-    1.1387886347566916, 1.1511892299529827, 1.1637248587775775, 1.1763969916502812,
-    1.189207115002721, 1.202156731452703, 1.215247359980469, 1.22848053610687,
-    1.241857812073484, 1.255380757024691, 1.2690509571917332, 1.2828700160787783,
-    1.2968395546510096, 1.3109612115247644, 1.3252366431597413, 1.339667524053303,
-    1.3542555469368927, 1.3690024229745905, 1.383909881963832, 1.3989796725383112,
-    1.4142135623730951, 1.42961333839197, 1.4451808069770467, 1.460917794180647,
-    1.4768261459394993, 1.4929077282912648, 1.5091644275934228, 1.5255981507445384,
-    1.5422108254079407, 1.559004400237837, 1.5759808451078865, 1.593142151342267,
-    1.6104903319492543, 1.6280274218573478, 1.645755478153965, 1.6636765803267364,
-    1.681792830507429, 1.7001063537185235, 1.718619298122478, 1.7373338352737062,
-    1.7562521603732995, 1.7753764925265212, 1.7947090750031072, 1.8142521755003989,
-    1.8340080864093424, 1.8539791250833855, 1.8741676341103, 1.8945759815869656,
-    1.9152065613971474, 1.9360617934922943, 1.9571441241754002, 1.978456026387951
-};
+__constant__ double c_exp2_tab[64] = {SLB_EXP2_TAB64};
 
 SLB_DEV void load_exp_table(double* tab_smem) {
     for (int i = threadIdx.x; i < 64; i += blockDim.x) tab_smem[i] = c_exp2_tab[i];
@@ -324,76 +292,21 @@ SLB_DEV double fmod_exact_pos(double a, double b) {
 }
 
 // ---- Triangulation (functions.py:1103-1158 lookup, :1473-1499 evaluation) ----------------
-// Simplex of the unit cell for unit coordinates `unit`: the first simplex whose barycentric weights
-// are all >= -tol, else the one with the largest smallest weight.  `skip`: return `best` unsearched.
-SLB_DEV int tri_find_simplex(const slb_function& f, const double* unit, int best = 0, bool skip = false) {
-    const slb_grid& g = f.grid;
-    const int d = g.ndim;
-    double best_min = -1e300;
-    for (int s = 0; s < f.nsimplex && !skip; ++s) {
-        const int64_t v0 = f.unit_simplices[s * (d + 1)];
-        double o[SLB_MAX_DIM];
-        if (g.nindex <= 0x7fffffffll) {        // 32-bit index arithmetic (same integers)
-            unsigned t = (unsigned)v0;
-            for (int c = d - 1; c >= 0; --c) {
-                const unsigned n = (unsigned)g.num_points[c];
-                const unsigned qq = t / n;
-                o[c] = (double)(t - qq * n) * g.unit_maxes[c];
-                t = qq;
-            }
-        } else {
-            int64_t t = v0;
-            for (int c = d - 1; c >= 0; --c) {
-                o[c] = (double)(t % g.num_points[c]) * g.unit_maxes[c];
-                t /= g.num_points[c];
-            }
-        }
-        const double* H = f.hyperplanes + (size_t)s * d * d;
-        double wsum = 0.0, wmin = 1e300;
-        for (int c = 0; c < d; ++c) {
-            double w = 0.0;
-            for (int k = 0; k < d; ++k) w += (unit[k] - o[k]) * H[k * d + c];
-            wsum += w;
-            wmin = fmin(wmin, w);
-        }
-        wmin = fmin(wmin, 1.0 - wsum);
-        if (wmin > best_min) { best_min = wmin; best = s; }
-        if (wmin >= -1e-12) break;
-    }
-    return best;
-}
+// The one lookup of the point xin in the Triangulation f, in three forms:
+//   TRI_EVAL     f(xin), or its gradient, into out (every function object inlines this form);
+//   TRI_WEIGHTS  stops after the barycentric weights: out = w[0..d], *corner = the rectangle's lowest
+//                vertex, *simplex = the simplex (the rows of the value operator, value_opt.cu);
+//   TRI_CELL     as TRI_WEIGHTS, but searches the simplex from unit coordinates taken relative to the
+//                rectangle's own lowest vertex (clipped xin - that vertex): the value operator's
+//                repair of rows whose `% unit_maxes` picked a simplex on the wrong side of the cell.
+// The forms differ in `if constexpr` blocks only, so that TRI_EVAL compiles to this code written out
+// by itself: routing it through helper functions changed register allocation (and added spills) in
+// the kernels that inline it.
+enum { TRI_EVAL, TRI_WEIGHTS, TRI_CELL };
 
-// Barycentric weights w[0..d] of the point xin (clipped to the limits when projected) in simplex
-// `s` of the rectangle whose lowest vertex is `corner`   (:1479-1491)
-SLB_DEV void tri_barycentric(const slb_function& f, const double* xin, int64_t corner, int s,
-                             double* w) {
-    const slb_grid& g = f.grid;
-    const int d = g.ndim;
-    const int64_t* simp = f.unit_simplices + (size_t)s * (d + 1);
-    const double* H = f.hyperplanes + (size_t)s * d * d;
-    double origin[SLB_MAX_DIM], off[SLB_MAX_DIM];
-    grid_index_to_state(g, simp[0] + corner, origin);
-    for (int c = 0; c < d; ++c) {
-        double xc = xin[c];
-        if (f.flags & SLB_FLAG_PROJECT) xc = fmin(fmax(xc, g.offset[c]), g.upper[c]);
-        off[c] = f64sub(xc, origin[c]);
-    }
-    for (int c = 0; c < d; ++c) {
-        double acc = f64mul(off[0], H[c]);
-        for (int k = 1; k < d; ++k) acc = f64add(acc, f64mul(off[k], H[k * d + c]));
-        w[c + 1] = acc;
-    }
-    double acc = w[1];
-    for (int c = 2; c <= d; ++c) acc = f64add(acc, w[c]);
-    w[0] = f64sub(1.0, acc);
-}
-
-// The reference's lookup of xin: rectangle (lowest vertex -> *corner_out), simplex (returned) and
-// barycentric weights w[0..d] -- eval_triangulation's lookup operation for operation.  The value
-// operator (value_opt.cu) builds its rows from it; eval_triangulation keeps its own inline copy
-// because routing it through these helpers changes register allocation (and adds spills) in the
-// filter, argmax-tile and rollout kernels that inline it.
-SLB_DEV int tri_locate(const slb_function& f, const double* xin, int64_t* corner_out, double* w) {
+template <int FORM>
+SLB_DEV void tri_lookup(const slb_function& f, const double* xin, double* out, int64_t* corner_out = nullptr,
+                        int* simplex_out = nullptr) {
     const slb_grid& g = f.grid;
     const int d = g.ndim;
     const double eps = 2.220446049250313e-16;
@@ -423,45 +336,11 @@ SLB_DEV int tri_locate(const slb_function& f, const double* xin, int64_t* corner
         else all_clipped = false;
         unit[c] = fmod_exact_pos(cen, g.unit_maxes[c]);
     }
-    // simplex inside the unit cell; weights with the ORIGINAL (optionally projected) point
-    const bool tabled = all_clipped && f.corner_simplex != nullptr;
-    const int best = tri_find_simplex(f, unit, tabled ? f.corner_simplex[pattern] : 0, tabled);
-    *corner_out = corner;
-    tri_barycentric(f, xin, corner, best, w);
-    return best;
-}
-
-// The lookup below is restated, operation for operation, by tri_locate / tri_find_simplex /
-// tri_barycentric above (used by the value operator); a change here must be made there too.
-SLB_DEV void eval_triangulation(const slb_function& f, const double* xin, double* out) {
-    const slb_grid& g = f.grid;
-    const int d = g.ndim;
-    const double eps = 2.220446049250313e-16;
-    double unit[SLB_MAX_DIM];
-    int64_t corner = 0;
-    int poff = 0;
-    int pattern = 0;
-    bool all_clipped = true;
-    for (int c = 0; c < d; ++c) {
-        const double* pts = g.discrete_points + poff;
-        const int n = (int)g.num_points[c];
-        poff += n;
-        const double xc = xin[c];
-        // np.digitize(x, pts) - 1 clipped to [0, n-2]   (functions.py:771-773)
-        int k = (int)floor((xc - g.offset[c]) / g.unit_maxes[c]);
-        k = k < 0 ? 0 : (k > n - 1 ? n - 1 : k);
-        while (k + 1 <= n - 1 && pts[k + 1] <= xc) ++k;
-        while (k >= 0 && pts[k] > xc) --k;            // k = -1 when x < pts[0]
-        k = k < 0 ? 0 : (k > n - 2 ? n - 2 : k);
-        corner = corner * g.num_points[c] + k;        // rectangle_corner_index (:800-817)
-        // _center_states(clip=True) % unit_maxes          (:691-712, :1120-1123)
-        double cen = f64sub(xc, g.offset[c]);
-        const double lo = 2.0 * eps;
-        const double hi = f64sub(f64sub(g.upper[c], g.offset[c]), 2.0 * eps);
-        if (cen < lo) cen = lo;
-        else if (cen > hi) { cen = hi; pattern |= 1 << c; }
-        else all_clipped = false;
-        unit[c] = fmod_exact_pos(cen, g.unit_maxes[c]);
+    if constexpr (FORM == TRI_CELL) {
+        double base[SLB_MAX_DIM];
+        grid_index_to_state(g, corner, base);
+        for (int c = 0; c < d; ++c) unit[c] = f64sub(fmin(fmax(xin[c], g.offset[c]), g.upper[c]), base[c]);
+        all_clipped = false;
     }
     // simplex inside the unit cell: first simplex whose barycentric weights are all >= -tol
     int best = 0;
@@ -517,6 +396,12 @@ SLB_DEV void eval_triangulation(const slb_function& f, const double* xin, double
     double acc = w[1];
     for (int c = 2; c <= d; ++c) acc = f64add(acc, w[c]);
     w[0] = f64sub(1.0, acc);
+    if constexpr (FORM != TRI_EVAL) {
+        for (int c = 0; c <= d; ++c) out[c] = w[c];
+        *corner_out = corner;
+        *simplex_out = best;
+        return;
+    }
     if (f.flags & SLB_FLAG_GRADIENT) {
         // Triangulation.gradient (:1260-1326): weights[k][0] = -sum_c H[k][c], weights[k][1 + c] =
         // H[k][c]; d/dx_k = sum_v weights[k][v] * value[vertex v]   (one output column)
@@ -682,7 +567,7 @@ SLB_EVAL_ATTR int eval_fn(const slb_function& f, const double* in, double* out) 
         break;
     }
     case SLB_FN_TRIANGULATION:
-        eval_triangulation(f, in, out);
+        tri_lookup<TRI_EVAL>(f, in, out);
         break;
     case SLB_FN_PENDULUM:
         eval_pendulum(f, in, out); od = 2;

@@ -951,18 +951,9 @@ int slb_lyapunov_sweep_filtered(void* stream, const slb_sweep* cfg, int64_t idx_
         a.n = n; a.idx_begin = idx_begin + off;
         a.negative = negative_dev + off;
         a.values = values_dev ? values_dev + off : nullptr;
-        int rc;
-        switch (din) {
-        case 1: rc = launch_filter<1>(st, *cfg, a, smem); break;
-        case 2: rc = launch_filter<2>(st, *cfg, a, smem); break;
-        case 3: rc = launch_filter<3>(st, *cfg, a, smem); break;
-        case 4: rc = launch_filter<4>(st, *cfg, a, smem); break;
-        case 5: rc = launch_filter<5>(st, *cfg, a, smem); break;
-        case 6: rc = launch_filter<6>(st, *cfg, a, smem); break;
-        default:
-            slb_set_error("GP input_dim %d not compiled (1..6)", din);
-            return 1;
-        }
+        int rc = slb_dispatch_dim<1, 6>(din, "GP input_dim", [&](auto D) {
+            return launch_filter<D>(st, *cfg, a, smem);
+        });
         if (rc) return rc;
         if (!(g_filter_stages & 2)) continue;
         rc = slb_launch_refine(st, *cfg, n, idx_begin + off, a.list_b, a.counts + 1,

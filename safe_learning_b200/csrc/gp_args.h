@@ -33,4 +33,9 @@ struct slb_gp_args {
     long long* timing;      // diagnostics: [tile][warp][8]: cycles in {generate, contract, epilogue, total}, globaltimer ns {start, end}, cycles waiting at barriers, 0
 };
 
+// The GP tile kernel for input dimension DIN and TPV points per CTA.  Each (DIN, TPV) is instantiated
+// in a translation unit of its own (gp_tile_inst.cu), so each has a symbol of its own: templates of
+// gp_tile.cuh's unnamed namespace are weak symbols shared by all units of that source file.
+template <int DIN, int TPV>
+int slb_gp_tile_launch(cudaStream_t st, const slb_sweep& cfg, const slb_gp_args& a, bool kexpr, bool timing);
 

@@ -7,13 +7,6 @@
 
 #include "gp_args.h"
 
-#define SLB_DECLARE_TILE(d) \
-    int slb_gp_tile_launch_##d##_64(cudaStream_t, const slb_sweep&, const slb_gp_args&, bool, bool); \
-    int slb_gp_tile_launch_##d##_32(cudaStream_t, const slb_sweep&, const slb_gp_args&, bool, bool);
-SLB_DECLARE_TILE(1) SLB_DECLARE_TILE(2) SLB_DECLARE_TILE(3)
-SLB_DECLARE_TILE(4) SLB_DECLARE_TILE(5) SLB_DECLARE_TILE(6)
-#undef SLB_DECLARE_TILE
-
 namespace {
 
 // Packed factor: for 8-row block b and k-step PAIR kp <= b, 32 lanes x 2 doubles: lane T holds
@@ -63,18 +56,10 @@ int dispatch_gp_tile(cudaStream_t st, const slb_sweep& cfg, const slb_gp_args& a
     const bool timing = a.timing != nullptr;
     bool kexpr = false;
     for (int f = 0; f < cfg.gp.num_factors; ++f) kexpr |= cfg.gp.factors[f].kernel.num_prims > 0;
-#define SLB_TILE_CASE(d)                                                                   \
-    case d:                                                                                \
-        return tp == 64 ? slb_gp_tile_launch_##d##_64(st, cfg, a, kexpr, timing)           \
-                        : slb_gp_tile_launch_##d##_32(st, cfg, a, kexpr, timing);
-    switch (cfg.gp.input_dim) {
-        SLB_TILE_CASE(1) SLB_TILE_CASE(2) SLB_TILE_CASE(3)
-        SLB_TILE_CASE(4) SLB_TILE_CASE(5) SLB_TILE_CASE(6)
-#undef SLB_TILE_CASE
-    default:
-        slb_set_error("GP input_dim %d not compiled (1..6)", cfg.gp.input_dim);
-        return 1;
-    }
+    return slb_dispatch_dim<1, 6>(cfg.gp.input_dim, "GP input_dim", [&](auto D) {
+        return tp == 64 ? slb_gp_tile_launch<D, 64>(st, cfg, a, kexpr, timing)
+                        : slb_gp_tile_launch<D, 32>(st, cfg, a, kexpr, timing);
+    });
 }
 
 }  // namespace

@@ -765,6 +765,21 @@ pivoted_subset_kernel(const double* __restrict__ K, int M, int r, int64_t* __res
 
 inline unsigned blocks_for(int64_t n) { return (unsigned)((n + LT - 1) / LT); }
 
+// The thread-per-point Bellman kernels (sweep, per-action argmax) at d_in = state + action dimension:
+// launch(D, smem, chunk_rows, nomax) issues the kernel of dimension D with the staged-mean
+// configuration of bellman_stage_config.
+template <class F>
+int launch_bellman(const slb_bellman& cfg, int m, F&& launch) {
+    const int din = cfg.grid.ndim + m;
+    int chunk_rows, nomax;
+    const size_t smem = bellman_stage_config(cfg, din, &chunk_rows, &nomax);
+    return slb_dispatch_dim<1, 6>(din, "bellman: state+action dimension", [&](auto D) {
+        launch(D, smem, chunk_rows, nomax);
+        SLB_LAUNCH_CHECK();
+        return 0;
+    });
+}
+
 bool g_det_fast = true;           // slb_debug_det_fast: A/B against the generic interpreter
 
 }  // namespace
@@ -804,6 +819,65 @@ int slb_launch_argmax_factored(cudaStream_t st, const slb_bellman& cfg, int64_t 
                                const double* actions, int n_actions, int m, const double* constraint,
                                int32_t* best, double* best_value, void* workspace);
 
+// The first-fail reduction (slb_first_fail, slb_first_fail_x) and the prefix application
+// (slb_apply_prefix, slb_apply_prefix_x); `x` is the validated peer exchange of the _x forms, or
+// nullptr for a single process.  `who` names the entry point in error messages.
+static int first_fail(const char* who, void* stream, const double* values_dev, const uint8_t* negative_dev,
+                      const uint8_t* initial_dev, int64_t n, int64_t idx_begin, void* workspace_dev,
+                      slb_fail_key* result_dev, const slb_exchange* x) {
+    SLB_CHECK(n >= 0, "%s: negative n", who);
+    SLB_CHECK(workspace_dev && result_dev, "%s: null workspace/result", who);
+    SLB_CHECK(n == 0 || (values_dev && negative_dev), "%s: null input", who);
+    const int64_t want = (n + LT - 1) / LT;
+    const int nparts = (int)(want < 1 ? 1 : (want > FF_BLOCKS ? FF_BLOCKS : want));
+    cudaStream_t st = (cudaStream_t)stream;
+    first_fail_partial_kernel<<<nparts, LT, 0, st>>>(values_dev, negative_dev, initial_dev, n, idx_begin,
+                                                     (ff_partial*)workspace_dev);
+    SLB_LAUNCH_CHECK();
+    slb_exchange none;
+    memset(&none, 0, sizeof(none));
+    first_fail_final_kernel<<<1, FF_BLOCKS, 0, st>>>((const ff_partial*)workspace_dev, nparts, result_dev,
+                                                     x != nullptr ? *x : none);
+    SLB_LAUNCH_CHECK();
+    return 0;
+}
+
+static int apply_prefix(const char* who, void* stream, const double* values_dev, const uint8_t* initial_dev,
+                        int64_t n, int64_t idx_begin, slb_fail_key* key_dev, uint8_t* safe_dev,
+                        slb_prefix_stats* stats_dev, const slb_exchange* x) {
+    SLB_CHECK(n >= 0, "%s: negative n", who);
+    SLB_CHECK(key_dev && stats_dev, "%s: null key/stats", who);
+    SLB_CHECK(n == 0 || (values_dev && safe_dev), "%s: null buffer", who);
+    cudaStream_t st = (cudaStream_t)stream;
+    SLB_CUDA(cudaMemsetAsync(stats_dev, 0, sizeof(slb_prefix_stats), st));
+    // an empty range launches nothing, except that a rank with an empty slab still takes part in the
+    // exchange (one block, no points)
+    if (n == 0 && x == nullptr) return 0;
+    const int64_t want = (n + LT - 1) / LT;
+    const unsigned blocks = (unsigned)(want > 2048 ? 2048 : (want < 1 ? 1 : want));
+    slb_exchange none;
+    memset(&none, 0, sizeof(none));
+    if (x != nullptr && x->world > 1)
+        apply_prefix_kernel<true><<<blocks, LT, 0, st>>>(values_dev, initial_dev, n, idx_begin, key_dev,
+                                                         safe_dev, stats_dev, *x);
+    else
+        apply_prefix_kernel<false><<<blocks, LT, 0, st>>>(values_dev, initial_dev, n, idx_begin, key_dev,
+                                                          safe_dev, stats_dev, x != nullptr ? *x : none);
+    SLB_LAUNCH_CHECK();
+    return 0;
+}
+
+static int validate_exchange(const slb_exchange* x, const char* who) {
+    SLB_CHECK(x != nullptr, "%s: null exchange", who);
+    SLB_CHECK(x->world >= 1 && x->world <= SLB_MAX_RANKS && x->rank >= 0 && x->rank < x->world,
+              "%s: bad exchange (world %d, rank %d, at most %d ranks)", who, x->world, x->rank,
+              SLB_MAX_RANKS);
+    SLB_CHECK(x->seq_dev != nullptr, "%s: exchange without a sequence counter", who);
+    for (int r = 0; r < x->world; ++r)
+        SLB_CHECK(x->slots[r] != nullptr, "%s: exchange slot array of rank %d is not mapped", who, r);
+    return 0;
+}
+
 extern "C" {
 
 int slb_abi_version(void) { return SLB_ABI_VERSION; }
@@ -842,51 +916,16 @@ int64_t slb_first_fail_workspace(int64_t n) {
 int slb_first_fail(void* stream, const double* values_dev, const uint8_t* negative_dev,
                    const uint8_t* initial_dev, int64_t n, int64_t idx_begin, void* workspace_dev,
                    slb_fail_key* result_dev) {
-    SLB_CHECK(n >= 0, "slb_first_fail: negative n");
-    SLB_CHECK(workspace_dev && result_dev, "slb_first_fail: null workspace/result");
-    SLB_CHECK(n == 0 || (values_dev && negative_dev), "slb_first_fail: null input");
-    const int64_t want = (n + LT - 1) / LT;
-    const int nparts = (int)(want < 1 ? 1 : (want > FF_BLOCKS ? FF_BLOCKS : want));
-    cudaStream_t st = (cudaStream_t)stream;
-    first_fail_partial_kernel<<<nparts, LT, 0, st>>>(values_dev, negative_dev, initial_dev, n, idx_begin,
-                                                     (ff_partial*)workspace_dev);
-    SLB_LAUNCH_CHECK();
-    slb_exchange none;
-    memset(&none, 0, sizeof(none));
-    first_fail_final_kernel<<<1, FF_BLOCKS, 0, st>>>((const ff_partial*)workspace_dev, nparts, result_dev,
-                                                     none);
-    SLB_LAUNCH_CHECK();
-    return 0;
-}
-
-static int validate_exchange(const slb_exchange* x, const char* who) {
-    SLB_CHECK(x != nullptr, "%s: null exchange", who);
-    SLB_CHECK(x->world >= 1 && x->world <= SLB_MAX_RANKS && x->rank >= 0 && x->rank < x->world,
-              "%s: bad exchange (world %d, rank %d, at most %d ranks)", who, x->world, x->rank,
-              SLB_MAX_RANKS);
-    SLB_CHECK(x->seq_dev != nullptr, "%s: exchange without a sequence counter", who);
-    for (int r = 0; r < x->world; ++r)
-        SLB_CHECK(x->slots[r] != nullptr, "%s: exchange slot array of rank %d is not mapped", who, r);
-    return 0;
+    return first_fail("slb_first_fail", stream, values_dev, negative_dev, initial_dev, n, idx_begin,
+                      workspace_dev, result_dev, nullptr);
 }
 
 int slb_first_fail_x(void* stream, const double* values_dev, const uint8_t* negative_dev,
                      const uint8_t* initial_dev, int64_t n, int64_t idx_begin, void* workspace_dev,
                      slb_fail_key* result_dev, const slb_exchange* xchg) {
     if (validate_exchange(xchg, "slb_first_fail_x")) return 1;
-    SLB_CHECK(n >= 0, "slb_first_fail_x: negative n");
-    SLB_CHECK(workspace_dev && result_dev, "slb_first_fail_x: null workspace/result");
-    SLB_CHECK(n == 0 || (values_dev && negative_dev), "slb_first_fail_x: null input");
-    const int64_t want = (n + LT - 1) / LT;
-    const int nparts = (int)(want < 1 ? 1 : (want > FF_BLOCKS ? FF_BLOCKS : want));
-    cudaStream_t st = (cudaStream_t)stream;
-    first_fail_partial_kernel<<<nparts, LT, 0, st>>>(values_dev, negative_dev, initial_dev, n, idx_begin,
-                                                     (ff_partial*)workspace_dev);
-    SLB_LAUNCH_CHECK();
-    first_fail_final_kernel<<<1, FF_BLOCKS, 0, st>>>((const ff_partial*)workspace_dev, nparts, result_dev,
-                                                     *xchg);
-    SLB_LAUNCH_CHECK();
-    return 0;
+    return first_fail("slb_first_fail_x", stream, values_dev, negative_dev, initial_dev, n, idx_begin,
+                      workspace_dev, result_dev, xchg);
 }
 
 int slb_apply_prefix_x(void* stream, const double* values_dev, const uint8_t* initial_dev,
@@ -894,22 +933,8 @@ int slb_apply_prefix_x(void* stream, const double* values_dev, const uint8_t* in
                        void* workspace_dev, slb_prefix_stats* stats_dev, const slb_exchange* xchg) {
     (void)workspace_dev;
     if (validate_exchange(xchg, "slb_apply_prefix_x")) return 1;
-    SLB_CHECK(n >= 0, "slb_apply_prefix_x: negative n");
-    SLB_CHECK(key_out_dev && stats_dev, "slb_apply_prefix_x: null key/stats");
-    SLB_CHECK(n == 0 || (values_dev && safe_dev), "slb_apply_prefix_x: null buffer");
-    cudaStream_t st = (cudaStream_t)stream;
-    SLB_CUDA(cudaMemsetAsync(stats_dev, 0, sizeof(slb_prefix_stats), st));
-    // a rank with an empty slab still takes part in the exchange (one block, no points)
-    const int64_t want = (n + LT - 1) / LT;
-    const unsigned blocks = (unsigned)(want > 2048 ? 2048 : (want < 1 ? 1 : want));
-    if (xchg->world > 1)
-        apply_prefix_kernel<true><<<blocks, LT, 0, st>>>(values_dev, initial_dev, n, idx_begin, key_out_dev,
-                                                         safe_dev, stats_dev, *xchg);
-    else
-        apply_prefix_kernel<false><<<blocks, LT, 0, st>>>(values_dev, initial_dev, n, idx_begin, key_out_dev,
-                                                          safe_dev, stats_dev, *xchg);
-    SLB_LAUNCH_CHECK();
-    return 0;
+    return apply_prefix("slb_apply_prefix_x", stream, values_dev, initial_dev, n, idx_begin, key_out_dev,
+                        safe_dev, stats_dev, xchg);
 }
 
 int slb_combine_fail_keys(void* stream, const slb_fail_key* gathered_dev, int32_t world,
@@ -924,21 +949,8 @@ int slb_apply_prefix(void* stream, const double* values_dev, const uint8_t* init
                      int64_t idx_begin, const slb_fail_key* key_dev, uint8_t* safe_dev,
                      void* workspace_dev, slb_prefix_stats* stats_dev) {
     (void)workspace_dev;
-    SLB_CHECK(n >= 0, "slb_apply_prefix: negative n");
-    SLB_CHECK(key_dev && stats_dev, "slb_apply_prefix: null key/stats");
-    SLB_CHECK(n == 0 || (values_dev && safe_dev), "slb_apply_prefix: null buffer");
-    cudaStream_t st = (cudaStream_t)stream;
-    SLB_CUDA(cudaMemsetAsync(stats_dev, 0, sizeof(slb_prefix_stats), st));
-    if (n == 0) return 0;
-    const int64_t want = (n + LT - 1) / LT;
-    const unsigned blocks = (unsigned)(want > 2048 ? 2048 : want);
-    slb_exchange none;
-    memset(&none, 0, sizeof(none));
-    apply_prefix_kernel<false><<<blocks, LT, 0, st>>>(values_dev, initial_dev, n, idx_begin,
-                                                      const_cast<slb_fail_key*>(key_dev), safe_dev, stats_dev,
-                                                      none);
-    SLB_LAUNCH_CHECK();
-    return 0;
+    return apply_prefix("slb_apply_prefix", stream, values_dev, initial_dev, n, idx_begin,
+                        const_cast<slb_fail_key*>(key_dev), safe_dev, stats_dev, nullptr);
 }
 
 int slb_eval_function(void* stream, const slb_function* fn, const double* points_dev, int64_t n,
@@ -977,21 +989,10 @@ int slb_bellman_sweep(void* stream, const slb_bellman* cfg, int64_t idx_begin, i
     const int64_t n = idx_end - idx_begin;
     if (n == 0) return 0;
     SLB_CHECK(out_dev != nullptr, "slb_bellman_sweep: null output");
-    const int din = cfg->grid.ndim + m;
-    int chunk_rows, nomax;
-    const size_t smem = bellman_stage_config(*cfg, din, &chunk_rows, &nomax);
-#define SLB_BELLMAN_CASE(D) \
-    case D: bellman_kernel<D><<<blocks_for(n), LT, smem, (cudaStream_t)stream>>>(*cfg, idx_begin, n, out_dev, chunk_rows, nomax); break;
-    switch (din) {
-        SLB_BELLMAN_CASE(1) SLB_BELLMAN_CASE(2) SLB_BELLMAN_CASE(3) SLB_BELLMAN_CASE(4)
-        SLB_BELLMAN_CASE(5) SLB_BELLMAN_CASE(6)
-    default:
-        slb_set_error("bellman: state+action dimension %d not compiled (1..6)", din);
-        return 1;
-    }
-#undef SLB_BELLMAN_CASE
-    SLB_LAUNCH_CHECK();
-    return 0;
+    return launch_bellman(*cfg, m, [&](auto D, size_t smem, int chunk_rows, int nomax) {
+        bellman_kernel<D><<<blocks_for(n), LT, smem, (cudaStream_t)stream>>>(*cfg, idx_begin, n, out_dev,
+                                                                            chunk_rows, nomax);
+    });
 }
 
 int slb_debug_det_fast(int32_t enable) {
@@ -1020,23 +1021,11 @@ int slb_bellman_argmax(void* stream, const slb_bellman* cfg, int64_t idx_begin, 
         return slb_launch_argmax_factored((cudaStream_t)stream, *cfg, idx_begin, n, actions_dev,
                                           n_actions, m, constraint_dev, best_dev, best_value_dev,
                                           workspace_dev);
-    const int din = cfg->grid.ndim + m;
-    int chunk_rows, nomax;
-    const size_t smem = bellman_stage_config(*cfg, din, &chunk_rows, &nomax);
-#define SLB_ARGMAX_CASE(D)                                                               \
-    case D: bellman_argmax_kernel<D><<<blocks_for(n), LT, smem, (cudaStream_t)stream>>>(  \
-        *cfg, idx_begin, n, actions_dev, n_actions, m, constraint_dev, best_dev, best_value_dev, \
-        chunk_rows, nomax); break;
-    switch (din) {
-        SLB_ARGMAX_CASE(1) SLB_ARGMAX_CASE(2) SLB_ARGMAX_CASE(3) SLB_ARGMAX_CASE(4)
-        SLB_ARGMAX_CASE(5) SLB_ARGMAX_CASE(6)
-    default:
-        slb_set_error("bellman: state+action dimension %d not compiled (1..6)", din);
-        return 1;
-    }
-#undef SLB_ARGMAX_CASE
-    SLB_LAUNCH_CHECK();
-    return 0;
+    return launch_bellman(*cfg, m, [&](auto D, size_t smem, int chunk_rows, int nomax) {
+        bellman_argmax_kernel<D><<<blocks_for(n), LT, smem, (cudaStream_t)stream>>>(
+            *cfg, idx_begin, n, actions_dev, n_actions, m, constraint_dev, best_dev, best_value_dev,
+            chunk_rows, nomax);
+    });
 }
 
 int slb_max_abs_diff(void* stream, const double* a_dev, const double* b_dev, int64_t n,

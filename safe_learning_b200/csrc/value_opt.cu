@@ -57,18 +57,19 @@ SLB_DEV void stats_flush(row_stats& s, unsigned long long* __restrict__ stats) {
 }
 
 // Row of T for the next state xp: columns (vertex indices) and weights.  The reference's lookup
-// (tri_locate); when it yields a weight < -W_TOL although the point is inside the grid (or projected
-// onto it), the point lies on a grid line where `% unit_maxes` rounded to ~unit_maxes and picked a
-// simplex of the wrong side of the cell: search the cell again with unit coordinates taken relative
-// to the cell's own lowest vertex.
+// (tri_lookup, common.cuh); when it yields a weight < -W_TOL although the point is inside the grid
+// (or projected onto it), the point lies on a grid line where `% unit_maxes` rounded to ~unit_maxes
+// and picked a simplex of the wrong side of the cell: search the cell again with unit coordinates
+// taken relative to the cell's own lowest vertex (TRI_CELL).
 template <typename IDX>
 SLB_DEV void operator_row(const slb_function& f, const double* xp, IDX* __restrict__ cols,
                           double* __restrict__ W, row_stats& st) {
     const slb_grid& g = f.grid;
     const int d = g.ndim;
     int64_t corner;
+    int s;
     double w[SLB_MAX_DIM + 1];
-    int s = tri_locate(f, xp, &corner, w);
+    tri_lookup<TRI_WEIGHTS>(f, xp, w, &corner, &s);
     double wmin = w[0];
     bool inside = true, bad = false;
     for (int k = 0; k < d; ++k) {
@@ -77,12 +78,7 @@ SLB_DEV void operator_row(const slb_function& f, const double* xp, IDX* __restri
         bad = bad || xp[k] != xp[k];
     }
     if (wmin < -W_TOL && ((f.flags & SLB_FLAG_PROJECT) || inside)) {
-        double lo[SLB_MAX_DIM], unit[SLB_MAX_DIM];
-        grid_index_to_state(g, corner, lo);
-        for (int k = 0; k < d; ++k)
-            unit[k] = f64sub(fmin(fmax(xp[k], g.offset[k]), g.upper[k]), lo[k]);
-        s = tri_find_simplex(f, unit);
-        tri_barycentric(f, xp, corner, s, w);
+        tri_lookup<TRI_CELL>(f, xp, w, &corner, &s);
         st.repaired += 1;
     }
     const int64_t* simp = f.unit_simplices + (size_t)s * (d + 1);
@@ -160,7 +156,7 @@ struct solve_args {
     int64_t max_iters;
 };
 
-// r_i + gamma (w_0 v[c_0] + w_1 v[c_1] + ...): eval_triangulation's and bellman_value's arithmetic
+// r_i + gamma (w_0 v[c_0] + w_1 v[c_1] + ...): tri_lookup's and bellman_value's arithmetic
 template <typename IDX>
 SLB_DEV double apply_row(const IDX* __restrict__ cols, const double* __restrict__ W, double r, int ncols,
                          double gamma, const double* v, int64_t i) {
@@ -413,22 +409,14 @@ int slb_value_operator(void* stream, const slb_bellman* cfg, int64_t idx_begin, 
     const unsigned blocks = (unsigned)((n + VT - 1) / VT);
     const bool wide = wide_index(cfg->value.grid.nindex);
     unsigned long long* stats = reinterpret_cast<unsigned long long*>(stats_dev);
-#define SLB_VOP_CASE(D)                                                                             \
-    case D:                                                                                         \
-        if (wide) value_operator_kernel<D, int64_t><<<blocks, VT, smem, st>>>(                      \
-            *cfg, idx_begin, n, (int64_t*)cols_dev, weights_dev, rewards_dev, stats, chunk_rows, nomax); \
-        else value_operator_kernel<D, int32_t><<<blocks, VT, smem, st>>>(                           \
-            *cfg, idx_begin, n, (int32_t*)cols_dev, weights_dev, rewards_dev, stats, chunk_rows, nomax); \
-        break;
-    switch (din) {
-        SLB_VOP_CASE(2) SLB_VOP_CASE(3) SLB_VOP_CASE(4) SLB_VOP_CASE(5) SLB_VOP_CASE(6)
-    default:
-        slb_set_error("slb_value_operator: state+action dimension %d not compiled (2..6)", din);
-        return 1;
-    }
-#undef SLB_VOP_CASE
-    SLB_LAUNCH_CHECK();
-    return 0;
+    return slb_dispatch_dim<2, 6>(din, "slb_value_operator: state+action dimension", [&](auto D) {
+        if (wide) value_operator_kernel<D, int64_t><<<blocks, VT, smem, st>>>(
+            *cfg, idx_begin, n, (int64_t*)cols_dev, weights_dev, rewards_dev, stats, chunk_rows, nomax);
+        else value_operator_kernel<D, int32_t><<<blocks, VT, smem, st>>>(
+            *cfg, idx_begin, n, (int32_t*)cols_dev, weights_dev, rewards_dev, stats, chunk_rows, nomax);
+        SLB_LAUNCH_CHECK();
+        return 0;
+    });
 }
 
 int slb_value_operator_points(void* stream, const slb_function* value, const double* next_states_dev,

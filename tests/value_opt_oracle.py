@@ -11,7 +11,7 @@ EPS = np.finfo(np.float64).eps
 
 def _search(tri, unit):
     """First simplex of the unit cell whose barycentric weights at `unit` are all >= -W_TOL, else the
-    one whose smallest weight is largest (common.cuh tri_find_simplex)."""
+    one whose smallest weight is largest (common.cuh tri_lookup)."""
     disc = tri.discretization
     d = tri.input_dim
     best, best_min = 0, -np.inf

@@ -3,7 +3,8 @@
 #include <stdint.h>
 #include <string.h>
 #include <stdlib.h>
-#include "exp2_tab.h"
+#include "../safe_learning_b200/csrc/exp2_tab64.h"
+static const double EXP2_TAB[64] = {SLB_EXP2_TAB64};
 static inline double exp_neg_tab(double x){
   const double MAGIC = 6755399441055744.0;
   double t = fma(x, 92.332482616893656877, MAGIC);         // 64/ln2
