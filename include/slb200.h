@@ -516,7 +516,7 @@ int slb_value_solve(void* stream, int64_t n, int32_t ncols, const void* cols_dev
  *                                   the plants, which have no parameters
  *        out_dev         [n, out] = the forward pass recomputed by the gradient kernel, bit-identical to
  *                                   slb_eval_function (or NULL)
- *      Kinds MLP, LYAPUNOV_NN, PENDULUM and CARTPOLE without post-op flags.  Gradient conventions: ReLU' = 0
+ *      Kinds MLP, LYAPUNOV_NN, PENDULUM and CARTPOLE (and TRIANGULATION, below) without post-op flags.  Gradient conventions: ReLU' = 0
  *      at 0, tanh' = 1 - tanh^2.  The parameter gradient is reduced in a fixed order without atomics: two
  *      calls with the same inputs give bit-identical results.  n == 0 zeroes grad_params and launches
  *      nothing.  workspace_dev: >= slb_function_vjp_workspace(fn, n) bytes when grad_params_dev is
@@ -525,6 +525,22 @@ int64_t slb_function_vjp_workspace(const slb_function* fn, int64_t n);
 int slb_function_vjp(void* stream, const slb_function* fn, const double* points_dev, int64_t n,
                      const double* grad_out_dev, double* grad_in_dev, double* grad_params_dev,
                      double* out_dev, void* workspace_dev);
+/* ---- SLB_FN_TRIANGULATION in slb_function_vjp (the tf.gather of functions.py:1494-1499 under
+ *      tf.gradients): grad_params_dev [nindex, out] = sum over the points p and simplex vertices k of
+ *      w_pk grad_out[p] scattered to vertex c_pk, OVERWRITTEN; (c_pk, w_pk) are the vertices and barycentric
+ *      weights of the forward evaluation (slb_triangulation_rows).  Each entry is summed sequentially in
+ *      ascending j = p (d + 1) + k from +0.0, without atomics: bit for bit np.add.at over the rows, and two
+ *      calls give identical results.  grad_in_dev must be NULL (the point gradient is the SLB_FLAG_GRADIENT
+ *      evaluation); out_dev [n, out] is the forward, bit-identical to slb_eval_function.  No post-op flags
+ *      (SLB_FLAG_PROJECT applies).  n == 0 zeroes grad_params.  The workspace (rows, sort keys, sort scratch)
+ *      is needed when grad_params_dev is given and n > 0; a batch whose sort key (bits of nindex - 1 plus
+ *      bits of n (d + 1) - 1) exceeds 64 bits is rejected.  One thread sums each vertex, so a batch whose
+ *      points all land on one vertex costs n (d + 1) serial additions. */
+/* the rows of _Triangulation.parameter_derivative (functions.py:1228-1259) at points_dev [n, d]:
+ * cols_dev int64 [n, d + 1] vertex indices and weights_dev [n, d + 1] barycentric weights of the forward
+ * evaluation (projection, corner table and simplex choice included) */
+int slb_triangulation_rows(void* stream, const slb_function* fn, const double* points_dev, int64_t n,
+                           int64_t* cols_dev, double* weights_dev);
 
 #ifdef __cplusplus
 }

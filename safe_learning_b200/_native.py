@@ -175,6 +175,7 @@ SIGNATURES = {
                                   _vp, _vp]),
     "slb_function_vjp_workspace": (C.c_int64, [C.POINTER(SlbFunction), _i64]),
     "slb_function_vjp": (C.c_int, [_vp, C.POINTER(SlbFunction), _dp, _i64, _dp, _dp, _dp, _dp, _vp]),
+    "slb_triangulation_rows": (C.c_int, [_vp, C.POINTER(SlbFunction), _dp, _i64, _vp, _dp]),
 }
 
 _lib = None

@@ -18,9 +18,17 @@
 //
 // Plants (SLB_FN_PENDULUM, SLB_FN_CARTPOLE): one thread per point, forward mode over the 3 or 5
 // inputs through the ten Euler sub-steps (state and tangents in registers), then grad_in = g^T J.
+//
+// SLB_FN_TRIANGULATION: the vertex-value gradient of triangulation_grad.cu.
 #include "common.cuh"
 
 #include <string.h>
+
+// triangulation_grad.cu
+int64_t slb_triangulation_vjp_workspace(const slb_function* fn, int64_t n);
+int slb_triangulation_vjp(cudaStream_t st, const slb_function* fn, const double* points_dev, int64_t n,
+                          const double* grad_out_dev, double* grad_in_dev, double* grad_params_dev,
+                          double* out_dev, void* workspace_dev);
 
 namespace {
 
@@ -333,11 +341,12 @@ int network_ctas(const net_shape& S, int64_t n) {
 int vjp_validate(const slb_function* fn, const char* what) {
     SLB_CHECK(fn != nullptr, "%s: null function", what);
     SLB_CHECK(fn->kind == SLB_FN_MLP || fn->kind == SLB_FN_LYAPUNOV_NN || fn->kind == SLB_FN_PENDULUM ||
-              fn->kind == SLB_FN_CARTPOLE,
-              "%s: function kind %d has no VJP (NeuralNetwork, LyapunovNetwork, InvertedPendulum, CartPole)",
-              what, fn->kind);
-    SLB_CHECK(fn->flags == 0, "%s: post-op flags 0x%x are not differentiated here (compose them in torch)",
-              what, fn->flags);
+              fn->kind == SLB_FN_CARTPOLE || fn->kind == SLB_FN_TRIANGULATION,
+              "%s: function kind %d has no VJP (NeuralNetwork, LyapunovNetwork, InvertedPendulum, CartPole, "
+              "Triangulation)", what, fn->kind);
+    const uint32_t allowed = fn->kind == SLB_FN_TRIANGULATION ? SLB_FLAG_PROJECT : 0u;   // not a post-op
+    SLB_CHECK((fn->flags & ~allowed) == 0,
+              "%s: post-op flags 0x%x are not differentiated here (compose them in torch)", what, fn->flags);
     return slb_validate_function(fn, what, 0);
 }
 
@@ -346,6 +355,7 @@ int vjp_validate(const slb_function* fn, const char* what) {
 extern "C" int64_t slb_function_vjp_workspace(const slb_function* fn, int64_t n) {
     if (vjp_validate(fn, "slb_function_vjp_workspace")) return -1;
     if (n < 0) { slb_set_error("slb_function_vjp_workspace: negative n"); return -1; }
+    if (fn->kind == SLB_FN_TRIANGULATION) return slb_triangulation_vjp_workspace(fn, n);
     if (fn->kind == SLB_FN_PENDULUM || fn->kind == SLB_FN_CARTPOLE) return 0;
     net_shape S;
     network_shape(*fn, &S);
@@ -358,12 +368,18 @@ extern "C" int slb_function_vjp(void* stream, const slb_function* fn, const doub
                                 double* out_dev, void* workspace_dev) {
     if (vjp_validate(fn, "slb_function_vjp")) return 1;
     SLB_CHECK(n >= 0, "slb_function_vjp: negative n (%lld)", (long long)n);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (fn->kind == SLB_FN_TRIANGULATION) {
+        SLB_CHECK(n == 0 || (points_dev != nullptr && grad_out_dev != nullptr),
+                  "slb_function_vjp: null points or cotangent");
+        return slb_triangulation_vjp(st, fn, points_dev, n, grad_out_dev, grad_in_dev, grad_params_dev, out_dev,
+                                     workspace_dev);
+    }
     const bool plant = fn->kind == SLB_FN_PENDULUM || fn->kind == SLB_FN_CARTPOLE;
     SLB_CHECK(!plant || grad_params_dev == nullptr,
               "slb_function_vjp: the plants have no parameters (grad_params must be NULL)");
     SLB_CHECK(n == 0 || (points_dev != nullptr && grad_out_dev != nullptr),
               "slb_function_vjp: null points or cotangent");
-    cudaStream_t st = (cudaStream_t)stream;
     if (plant) {
         if (n == 0 || (grad_in_dev == nullptr && out_dev == nullptr)) return 0;
         vjp_plant_kernel<<<(unsigned)((n + NT - 1) / NT), NT, 0, st>>>(*fn, points_dev, n, grad_out_dev,

@@ -15,9 +15,11 @@ from __future__ import annotations
 
 import hashlib
 import itertools
+import weakref
 
 import numpy as np
 import scipy.signal
+import scipy.sparse
 import scipy.spatial
 import torch
 
@@ -213,6 +215,14 @@ class Function(object):
         under ``tf.gradients`` in ``examples/inverted_pendulum.ipynb`` cell 17)."""
         return _FusedApply.apply(points, self)
 
+    def _trainable_tensors(self):
+        """The leaf tensors ``torch(points)`` differentiates besides the points (none here)."""
+        return []
+
+    def _param_vjp(self, points, grad_out):
+        """Gradients of ``sum(grad_out * fun(points))`` for each of ``_trainable_tensors()``."""
+        raise NotImplementedError("%s has no trainable tensors" % type(self).__name__)
+
     # algebra (``functions.py:112-122``) --------------------------------------------------
     def __neg__(self):
         return ScaledFunction(self, -1.0)
@@ -249,6 +259,32 @@ class _FusedApply(torch.autograd.Function):
             return _function_vjp(ctx.fun, points, grad_out)[0], None
         jac = ctx.fun.jacobian_device(points)                       # [n, out, in]
         return torch.einsum("no,noi->ni", grad_out.contiguous(), jac), None
+
+
+class _PostOpApply(torch.autograd.Function):
+    """A post-op wrapper in torch's autograd graph with the wrapped object's trainable tensors as
+    inputs: the points' gradient is ``_FusedApply``'s, the tensors' gradients are the wrapped object's
+    VJP of the cotangent mapped through the wrapper (``_PostOp._param_vjp``)."""
+
+    @staticmethod
+    def forward(ctx, points, fun, *params):
+        points = points.detach().contiguous()
+        ctx.fun = fun
+        ctx.save_for_backward(points, *params)       # torch refuses backward after an in-place update
+        return fun.evaluate_device(points)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_out):
+        points, params = ctx.saved_tensors[0], ctx.saved_tensors[1:]
+        fun, grad_out = ctx.fun, grad_out.contiguous()
+        gin = None
+        if ctx.needs_input_grad[0]:
+            gin = torch.einsum("no,noi->ni", grad_out, fun.jacobian_device(points))
+        grads = [None] * len(params)
+        if any(ctx.needs_input_grad[2:]):
+            grads = fun._param_vjp(points, grad_out)
+        return (gin, None) + tuple(grads)
 
 
 def _function_vjp(fun, points, grad_out, want_in=True, nparams=0, want_out=False):
@@ -400,6 +436,34 @@ class _PostOp(DeterministicFunction):
         return (id(self.fun), self.fun.version, getattr(self, "lower", None),
                 getattr(self, "upper", None), getattr(self, "factor", None))
 
+    def _inner_cotangent(self, inner, grad_out):
+        """The cotangent of the wrapped function's output ``inner`` [n, out] for the cotangent
+        ``grad_out`` of this wrapper's output (the rule of ``jacobian_device``)."""
+        raise NotImplementedError("%s does not pass gradients to the wrapped function's parameters"
+                                  % type(self).__name__)
+
+    def _trainable_tensors(self):
+        return self.fun._trainable_tensors()
+
+    def _param_vjp(self, points, grad_out):
+        inner = self.fun.evaluate_device(points)
+        return self.fun._param_vjp(points, self._inner_cotangent(inner, grad_out))
+
+    def torch(self, points):
+        """As ``Function.torch``; when the wrapped object has trainable tensors (a network, or a
+        Triangulation whose ``vertex_values`` were requested) they are inputs of the node too: the
+        forward is still the fused evaluation of the whole wrapper, and their gradients are the
+        wrapped object's VJP of the cotangent mapped through this wrapper."""
+        base = self.fun
+        while isinstance(base, _PostOp):
+            base = base.fun
+        if isinstance(base, NeuralNetwork):
+            base.build(points.shape[1])
+        params = self._trainable_tensors()
+        if not params:
+            return _FusedApply.apply(points, self)
+        return _PostOpApply.apply(points, self, *params)
+
 
 class Saturation(_PostOp):
     """``min(max(fun(x), lower), upper)`` (``functions.py:310-354``)."""
@@ -417,10 +481,17 @@ class Saturation(_PostOp):
         d.lower, d.upper = self.lower, self.upper
         return d
 
+    def _free(self, inner):
+        # strictly inside the bounds; tf.clip_by_value also passes the gradient at equality (DESIGN.md
+        # §3.11)
+        return ((inner > self.lower) & (inner < self.upper)).to(torch.float64)
+
+    def _inner_cotangent(self, inner, grad_out):
+        return grad_out * self._free(inner)
+
     def jacobian_device(self, points):
         inner = self.fun.evaluate_device(points)
-        free = ((inner > self.lower) & (inner < self.upper)).to(torch.float64)
-        return self.fun.jacobian_device(points) * free.unsqueeze(2)   # tf.clip_by_value's gradient
+        return self.fun.jacobian_device(points) * self._free(inner).unsqueeze(2)
 
 
 class AbsFunction(_PostOp):
@@ -438,6 +509,9 @@ class AbsFunction(_PostOp):
         d = self.fun.descriptor()
         d.flags |= nat.FLAG_ABS
         return d
+
+    def _inner_cotangent(self, inner, grad_out):
+        return grad_out * torch.sign(inner)
 
     def jacobian_device(self, points):
         sign = torch.sign(self.fun.evaluate_device(points))
@@ -457,6 +531,9 @@ class Norm1Function(_PostOp):
         d = self.fun.descriptor()
         d.flags |= nat.FLAG_NORM1
         return d
+
+    def _inner_cotangent(self, inner, grad_out):
+        return grad_out * torch.sign(inner)                          # [n, 1] against [n, out]
 
     def jacobian_device(self, points):
         sign = torch.sign(self.fun.evaluate_device(points))
@@ -501,6 +578,9 @@ class ScaledFunction(_PostOp):
         d.out_scale = self.factor
         return d
 
+    def _inner_cotangent(self, inner, grad_out):
+        return grad_out * self.factor
+
     def jacobian_device(self, points):
         return self.fun.jacobian_device(points) * self.factor
 
@@ -520,10 +600,11 @@ class _TriangulationTables(object):
     hyper-rectangle is triangulated once by Qhull; the kernels take the resulting
     ``unit_simplices`` / ``hyperplanes`` instead of assuming a particular split."""
 
-    def __init__(self, discretization, project=False):
+    def __init__(self, discretization, project=False, owner=None):
         self.discretization = disc = discretization
         self.input_dim = disc.ndim
         self.project = project
+        self._owner = weakref.ref(owner) if owner is not None else None
         if disc.ndim == 1:
             self.triangulation = _Delaunay1D(np.array([[0.0], [disc.unit_maxes[0]]]))
         else:
@@ -558,6 +639,30 @@ class _TriangulationTables(object):
     def nindex(self):
         return self.discretization.nindex
 
+    def parameter_derivative(self, points):
+        """``_Triangulation.parameter_derivative`` (``functions.py:1228-1259``): the sparse [n, nindex]
+        matrix B with ``tri(points) = B @ vertex_values``, in the reference's layout (rows
+        ``repeat(arange(n), d + 1)``, cols the simplex vertices of each point, data the barycentric
+        weights).  The rows are the forward evaluation's, computed on the device
+        (``slb_triangulation_rows``)."""
+        owner = self._owner() if self._owner is not None else None
+        if owner is None:
+            raise ValueError("parameter_derivative needs the Triangulation these tables belong to")
+        lib = nat.load()
+        desc = owner.descriptor()
+        pts = dev.to_device(np.atleast_2d(np.asarray(points, dtype=np.float64)))
+        if pts.shape[1] != self.input_dim:
+            raise DimensionError("parameter_derivative expects %d input columns, got shape %s"
+                                 % (self.input_dim, tuple(pts.shape)))
+        n, nsimp = pts.shape[0], self.input_dim + 1
+        cols = dev.empty((n, nsimp), torch.int64)
+        weights = dev.empty((n, nsimp))
+        nat.check(lib.slb_triangulation_rows(dev.stream(), desc, pts.data_ptr(), n, cols.data_ptr(),
+                                             weights.data_ptr()), "slb_triangulation_rows")
+        rows = np.repeat(np.arange(n), nsimp)
+        return scipy.sparse.coo_matrix((weights.cpu().numpy().ravel(), (rows, cols.cpu().numpy().ravel())),
+                                       shape=(n, self.nindex))
+
 
 class Triangulation(DeterministicFunction):
     """Piecewise-linear interpolation on a GridWorld (``functions.py:1372-1510``).
@@ -565,11 +670,17 @@ class Triangulation(DeterministicFunction):
     The vertex values live in HBM (``_param_dev`` [nindex, out]); ``parameters`` exposes
     them like the reference's single tf.Variable: ``tri.parameters[0]`` is the [nindex, out]
     array, and assigning ``tri.parameters = values`` re-uploads.
+
+    ``vertex_values`` hands out that buffer as a float64 leaf tensor with ``requires_grad``, for
+    ``torch.optim``: from then on every writer (the ``parameters`` setter, ``value_iteration``,
+    ``optimize_value_function``, ``discrete_policy_optimization``) copies into it in place, so the
+    leaf, the descriptor and the optimizer keep seeing one tensor, and ``version`` follows its
+    in-place updates.  ``torch(points)`` differentiates the points and the vertex values.
     """
 
     def __init__(self, discretization, vertex_values, project=False, name="triangulation"):
         super().__init__(name)
-        self.tri = _TriangulationTables(discretization, project=project)
+        self.tri = _TriangulationTables(discretization, project=project, owner=self)
         self.input_dim = self.tri.input_dim
         self._param_dev = None
         self._hyper_dev = None
@@ -600,27 +711,62 @@ class Triangulation(DeterministicFunction):
     def parameters(self):
         if self._param_dev is None:
             return []
-        return [self._param_dev.cpu().numpy()]
+        return [self._param_dev.detach().cpu().numpy()]
 
     @parameters.setter
     def parameters(self, values):
         if isinstance(values, (list, tuple)) and len(values) == 1:
             values = values[0]
         if isinstance(values, torch.Tensor):
-            vals = values.to(dtype=torch.float64).reshape(self.nindex, -1)
-            self._param_dev = vals.to(dev.device()).contiguous().clone()
+            vals = values.detach().to(dtype=torch.float64).reshape(self.nindex, -1)
+            self._store(vals.to(dev.device()).contiguous().clone())
         else:
             vals = np.asarray(values, dtype=np.float64).reshape(self.nindex, -1)
-            self._param_dev = dev.to_device(vals)
-        self.output_dim = int(self._param_dev.shape[1])
+            self._store(dev.to_device(vals))
         self._version += 1
 
     @property
+    def vertex_values(self):
+        """The vertex table [nindex, out] as a float64 leaf tensor with ``requires_grad`` -- the
+        descriptor's buffer itself, so in-place ``torch.optim`` steps are what the fused sweeps read."""
+        if self._param_dev is None:
+            raise ValueError("Triangulation has no vertex values")
+        if not self._param_dev.requires_grad:
+            self._param_dev = self._param_dev.detach().clone().requires_grad_(True)
+        return self._param_dev
+
+    def _store(self, values):
+        """The one writer of the vertex table (a device tensor [nindex, out]): swaps the buffer until
+        ``vertex_values`` has been handed out, then copies into that leaf in place."""
+        leaf = self._param_dev
+        if leaf is not None and leaf.requires_grad:
+            if tuple(values.shape) != tuple(leaf.shape):
+                raise DimensionError("vertex values of shape %s for a table of shape %s (the "
+                                     "vertex_values leaf keeps its shape)"
+                                     % (tuple(values.shape), tuple(leaf.shape)))
+            with torch.no_grad():
+                leaf.copy_(values)
+            return
+        self._param_dev = values
+        self.output_dim = int(values.shape[1])
+
+    def _trainable_tensors(self):
+        leaf = self._param_dev
+        return [leaf] if leaf is not None and leaf.requires_grad else []
+
+    def _param_vjp(self, points, grad_out):
+        _, gflat, _ = _function_vjp(self, points, grad_out, want_in=False,
+                                    nparams=self._param_dev.numel())
+        return [gflat.view(self._param_dev.shape).to(self._param_dev.device)]
+
+    @property
     def version(self):
-        # the vertex table is swapped (new device buffer) by value_iteration, so its address
-        # is part of the descriptor identity
-        return (self._version, self.project,
-                0 if self._param_dev is None else self._param_dev.data_ptr())
+        # the vertex table is swapped (new device buffer) by value_iteration until vertex_values is
+        # handed out, and updated in place after, so its address and its version counter are part of
+        # the descriptor identity
+        if self._param_dev is None:
+            return (self._version, self.project, 0, 0)
+        return (self._version, self.project, self._param_dev.data_ptr(), self._param_dev._version)
 
     def descriptor(self):
         if self._param_dev is None:
@@ -642,6 +788,12 @@ class Triangulation(DeterministicFunction):
         d.grid = self.discretization.descriptor(need_points=True)
         return d
 
+    def torch(self, points):
+        """``tri(points)`` as one autograd node with inputs (points, vertex table): the points'
+        gradient is ``Function.torch``'s, the vertex values' is one ``slb_function_vjp`` call (the
+        transpose of the lookup, summed in a fixed order)."""
+        return _TriangulationApply.apply(points, self, self._param_dev)
+
     def gradient_function(self):
         """The gradient of the interpolant as a fusable function object (one value column)."""
         return TriangulationGradient(self)
@@ -661,9 +813,34 @@ class Triangulation(DeterministicFunction):
         return grad.unsqueeze(1)
 
 
+class _TriangulationApply(torch.autograd.Function):
+    """A Triangulation in torch's autograd graph with its vertex table as an input."""
+
+    @staticmethod
+    def forward(ctx, points, fun, vertex_values):
+        points = points.detach().contiguous()
+        ctx.fun = fun
+        ctx.save_for_backward(points, vertex_values)  # a table write before backward raises
+        return fun.evaluate_device(points)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_out):
+        points, _ = ctx.saved_tensors
+        fun, grad_out = ctx.fun, grad_out.contiguous()
+        gin = gv = None
+        if ctx.needs_input_grad[0]:
+            gin = torch.einsum("no,noi->ni", grad_out, fun.jacobian_device(points))
+        if ctx.needs_input_grad[2]:
+            (gv,) = fun._param_vjp(points, grad_out)
+        return gin, None, gv
+
+
 class TriangulationGradient(DeterministicFunction):
     """``x -> d Triangulation(x) / dx`` (piecewise constant; ``functions.py:1260-1326``), evaluated
-    by the same simplex lookup as the value (``SLB_FLAG_GRADIENT``)."""
+    by the same simplex lookup as the value (``SLB_FLAG_GRADIENT``).  Its ``torch`` differentiates
+    the points only: like the reference's ``py_func`` gradient, it passes no gradient to the vertex
+    values."""
 
     def __init__(self, triangulation, name="triangulation_gradient"):
         super().__init__(name)
@@ -873,6 +1050,13 @@ class _TrainableNetwork(DeterministicFunction):
 
     def jacobian_device(self, points):
         return _unit_vjp_jacobian(self, points)
+
+    def _trainable_tensors(self):
+        return list(self._params)
+
+    def _param_vjp(self, points, grad_out):
+        _, gflat, _ = _function_vjp(self, points, grad_out, False, self._packed_device().numel())
+        return self._grads_like(gflat, self._params)
 
     def vjp(self, points, grad_out, want_out=False):
         """(grad_in [n, in], [grad of each parameter], recomputed forward or None) for the cotangent

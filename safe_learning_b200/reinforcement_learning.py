@@ -101,8 +101,10 @@ class PolicyIteration(object):
         Lyapunov penalty, ``examples/inverted_pendulum.ipynb`` cell 17): every fused function
         object is one autograd node (CUDA evaluation forward, its device Jacobian backward,
         ``Function.torch``), the GP mean / variance are torch operations on the cached Cholesky
-        factor.  ``policy`` may be any callable on tensors (e.g. a ``torch.nn.Module``); gradients
-        flow to ``actions`` / the policy's parameters and to ``states`` if they require them."""
+        factor.  ``policy`` may be any callable on tensors (e.g. a ``torch.nn.Module``), and
+        ``dynamics`` / ``reward_function`` any callable ``fn(states, actions)`` on tensors, as in the
+        reference; gradients flow to ``actions`` / the policy's parameters (network weights,
+        Triangulation ``vertex_values``) and to ``states`` if they require them."""
         states = dev.to_device(states) if not isinstance(states, torch.Tensor) else states
         if actions is None:
             fn = policy or self.policy
@@ -114,9 +116,15 @@ class PolicyIteration(object):
         err = None
         if isinstance(self.dynamics, (FunctionStack, GaussianProcess)):
             mean, err = self.dynamics.torch(z)                                   # :92, :98-99
-        else:
+        elif isinstance(self.dynamics, Function):
             mean = self.dynamics.torch(z)
-        updated = self.reward_function.torch(z) + self.gamma * self.value_function.torch(mean)
+        else:
+            mean = self.dynamics(states, actions)
+            if isinstance(mean, tuple):
+                mean, err = mean
+        reward = self.reward_function
+        rewards = reward.torch(z) if isinstance(reward, Function) else reward(states, actions)
+        updated = rewards + self.gamma * self.value_function.torch(mean)
         if lyapunov is not None:                                                 # :107-112
             v_fn, lv = lyapunov.lyapunov_function, lyapunov._lipschitz_lyapunov
             decrease = v_fn.torch(mean) - v_fn.torch(states)
@@ -194,7 +202,7 @@ class PolicyIteration(object):
         residual = dev.zeros((1,))
         nat.check(lib.slb_max_abs_diff(dev.stream(), new.data_ptr(), old.data_ptr(),
                                        new.numel(), residual.data_ptr()), "slb_max_abs_diff")
-        tri._param_dev = new.reshape(-1, 1).contiguous()
+        tri._store(new.reshape(-1, 1).contiguous())
         return float(residual.item())
 
     def discrete_policy_optimization(self, action_space, constraint=None):
@@ -320,7 +328,7 @@ class PolicyIteration(object):
             nat.check(lib.slb_value_operator_points(dev.stream(), tri.descriptor(), nxt.data_ptr(), n,
                                                     cols.data_ptr(), weights.data_ptr(),
                                                     stats.data_ptr()), "slb_value_operator_points")
-        values = tri._param_dev.reshape(-1).clone()                           # warm start
+        values = tri._param_dev.detach().reshape(-1).clone()                  # warm start
         need = int(lib.slb_value_solve_workspace(n, ncols))
         work = dev.empty((need // 8,)) if need else None
         nat.check(lib.slb_value_solve(dev.stream(), n, ncols, cols.data_ptr(), weights.data_ptr(),
@@ -338,5 +346,5 @@ class PolicyIteration(object):
         self.last_solve = info
         out = host[:n].reshape(n, 1).copy()
         if info["status"] == nat.VALUE_CONVERGED:
-            tri._param_dev = values.reshape(-1, 1)
+            tri._store(values.reshape(-1, 1))
         return out, info

@@ -524,6 +524,89 @@ def train():
                           **info}))
 
 
+def tri_train():
+    """Triangulation vertex gradient (slb_function_vjp, deterministic) against torch.index_add_ (atomic
+    scatter, not deterministic) and torch.sparse.mm of parameter_derivative^T, and one SGD step of the
+    two Triangulation training loops of test_gpu_triangulation_grad.py.  Bytes per point of the VJP:
+    rows (d + 1) x (8 B key + 8 B weight written), sort (~4 passes of 16 B per key), sum (key, weight
+    and cotangent read once more)."""
+    rng = np.random.default_rng(0)
+    cases = (("55x55", [[-1, 1], [-1, 1]], [55, 55]), ("512x512", [[-1, 1], [-1, 1]], [512, 512]),
+             ("21^4", [[-1, 1]] * 4, [21] * 4))
+    info = None
+    for name, limits, num in cases:
+        grid = sl.GridWorld(limits, num)
+        tri = sl.Triangulation(grid, rng.normal(size=(grid.nindex, 1)), project=True)
+        d = grid.ndim
+        for n in (10 ** 3, 10 ** 5, 10 ** 6):
+            x = torch.tensor(rng.uniform(-1.1, 1.1, (n, d)), device="cuda")
+            g = torch.tensor(rng.normal(size=(n, 1)), device="cuda")
+            if info is None:
+                info = _gpu_info(lambda: tri._param_vjp(x, g))
+            ms_vjp = timed(lambda: tri._param_vjp(x, g), steps=20, warmup=3)
+            pd = tri.tri.parameter_derivative(x.cpu().numpy())
+            cols = torch.tensor(pd.col, device="cuda")
+            w = torch.tensor(pd.data, device="cuda")
+            rows = torch.tensor(pd.row, device="cuda")
+            out = torch.zeros((grid.nindex, 1), dtype=torch.float64, device="cuda")
+
+            def index_add():
+                out.zero_()
+                out.index_add_(0, cols, (w * g[rows, 0])[:, None])
+            ms_index_add = timed(index_add, steps=20, warmup=3)
+            spt = torch.sparse_coo_tensor(torch.stack([cols, rows]), w, (grid.nindex, n)).coalesce()
+            ms_sparse = timed(lambda: torch.sparse.mm(spt, g), steps=20, warmup=3)
+            ref = tri._param_vjp(x, g)[0]
+            index_add()
+            print(json.dumps({"bench": "tri_vjp", "grid": name, "vertices": grid.nindex, "points": n,
+                              "ms_slb_function_vjp": ms_vjp, "ms_torch_index_add": ms_index_add,
+                              "ms_torch_sparse_mm_coalesced": ms_sparse,
+                              "max_abs_diff_index_add": float((out - ref).abs().max()),
+                              "note": "median of CUDA events; index_add_ and sparse.mm start from rows "
+                                      "already built (parameter_derivative), the VJP builds its own",
+                              **info}))
+    # one SGD step of tests/test_rl.py:29-77 and of the mountain-car loop
+    a, b = np.array([[1.2]]), np.array([[0.9]])
+    disc = sl.GridWorld([[-1, 1]], 19)
+    pdisc = sl.GridWorld([-1, 1], 5)
+    policy = sl.Triangulation(pdisc, -0.3 * pdisc.all_points)
+    rl = sl.PolicyIteration(policy, sl.LinearSystem((a, b)),
+                            sl.QuadraticFunction(-scipy.linalg.block_diag([[1.]], [[0.1]])),
+                            sl.Triangulation(disc, 0. * disc.all_points, project=True))
+    opt = torch.optim.SGD([policy.vertex_values], lr=0.01)
+    st = torch.tensor(rl.state_space, device="cuda")
+
+    def rl_step():
+        loss = -torch.sum(rl.future_values(st))
+        opt.zero_grad()
+        loss.backward()
+        opt.step()
+
+    mc = sl.GridWorld([[-1.2, 0.7], [-.07, .07]], [20, 20])
+    ptri = sl.Triangulation(mc, np.zeros(mc.nindex), project=True)
+
+    def dyn(s, u):
+        return torch.stack((s[:, 0] + s[:, 1], s[:, 1] + 0.001 * u[:, 0] - 0.0025 * torch.cos(3 * s[:, 0])), 1)
+
+    def rew(s, u):
+        return torch.where(s[:, :1] > 0.6, 0.01 * torch.ones_like(s[:, :1]), torch.zeros_like(s[:, :1]))
+    mrl = sl.PolicyIteration(sl.Saturation(ptri, -1., 1.), dyn, rew,
+                             sl.Triangulation(mc, np.linspace(0, 1, mc.nindex), project=True), gamma=0.99)
+    mopt = torch.optim.SGD([ptri.vertex_values], lr=1.)
+    ms = torch.tensor(mrl.state_space, device="cuda")
+
+    def mc_step():
+        loss = -100. * torch.mean(mrl.future_values(ms))
+        mopt.zero_grad()
+        loss.backward()
+        mopt.step()
+
+    for name, step in (("test_rl_integration_19pts", rl_step), ("mountain_car_20x20", mc_step)):
+        print(json.dumps({"bench": "tri_train_loop", "loop": name, "ms_per_step": timed(step, steps=50),
+                          "note": "median of CUDA events around one SGD step (forward, backward, update)",
+                          **info}))
+
+
 if __name__ == "__main__":
     which = sys.argv[1:] or ["bellman", "det", "det_linear", "c5", "shared", "c4", "nb", "argmax"]
     for name in which:
