@@ -425,6 +425,9 @@ int slb_apply_prefix(void* stream, const double* values_dev, const uint8_t* init
  *      points_dev [n, fn->in_dim] -> out_dev [n, out columns]. ---------------------------- */
 int slb_eval_function(void* stream, const slb_function* fn, const double* points_dev, int64_t n,
                       double* out_dev);
+/* fn's COLUMNS (see slb_sweep), the width of slb_eval_function's out_dev; -1 for a NULL fn.  The
+ * descriptor is not validated otherwise. */
+int slb_function_columns(const slb_function* fn);
 /* grid coordinates for flat indices [idx_begin, idx_end): GridWorld.index_to_state */
 int slb_index_to_state(void* stream, const slb_grid* grid, int64_t idx_begin, int64_t idx_end,
                        double* states_dev);

@@ -157,6 +157,7 @@ SIGNATURES = {
     "slb_combine_fail_keys": (C.c_int, [_vp, _vp, _i32, _vp]),
     "slb_apply_prefix": (C.c_int, [_vp, _dp, _dp, _i64, _i64, _vp, _dp, _vp, _vp]),
     "slb_eval_function": (C.c_int, [_vp, C.POINTER(SlbFunction), _dp, _i64, _dp]),
+    "slb_function_columns": (C.c_int, [C.POINTER(SlbFunction)]),
     "slb_index_to_state": (C.c_int, [_vp, C.POINTER(SlbGrid), _i64, _i64, _dp]),
     "slb_bellman_sweep": (C.c_int, [_vp, C.POINTER(SlbBellman), _i64, _i64, _dp]),
     "slb_bellman_argmax_workspace": (C.c_int64, [C.POINTER(SlbBellman), _i32]),

@@ -123,8 +123,8 @@ int slb_validate_function(const slb_function* f, const char* what, int expect_in
 }
 
 // The columns eval_fn (common.cuh) returns for f: the kind's count, then 1 after NORM1 / MAXABS.
-// Host code sizes kernels and checks shapes with this number and never with out_dim: a change to
-// eval_fn's return value must be made here too.
+// Host code (and Python, through slb_function_columns) sizes kernels and checks shapes with this number
+// and never with out_dim: a change to eval_fn's return value must be made here too.
 int slb_fn_columns(const slb_function& f) {
     if (f.flags & (SLB_FLAG_NORM1 | SLB_FLAG_MAXABS)) return 1;
     switch (f.kind) {
@@ -951,6 +951,14 @@ int slb_apply_prefix(void* stream, const double* values_dev, const uint8_t* init
     (void)workspace_dev;
     return apply_prefix("slb_apply_prefix", stream, values_dev, initial_dev, n, idx_begin,
                         const_cast<slb_fail_key*>(key_dev), safe_dev, stats_dev, nullptr);
+}
+
+int slb_function_columns(const slb_function* fn) {
+    if (fn == nullptr) {
+        slb_set_error("slb_function_columns: null function");
+        return -1;
+    }
+    return slb_fn_columns(*fn);
 }
 
 int slb_eval_function(void* stream, const slb_function* fn, const double* points_dev, int64_t n,

@@ -195,9 +195,7 @@ class Function(object):
         if pts.dim() != 2 or pts.shape[1] != desc.in_dim:
             raise DimensionError("%s expects %d input columns, got shape %s"
                                  % (type(self).__name__, desc.in_dim, tuple(pts.shape)))
-        ncols = 1 if (desc.flags & (nat.FLAG_NORM1 | nat.FLAG_MAXABS)
-                      or desc.kind == nat.FN_QUADRATIC) else desc.out_dim
-        out = dev.empty((pts.shape[0], ncols))
+        out = dev.empty((pts.shape[0], lib.slb_function_columns(desc)))
         nat.check(lib.slb_eval_function(dev.stream(), desc, pts.data_ptr(), pts.shape[0],
                                         out.data_ptr()), "slb_eval_function")
         return out
@@ -209,19 +207,34 @@ class Function(object):
         raise NotImplementedError("%s has no device Jacobian" % type(self).__name__)
 
     def torch(self, points):
-        """``fun(points)`` on a device tensor [n, in] as a node of torch's autograd graph: forward
-        = the fused CUDA evaluation, backward = ``grad_out @ jacobian_device(points)`` on the
-        device (``PolicyIteration.future_values`` with tensors, ``reinforcement_learning.py:65-114``
-        under ``tf.gradients`` in ``examples/inverted_pendulum.ipynb`` cell 17)."""
-        return _FusedApply.apply(points, self)
+        """``fun(points)`` on a device tensor [n, in] as one node of torch's autograd graph with
+        inputs (points, ``_trainable_tensors()``): forward = the fused CUDA evaluation, backward =
+        one ``_vjp`` call (``PolicyIteration.future_values`` with tensors,
+        ``reinforcement_learning.py:65-114`` under ``tf.gradients`` in
+        ``examples/inverted_pendulum.ipynb`` cell 17).  The backward is not differentiable itself:
+        a second derivative raises."""
+        if points.dim() == 2:
+            self._build(points.shape[1])
+        return _FusedApply.apply(points, self, *self._trainable_tensors())
+
+    def _build(self, input_dim):
+        """Create whatever depends on the input width before ``torch`` collects the trainable
+        tensors (a network in the reference's convention); nothing here."""
 
     def _trainable_tensors(self):
         """The leaf tensors ``torch(points)`` differentiates besides the points (none here)."""
         return []
 
+    def _vjp(self, points, grad_out, want_in, want_params):
+        """For the cotangent ``grad_out`` [n, out] of ``fun(points)``: (the points' gradient [n, in]
+        if ``want_in`` else None, one gradient per ``_trainable_tensors()`` if ``want_params`` else
+        []).  Here ``grad_out @ jacobian_device(points)`` and no tensors."""
+        gin = torch.einsum("no,noi->ni", grad_out, self.jacobian_device(points)) if want_in else None
+        return gin, []
+
     def _param_vjp(self, points, grad_out):
         """Gradients of ``sum(grad_out * fun(points))`` for each of ``_trainable_tensors()``."""
-        raise NotImplementedError("%s has no trainable tensors" % type(self).__name__)
+        return self._vjp(points, grad_out, False, True)[1]
 
     # algebra (``functions.py:112-122``) --------------------------------------------------
     def __neg__(self):
@@ -243,48 +256,25 @@ class Function(object):
 
 
 class _FusedApply(torch.autograd.Function):
-    """Fused CUDA evaluation of a Function object inside torch's autograd graph."""
+    """Fused CUDA evaluation of a Function object inside torch's autograd graph, with the object's
+    trainable tensors as inputs: the one node behind ``Function.torch``."""
 
     @staticmethod
-    def forward(ctx, points, fun):
+    def forward(ctx, points, fun, *tensors):
         points = points.detach().contiguous()
         ctx.fun = fun
-        ctx.save_for_backward(points)
-        return fun.evaluate_device(points)
-
-    @staticmethod
-    def backward(ctx, grad_out):
-        (points,) = ctx.saved_tensors
-        if isinstance(ctx.fun, (InvertedPendulum, CartPole)):      # one slb_function_vjp call
-            return _function_vjp(ctx.fun, points, grad_out)[0], None
-        jac = ctx.fun.jacobian_device(points)                       # [n, out, in]
-        return torch.einsum("no,noi->ni", grad_out.contiguous(), jac), None
-
-
-class _PostOpApply(torch.autograd.Function):
-    """A post-op wrapper in torch's autograd graph with the wrapped object's trainable tensors as
-    inputs: the points' gradient is ``_FusedApply``'s, the tensors' gradients are the wrapped object's
-    VJP of the cotangent mapped through the wrapper (``_PostOp._param_vjp``)."""
-
-    @staticmethod
-    def forward(ctx, points, fun, *params):
-        points = points.detach().contiguous()
-        ctx.fun = fun
-        ctx.save_for_backward(points, *params)       # torch refuses backward after an in-place update
+        ctx.save_for_backward(points, *tensors)      # torch refuses backward after an in-place update
         return fun.evaluate_device(points)
 
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, grad_out):
-        points, params = ctx.saved_tensors[0], ctx.saved_tensors[1:]
-        fun, grad_out = ctx.fun, grad_out.contiguous()
-        gin = None
-        if ctx.needs_input_grad[0]:
-            gin = torch.einsum("no,noi->ni", grad_out, fun.jacobian_device(points))
-        grads = [None] * len(params)
-        if any(ctx.needs_input_grad[2:]):
-            grads = fun._param_vjp(points, grad_out)
-        return (gin, None) + tuple(grads)
+        # the VJPs are not differentiable themselves: double backward raises instead of treating the
+        # gradient as a constant
+        points, ntensors = ctx.saved_tensors[0], len(ctx.saved_tensors) - 1
+        gin, grads = ctx.fun._vjp(points, grad_out.contiguous(), ctx.needs_input_grad[0],
+                                  any(ctx.needs_input_grad[2:]))
+        return (gin, None) + tuple(grads or [None] * ntensors)
 
 
 def _function_vjp(fun, points, grad_out, want_in=True, nparams=0, want_out=False):
@@ -294,7 +284,7 @@ def _function_vjp(fun, points, grad_out, want_in=True, nparams=0, want_out=False
     desc = fun.descriptor()
     pts = dev.to_device(points)
     n = pts.shape[0]
-    ncols = 1 if desc.kind == nat.FN_LYAPUNOV_NN else desc.out_dim
+    ncols = lib.slb_function_columns(desc)
     gout = dev.to_device(grad_out).reshape(n, ncols).contiguous()
     gin = dev.empty((n, desc.in_dim)) if want_in else None
     gpar = dev.empty((nparams,)) if nparams else None
@@ -442,27 +432,20 @@ class _PostOp(DeterministicFunction):
         raise NotImplementedError("%s does not pass gradients to the wrapped function's parameters"
                                   % type(self).__name__)
 
+    def _build(self, input_dim):
+        self.fun._build(input_dim)
+
     def _trainable_tensors(self):
         return self.fun._trainable_tensors()
 
-    def _param_vjp(self, points, grad_out):
-        inner = self.fun.evaluate_device(points)
-        return self.fun._param_vjp(points, self._inner_cotangent(inner, grad_out))
-
-    def torch(self, points):
-        """As ``Function.torch``; when the wrapped object has trainable tensors (a network, or a
-        Triangulation whose ``vertex_values`` were requested) they are inputs of the node too: the
-        forward is still the fused evaluation of the whole wrapper, and their gradients are the
-        wrapped object's VJP of the cotangent mapped through this wrapper."""
-        base = self.fun
-        while isinstance(base, _PostOp):
-            base = base.fun
-        if isinstance(base, NeuralNetwork):
-            base.build(points.shape[1])
-        params = self._trainable_tensors()
-        if not params:
-            return _FusedApply.apply(points, self)
-        return _PostOpApply.apply(points, self, *params)
+    def _vjp(self, points, grad_out, want_in, want_params):
+        """The points' gradient from this wrapper's ``jacobian_device``; the wrapped object's tensors'
+        gradients are its VJP of the cotangent mapped through this wrapper."""
+        gin, grads = super()._vjp(points, grad_out, want_in, False)
+        if want_params:
+            inner = self.fun.evaluate_device(points)
+            grads = self.fun._param_vjp(points, self._inner_cotangent(inner, grad_out))
+        return gin, grads
 
 
 class Saturation(_PostOp):
@@ -754,10 +737,15 @@ class Triangulation(DeterministicFunction):
         leaf = self._param_dev
         return [leaf] if leaf is not None and leaf.requires_grad else []
 
-    def _param_vjp(self, points, grad_out):
-        _, gflat, _ = _function_vjp(self, points, grad_out, want_in=False,
-                                    nparams=self._param_dev.numel())
-        return [gflat.view(self._param_dev.shape).to(self._param_dev.device)]
+    def _vjp(self, points, grad_out, want_in, want_params):
+        """The points' gradient from ``jacobian_device``; the vertex table's is one
+        ``slb_function_vjp`` call (the transpose of the lookup, summed in a fixed order)."""
+        gin, grads = super()._vjp(points, grad_out, want_in, False)
+        if want_params:
+            _, gflat, _ = _function_vjp(self, points, grad_out, want_in=False,
+                                        nparams=self._param_dev.numel())
+            grads = [gflat.view(self._param_dev.shape).to(self._param_dev.device)]
+        return gin, grads
 
     @property
     def version(self):
@@ -788,12 +776,6 @@ class Triangulation(DeterministicFunction):
         d.grid = self.discretization.descriptor(need_points=True)
         return d
 
-    def torch(self, points):
-        """``tri(points)`` as one autograd node with inputs (points, vertex table): the points'
-        gradient is ``Function.torch``'s, the vertex values' is one ``slb_function_vjp`` call (the
-        transpose of the lookup, summed in a fixed order)."""
-        return _TriangulationApply.apply(points, self, self._param_dev)
-
     def gradient_function(self):
         """The gradient of the interpolant as a fusable function object (one value column)."""
         return TriangulationGradient(self)
@@ -811,29 +793,6 @@ class Triangulation(DeterministicFunction):
             lim = dev.to_device(np.asarray(self.discretization.limits, dtype=np.float64))
             grad = grad * ((points >= lim[:, 0]) & (points <= lim[:, 1])).to(torch.float64)
         return grad.unsqueeze(1)
-
-
-class _TriangulationApply(torch.autograd.Function):
-    """A Triangulation in torch's autograd graph with its vertex table as an input."""
-
-    @staticmethod
-    def forward(ctx, points, fun, vertex_values):
-        points = points.detach().contiguous()
-        ctx.fun = fun
-        ctx.save_for_backward(points, vertex_values)  # a table write before backward raises
-        return fun.evaluate_device(points)
-
-    @staticmethod
-    @torch.autograd.function.once_differentiable
-    def backward(ctx, grad_out):
-        points, _ = ctx.saved_tensors
-        fun, grad_out = ctx.fun, grad_out.contiguous()
-        gin = gv = None
-        if ctx.needs_input_grad[0]:
-            gin = torch.einsum("no,noi->ni", grad_out, fun.jacobian_device(points))
-        if ctx.needs_input_grad[2]:
-            (gv,) = fun._param_vjp(points, grad_out)
-        return gin, None, gv
 
 
 class TriangulationGradient(DeterministicFunction):
@@ -929,6 +888,11 @@ class InvertedPendulum(DeterministicFunction):
         """d x+ / d [x, u] through the ten Euler sub-steps, [n, 2, 3] (``slb_function_vjp``)."""
         return _unit_vjp_jacobian(self, points)
 
+    def _vjp(self, points, grad_out, want_in, want_params):
+        """The points' gradient as one ``slb_function_vjp`` call (``jacobian_device`` makes one per
+        output)."""
+        return (_function_vjp(self, points, grad_out)[0] if want_in else None), []
+
 
 class CartPole(DeterministicFunction):
     """Cart-pole (``examples/utilities.py:292-437``)."""
@@ -972,6 +936,8 @@ class CartPole(DeterministicFunction):
     def jacobian_device(self, points):
         """d x+ / d [x, u] through the ten Euler sub-steps, [n, 4, 5] (``slb_function_vjp``)."""
         return _unit_vjp_jacobian(self, points)
+
+    _vjp = InvertedPendulum._vjp
 
 
 def _param_device():
@@ -1042,21 +1008,18 @@ class _TrainableNetwork(DeterministicFunction):
             self._packed_version = v
         return self._packed
 
-    def torch(self, points):
-        """``fun(points)`` on a device tensor [n, in] as one autograd node: forward = the fused
-        evaluation, backward = one ``slb_function_vjp`` call giving the gradients of ``points`` and
-        of every tensor in ``parameters``."""
-        return _NetworkApply.apply(points, self, *self._params)
-
     def jacobian_device(self, points):
         return _unit_vjp_jacobian(self, points)
 
     def _trainable_tensors(self):
         return list(self._params)
 
-    def _param_vjp(self, points, grad_out):
-        _, gflat, _ = _function_vjp(self, points, grad_out, False, self._packed_device().numel())
-        return self._grads_like(gflat, self._params)
+    def _vjp(self, points, grad_out, want_in, want_params):
+        """One ``slb_function_vjp`` call for the points and every parameter."""
+        gin, gflat, _ = _function_vjp(self, points, grad_out, want_in,
+                                      self._packed_device().numel() if want_params else 0)
+        return (gin.to(points.device) if gin is not None else None,
+                self._grads_like(gflat, self._params) if want_params else [])
 
     def vjp(self, points, grad_out, want_out=False):
         """(grad_in [n, in], [grad of each parameter], recomputed forward or None) for the cotangent
@@ -1069,32 +1032,6 @@ class _TrainableNetwork(DeterministicFunction):
         """The flat parameter gradient as one tensor per parameter, each on its parameter's device
         (a network built before ``torch.cuda.set_device`` keeps its leaves where they were made)."""
         return [g.to(p.device) for g, p in zip(self._unpack_grads(gflat), params)]
-
-
-class _NetworkApply(torch.autograd.Function):
-    """A NeuralNetwork / LyapunovNetwork in torch's autograd graph with its parameters as inputs."""
-
-    @staticmethod
-    def forward(ctx, points, fun, *params):
-        points = points.detach().contiguous()
-        ctx.fun = fun
-        ctx.save_for_backward(points, *params)       # torch refuses backward after an in-place update
-        return fun.evaluate_device(points)
-
-    @staticmethod
-    @torch.autograd.function.once_differentiable
-    def backward(ctx, grad_out):
-        # the VJP kernel is not itself differentiable: double backward raises instead of treating
-        # the gradient as a constant
-        points, params = ctx.saved_tensors[0], ctx.saved_tensors[1:]
-        fun = ctx.fun
-        want_params = any(ctx.needs_input_grad[2:])
-        gin, gflat, _ = _function_vjp(fun, points, grad_out, ctx.needs_input_grad[0],
-                                      fun._packed_device().numel() if want_params else 0)
-        if gin is not None:
-            gin = gin.to(points.device)
-        grads = fun._grads_like(gflat, params) if want_params else [None] * len(params)
-        return (gin, None) + tuple(grads)
 
 
 class LyapunovNetwork(_TrainableNetwork):
@@ -1309,6 +1246,8 @@ class NeuralNetwork(_TrainableNetwork):
         if not self.built:
             self._create(input_dim)
 
+    _build = build
+
     def _set_weights_biases(self, weights, biases):
         dims = self._dims
         weights = [np.asarray(w.detach().cpu().numpy() if isinstance(w, torch.Tensor) else w,
@@ -1414,10 +1353,6 @@ class NeuralNetwork(_TrainableNetwork):
         if pts.dim() == 2:
             self.build(pts.shape[1])
         return super().evaluate_device(pts)
-
-    def torch(self, points):
-        self.build(points.shape[1])
-        return super().torch(points)
 
 
 # =============================================================================== Gaussian processes
