@@ -80,7 +80,13 @@ enum slb_fn_kind {
 #define SLB_FLAG_GRADIENT 32u  /* TRIANGULATION with one output column: return the d partial
                                   derivatives of the piecewise-linear interpolant instead of its
                                   value (Triangulation.gradient, functions.py:1260-1326, 1506-1510);
-                                  out_dim = d                                              */
+                                  out_dim = d.
+                                  LYAPUNOV_NN, or MLP whose output width is 1: return the input
+                                  gradient d f / d x (tf.gradients(V(x), x), the Lipschitz lambda of
+                                  lyapunov_function_learning.ipynb cell 19), in_dim columns before
+                                  any NORM1 / MAXABS / SCALE; out_dim = in_dim <= SLB_MAX_OUT.  Equal
+                                  bit for bit to slb_function_vjp's grad_in for grad_out = 1, which
+                                  rejects the flag (its VJP would be a Hessian-vector product) */
 #define SLB_FLAG_MAXABS  64u   /* tf.reduce_max(tf.abs(.), axis=1, keepdims=True): the
                                   Lipschitz lambda of examples/inverted_pendulum.ipynb cell 14;
                                   applied after saturate, reduces to 1 column              */
@@ -207,7 +213,8 @@ typedef struct slb_gp_stack {
 
 /* ---- one Lyapunov sweep: the graph of lyapunov.py:433-441 -----------------------------
  * Shapes.  A function's COLUMNS are what it returns after its post-ops: out_dim, except 1 for
- * QUADRATIC and LYAPUNOV_NN, 2 for PENDULUM, 4 for CARTPOLE, and 1 after NORM1 or MAXABS.  With
+ * QUADRATIC and LYAPUNOV_NN, 2 for PENDULUM, 4 for CARTPOLE, in_dim for a network gradient
+ * (SLB_FLAG_GRADIENT on LYAPUNOV_NN / MLP with out_dim = in_dim), and 1 after NORM1 or MAXABS.  With
  * d = grid.ndim and m = the policy's columns:
  *   policy        d inputs, m = 1..SLB_MAX_ACT columns
  *   dynamics      d + m inputs, d columns                   (gp.num_outputs == 0)

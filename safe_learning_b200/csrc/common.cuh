@@ -473,6 +473,18 @@ SLB_DEV void eval_cartpole(const slb_function& f, const double* in, double* out)
 // (0 tanh, 1 relu, 2 identity); `matrix` holds the layer kernels [out_i, in_i] back to back
 // (kernel_i = [W^T W + eps I; W_extra], built on the host).  Widths up to SLB_NN_MAX_WIDTH.
 #define SLB_NN_MAX_WIDTH 64
+
+// The activations of both networks (0 tanh, 1 relu, 2 identity) and their derivatives from the
+// activation's output h (tanh' = 1 - h^2, ReLU' = [h > 0], so 0 at exactly 0, as TF's).  The VJP kernel
+// (network_grad.cu) and network_input_gradient below compile these same expressions.
+SLB_DEV double activate(double acc, int act) {
+    return act == 0 ? tanh(acc) : (act == 1 ? fmax(acc, 0.0) : acc);
+}
+
+SLB_DEV double activate_grad(double h, int act) {
+    return act == 0 ? 1.0 - h * h : (act == 1 ? (h > 0.0 ? 1.0 : 0.0) : 1.0);
+}
+
 SLB_DEV void eval_lyapunov_nn(const slb_function& f, const double* in, double* out) {
     double h[SLB_NN_MAX_WIDTH], g[SLB_NN_MAX_WIDTH];
     int width = f.in_dim;
@@ -527,8 +539,64 @@ SLB_DEV void eval_mlp(const slb_function& f, const double* in, double* out) {
     for (int k = 0; k < width; ++k) out[k] = f64mul(h[k], f.cparams[17]);
 }
 
+// SLB_FLAG_GRADIENT on SLB_FN_LYAPUNOV_NN or a one-output SLB_FN_MLP: out = d f / d x at one point
+// (in_dim columns).  Reverse mode in vjp_network_kernel's operation order (network_grad.cu) for the
+// cotangent 1: the forward of eval_lyapunov_nn / eval_mlp, delta = 2 h (LyapunovNetwork) or output_scale
+// (MLP) times activate_grad(h), then per input k the fma chain over the layer's outputs in ascending
+// order from 0.0.  The result equals slb_function_vjp(grad_out = 1).grad_in bit for bit.
+// Four width-64 arrays per thread: the activations are not stored, the forward is recomputed up to
+// layer l + 1 for the backward step through layer l (L (L + 1) / 2 layer evaluations; 6 for three
+// layers).  Never inlined, so the kernels that inline eval_fn carry one call site, not this body.
+static __device__ __noinline__ int network_input_gradient(const slb_function& f, const double* in, double* out) {
+    double h[SLB_NN_MAX_WIDTH], g[SLB_NN_MAX_WIDTH];          // forward: a layer's input and output
+    double d[SLB_NN_MAX_WIDTH], e[SLB_NN_MAX_WIDTH];          // backward: delta of layer l, dV/d(its input)
+    const int layers = (int)f.cparams[0];
+    const bool mlp = f.kind == SLB_FN_MLP;
+    const bool use_bias = mlp && f.cparams[18] != 0.0;
+    for (int l = layers - 1; l >= 0; --l) {
+        // forward through layers 0..l: h = the output of layer l, W = its weight [wo, wi]
+        int width = f.in_dim;
+        for (int k = 0; k < width; ++k) h[k] = in[k];
+        const double* P = f.matrix;
+        const double* W = P;
+        int wi = width;
+        for (int j = 0; j <= l; ++j) {
+            const int od = (int)f.cparams[1 + j];
+            const int act = (int)f.cparams[9 + j];
+            const bool bias = use_bias && (j + 1 < layers);
+            const double* b = P + (size_t)od * width;
+            for (int o = 0; o < od; ++o) {
+                const double* row = P + (size_t)o * width;
+                double acc = f64mul(h[0], row[0]);
+                for (int k = 1; k < width; ++k) acc = f64add(acc, f64mul(h[k], row[k]));
+                if (bias) acc = f64add(acc, b[o]);
+                g[o] = activate(acc, act);
+            }
+            W = P;
+            wi = width;
+            P += (size_t)od * width + (bias ? od : 0);
+            width = od;
+            for (int k = 0; k < width; ++k) h[k] = g[k];
+        }
+        const int act = (int)f.cparams[9 + l];
+        if (l == layers - 1) {
+            for (int o = 0; o < width; ++o) d[o] = (mlp ? f.cparams[17] : 2.0 * h[o]) * activate_grad(h[o], act);
+        } else {
+            for (int o = 0; o < width; ++o) d[o] = e[o] * activate_grad(h[o], act);
+        }
+        for (int k = 0; k < wi; ++k) {
+            double s = 0.0;
+            for (int o = 0; o < width; ++o) s = fma(d[o], W[(size_t)o * wi + k], s);
+            e[k] = s;
+        }
+    }
+    for (int k = 0; k < f.in_dim; ++k) out[k] = e[k];
+    return f.in_dim;
+}
+
 // Evaluate a fused function object. `in` has f.in_dim entries, `out` receives the result
-// columns; returns the number of columns (1 after NORM1 / MAXABS).  slb_fn_columns (light.cu) states
+// columns; returns the number of columns (in_dim for a network under SLB_FLAG_GRADIENT, 1 after
+// NORM1 / MAXABS).  slb_fn_columns (light.cu) states
 // that number on the host, where it sizes the kernels and checks shapes: a change to one must be
 // made to the other.  In gp_sweep.cu (SLB_EVAL_NOINLINE) it
 // is deliberately NOT inlined: the tile kernel calls it five times per point (policy, V twice,
@@ -575,10 +643,19 @@ SLB_EVAL_ATTR int eval_fn(const slb_function& f, const double* in, double* out) 
     case SLB_FN_CARTPOLE:
         eval_cartpole(f, in, out); od = 4;
         break;
+    // SLB_NO_NETWORK_GRADIENT (value_opt.cu): the unit's host entry points reject network gradients, and
+    // its kernels are compiled without the call (with it, ptxas gives value_operator_kernel<5, 6> 128
+    // registers and about 850 bytes of spills)
     case SLB_FN_LYAPUNOV_NN:
+#ifndef SLB_NO_NETWORK_GRADIENT
+        if (f.flags & SLB_FLAG_GRADIENT) { od = network_input_gradient(f, in, out); break; }
+#endif
         eval_lyapunov_nn(f, in, out); od = 1;
         break;
     case SLB_FN_MLP:
+#ifndef SLB_NO_NETWORK_GRADIENT
+        if (f.flags & SLB_FLAG_GRADIENT) { od = network_input_gradient(f, in, out); break; }
+#endif
         eval_mlp(f, in, out);
         break;
     default:

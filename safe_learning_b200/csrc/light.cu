@@ -48,9 +48,26 @@ int slb_validate_range(const char* who, int64_t idx_begin, int64_t idx_end, int6
     return 0;
 }
 
+// SLB_FLAG_GRADIENT on a network with `outputs` outputs (network_input_gradient, common.cuh): x -> d f /
+// d x has in_dim columns, and every kernel array that receives them before a reduction holds SLB_MAX_OUT
+static int validate_network_gradient(const slb_function* f, const char* what, const char* name, int outputs) {
+    SLB_CHECK(outputs == 1,
+              "%s: the gradient flag needs a one-output %s; this one maps %d inputs to %d outputs (its "
+              "derivative is a Jacobian)", what, name, f->in_dim, outputs);
+    SLB_CHECK(f->in_dim <= SLB_MAX_OUT,
+              "%s: the gradient of a %s with %d inputs and %d output has more than SLB_MAX_OUT = %d columns",
+              what, name, f->in_dim, outputs, SLB_MAX_OUT);
+    SLB_CHECK(f->out_dim == f->in_dim, "%s: the gradient of a %s with %d inputs and %d output needs out_dim %d, "
+              "got %d", what, name, f->in_dim, outputs, f->in_dim, f->out_dim);
+    return 0;
+}
+
 int slb_validate_function(const slb_function* f, const char* what, int expect_in) {
-    SLB_CHECK(!(f->flags & SLB_FLAG_GRADIENT) || f->kind == SLB_FN_TRIANGULATION,
-              "%s: the gradient flag is only defined for Triangulation", what);
+    SLB_CHECK(!(f->flags & SLB_FLAG_GRADIENT) || f->kind == SLB_FN_TRIANGULATION || f->kind == SLB_FN_LYAPUNOV_NN ||
+              f->kind == SLB_FN_MLP,
+              "%s: the gradient flag is only defined for Triangulation, LyapunovNetwork and one-output "
+              "NeuralNetwork (kind %d)", what, f->kind);
+    const bool grad = (f->flags & SLB_FLAG_GRADIENT) != 0;
     SLB_CHECK(!((f->flags & SLB_FLAG_NORM1) && (f->flags & SLB_FLAG_MAXABS)),
               "%s: norm1 and maxabs reductions are exclusive", what);
     switch (f->kind) {
@@ -93,11 +110,12 @@ int slb_validate_function(const slb_function* f, const char* what, int expect_in
         SLB_CHECK(f->matrix != nullptr, "%s: LyapunovNetwork without kernels", what);
         const int layers = (int)f->cparams[0];
         SLB_CHECK(layers >= 1 && layers <= 8, "%s: LyapunovNetwork with %d layers (1..8)", what, layers);
-        SLB_CHECK(f->in_dim >= 1 && f->in_dim <= SLB_MAX_IN && f->out_dim == 1,
+        SLB_CHECK(f->in_dim >= 1 && f->in_dim <= SLB_MAX_IN && (grad || f->out_dim == 1),
                   "%s: LyapunovNetwork maps <=%d inputs to 1 output", what, SLB_MAX_IN);
         for (int l = 0; l < layers; ++l)
             SLB_CHECK(f->cparams[1 + l] >= 1 && f->cparams[1 + l] <= 64,
                       "%s: LyapunovNetwork layer %d width %g outside 1..64", what, l, f->cparams[1 + l]);
+        if (grad && validate_network_gradient(f, what, "LyapunovNetwork", 1)) return 1;
         break;
     }
     case SLB_FN_MLP: {
@@ -109,8 +127,12 @@ int slb_validate_function(const slb_function* f, const char* what, int expect_in
         for (int l = 0; l < layers; ++l)
             SLB_CHECK(f->cparams[1 + l] >= 1 && f->cparams[1 + l] <= 64,
                       "%s: NeuralNetwork layer %d width %g outside 1..64", what, l, f->cparams[1 + l]);
-        SLB_CHECK((int)f->cparams[layers] == f->out_dim && f->out_dim <= SLB_MAX_OUT,
-                  "%s: NeuralNetwork output width must equal out_dim (<= %d)", what, SLB_MAX_OUT);
+        if (grad) {
+            if (validate_network_gradient(f, what, "NeuralNetwork", (int)f->cparams[layers])) return 1;
+        } else {
+            SLB_CHECK((int)f->cparams[layers] == f->out_dim && f->out_dim <= SLB_MAX_OUT,
+                      "%s: NeuralNetwork output width must equal out_dim (<= %d)", what, SLB_MAX_OUT);
+        }
         break;
     }
     default:
@@ -123,10 +145,14 @@ int slb_validate_function(const slb_function* f, const char* what, int expect_in
 }
 
 // The columns eval_fn (common.cuh) returns for f: the kind's count, then 1 after NORM1 / MAXABS.
-// Host code (and Python, through slb_function_columns) sizes kernels and checks shapes with this number
-// and never with out_dim: a change to eval_fn's return value must be made here too.
+// A network gradient (SLB_FLAG_GRADIENT on LYAPUNOV_NN / MLP with out_dim = in_dim, the shape
+// slb_validate_function requires) returns in_dim; a network descriptor that validation rejects keeps its
+// kind's count.  Host code (and Python, through slb_function_columns) sizes kernels and checks shapes
+// with this number and never with out_dim: a change to eval_fn's return value must be made here too.
 int slb_fn_columns(const slb_function& f) {
     if (f.flags & (SLB_FLAG_NORM1 | SLB_FLAG_MAXABS)) return 1;
+    const bool network = f.kind == SLB_FN_LYAPUNOV_NN || f.kind == SLB_FN_MLP;
+    if (network && (f.flags & SLB_FLAG_GRADIENT) && f.out_dim == f.in_dim) return f.in_dim;
     switch (f.kind) {
     case SLB_FN_QUADRATIC: case SLB_FN_LYAPUNOV_NN: return 1;
     case SLB_FN_PENDULUM: return 2;

@@ -59,15 +59,6 @@ struct net_shape {
     double scale;                 // MLP output_scale
 };
 
-SLB_DEV double activate(double acc, int act) {
-    return act == 0 ? tanh(acc) : (act == 1 ? fmax(acc, 0.0) : acc);
-}
-
-// d act / d pre-activation from the activation's output h
-SLB_DEV double activate_grad(double h, int act) {
-    return act == 0 ? 1.0 - h * h : (act == 1 ? (h > 0.0 ? 1.0 : 0.0) : 1.0);
-}
-
 __global__ void __launch_bounds__(NT) vjp_network_kernel(
         const __grid_constant__ net_shape S, const double* __restrict__ P, const double* __restrict__ x,
         int64_t n, const double* __restrict__ gout, double* __restrict__ gin, double* __restrict__ out,
@@ -344,6 +335,9 @@ int vjp_validate(const slb_function* fn, const char* what) {
               fn->kind == SLB_FN_CARTPOLE || fn->kind == SLB_FN_TRIANGULATION,
               "%s: function kind %d has no VJP (NeuralNetwork, LyapunovNetwork, InvertedPendulum, CartPole, "
               "Triangulation)", what, fn->kind);
+    SLB_CHECK(!(fn->flags & SLB_FLAG_GRADIENT) || (fn->kind != SLB_FN_MLP && fn->kind != SLB_FN_LYAPUNOV_NN),
+              "%s: the VJP of a network gradient (SLB_FLAG_GRADIENT) is a Hessian-vector product, which is "
+              "not implemented", what);
     const uint32_t allowed = fn->kind == SLB_FN_TRIANGULATION ? SLB_FLAG_PROJECT : 0u;   // not a post-op
     SLB_CHECK((fn->flags & ~allowed) == 0,
               "%s: post-op flags 0x%x are not differentiated here (compose them in torch)", what, fn->flags);

@@ -14,6 +14,9 @@
 //              gamma rho / (1 - gamma rho) ||v_k - v_{k-1}||_inf  <=  tol max(1, ||v_k||_inf),
 //              rho = max_i sum_j |w_ij|.  One CTA with both iterates in shared memory for small grids,
 //              else one cooperative launch with a grid barrier per iteration.
+// A network gradient (SLB_FLAG_GRADIENT on a network) is not compiled into the assembly kernel, and
+// slb_value_operator rejects one as its policy, dynamics or reward.
+#define SLB_NO_NETWORK_GRADIENT
 #include "bellman.cuh"
 
 #include <cooperative_groups.h>
@@ -355,6 +358,10 @@ static int validate_value_table(const slb_function& value, const char* who) {
     return 0;
 }
 
+static bool network_gradient(const slb_function& f) {
+    return (f.flags & SLB_FLAG_GRADIENT) && (f.kind == SLB_FN_LYAPUNOV_NN || f.kind == SLB_FN_MLP);
+}
+
 template <typename IDX>
 static int launch_solve(cudaStream_t st, const solve_args& a, const void* cols, const double* W,
                         const double* R, double* v, void* workspace, unsigned long long* stats) {
@@ -396,6 +403,8 @@ int slb_value_operator(void* stream, const slb_bellman* cfg, int64_t idx_begin, 
     if (slb_validate_bellman(cfg, &m)) return 1;
     SLB_CHECK(!cfg->fixed_action, "slb_value_operator: the policy is evaluated, fixed_action must be 0");
     if (validate_value_table(cfg->value, "slb_value_operator")) return 1;
+    SLB_CHECK(!network_gradient(cfg->policy) && !network_gradient(cfg->dynamics) && !network_gradient(cfg->reward),
+              "slb_value_operator: a network gradient (SLB_FLAG_GRADIENT) is not compiled into the value operator");
     if (slb_validate_range("slb_value_operator", idx_begin, idx_end, cfg->grid.nindex)) return 1;
     SLB_CHECK(stats_dev != nullptr, "slb_value_operator: null stats");
     const int64_t n = idx_end - idx_begin;

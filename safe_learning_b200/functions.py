@@ -32,7 +32,7 @@ config = Configuration()
 __all__ = ["DimensionError", "GridWorld", "Function", "DeterministicFunction",
            "UncertainFunction", "ConstantFunction", "LinearSystem", "QuadraticFunction",
            "Saturation", "AbsFunction", "Norm1Function", "MaxAbsFunction", "ScaledFunction",
-           "Triangulation", "TriangulationGradient",
+           "Triangulation", "TriangulationGradient", "NetworkGradient",
            "Kernel", "RBF", "Matern12", "Matern32", "Matern52", "Linear", "Constant", "Bias",
            "White", "Sum", "Add", "Product", "Prod", "kernels", "Likelihood", "GPRCached", "GPR",
            "GaussianProcess", "FunctionStack",
@@ -1033,6 +1033,10 @@ class _TrainableNetwork(DeterministicFunction):
         (a network built before ``torch.cuda.set_device`` keeps its leaves where they were made)."""
         return [g.to(p.device) for g, p in zip(self._unpack_grads(gflat), params)]
 
+    def gradient_function(self):
+        """``x -> d net(x) / dx`` as a fusable function object (a network with one output)."""
+        return NetworkGradient(self)
+
 
 class LyapunovNetwork(_TrainableNetwork):
     """Positive-definite network ``V(x) = |phi(x)|^2`` (``examples/utilities.py:48-104``):
@@ -1159,12 +1163,11 @@ class LyapunovNetwork(_TrainableNetwork):
         return grads
 
     def gradient(self, points):
-        """dV/dx at the points, numpy ``[n, d]`` (``tf.gradients(V(x), x)`` of the notebooks)."""
+        """dV/dx at the points, numpy ``[n, d]`` (``tf.gradients(V(x), x)`` of the notebooks), from
+        ``gradient_function()``."""
         pts = dev.to_device(concatenate_inputs([points]) if not isinstance(points, torch.Tensor)
                             else points)
-        gin, _, _ = _function_vjp(self, pts, torch.ones((pts.shape[0], 1), dtype=torch.float64,
-                                                          device=pts.device))
-        return gin.cpu().numpy()
+        return self.gradient_function().evaluate_device(pts).cpu().numpy()
 
 
 class NeuralNetwork(_TrainableNetwork):
@@ -1353,6 +1356,55 @@ class NeuralNetwork(_TrainableNetwork):
         if pts.dim() == 2:
             self.build(pts.shape[1])
         return super().evaluate_device(pts)
+
+
+class NetworkGradient(DeterministicFunction):
+    """``x -> d net(x) / dx`` of a ``LyapunovNetwork`` or a one-output ``NeuralNetwork``
+    (``tf.gradients(V(x), x)``: the Lipschitz lambda of ``lyapunov_function_learning.ipynb`` cell 19),
+    evaluated inside the fused kernels (``SLB_FLAG_GRADIENT``): reverse mode through the network at
+    each point, bit-identical to the network's VJP with cotangent 1.  Its ``torch`` evaluates; its
+    backward (the network's second derivative) is not implemented."""
+
+    def __init__(self, net, name="network_gradient"):
+        super().__init__(name)
+        if not isinstance(net, _TrainableNetwork):
+            raise TypeError("NetworkGradient wraps a LyapunovNetwork or NeuralNetwork")
+        self.net = net
+
+    @property
+    def input_dim(self):
+        return self.net.input_dim
+
+    @property
+    def output_dim(self):
+        return self.net.input_dim
+
+    @property
+    def parameters(self):
+        return self.net.parameters
+
+    @property
+    def version(self):
+        return ("grad", self.net.version)
+
+    def descriptor(self):
+        if self.net.output_dim != 1:
+            raise DimensionError("the fused gradient needs a network with one output, not %d (the "
+                                 "Jacobian of a multi-output network is not fused)" % self.net.output_dim)
+        d = self.net.descriptor()                  # an unbuilt NeuralNetwork raises DimensionError
+        if d.in_dim > nat.SLB_MAX_OUT:
+            raise DimensionError("the fused gradient of a network has at most %d input columns, not %d"
+                                 % (nat.SLB_MAX_OUT, d.in_dim))
+        d.flags |= nat.FLAG_GRADIENT
+        d.out_dim = d.in_dim
+        return d
+
+    def _trainable_tensors(self):
+        return self.net._trainable_tensors()
+
+    def _vjp(self, points, grad_out, want_in, want_params):
+        raise NotImplementedError("the backward of NetworkGradient is the network's second derivative "
+                                  "(a Hessian-vector product), which has no device kernel")
 
 
 # =============================================================================== Gaussian processes

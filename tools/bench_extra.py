@@ -21,8 +21,11 @@
             LyapunovNetwork(2, [64, 64, 64], tanh) and the 2-64-64-1 ReLU MLP on 100, 1000 and 251^2
             points, against torch's autograd of the same network on the same GPU (fp64 cuBLAS), and the
             per-step time of three notebook training loops (value net, policy net, Lyapunov pre-training)
+  nn_lv     L_V = |dV/dx|_1 of a LyapunovNetwork fused into the sweeps (Norm1Function(V.gradient_function())):
+            the notebook's 251^2 update_safe_set fused against composed, a 256^2 GP sweep (M = 500) and the
+            C4 shape against a constant L_V, and the gradient evaluation against slb_function_vjp
 
-    python tools/bench_extra.py [bellman] [det] [c5] [shared] [roa] [reward_rollout] [value_opt] [train]
+    python tools/bench_extra.py [bellman] [det] [c5] [shared] [roa] [reward_rollout] [value_opt] [train] [nn_lv]
 """
 import json
 import os
@@ -605,6 +608,78 @@ def tri_train():
         print(json.dumps({"bench": "tri_train_loop", "loop": name, "ms_per_step": timed(step, steps=50),
                           "note": "median of CUDA events around one SGD step (forward, backward, update)",
                           **info}))
+
+
+def nn_lv():
+    """L_V = |dV/dx|_1 of a LyapunovNetwork fused as Norm1Function(V.gradient_function()):
+    (1) lyapunov_function_learning.ipynb's 251^2 update_safe_set (pendulum plant, saturated LQR, V =
+        LyapunovNetwork(2, [64, 64, 64], tanh), tau = sum(unit) / 2), fused against the composed path
+        through V.gradient;
+    (2) a 256^2 pendulum GP sweep (M = 500) with the same V: filtered update_safe_set and the share of points
+        each stage decides, with L_V = |dV/dx|_1 against a constant L_V;
+    (3) the C4 shape (make_cartpole 16^4, M = 200): L_V = |dV/dx|_1 against L_v = 1.0;
+    (4) slb_eval_function with the gradient flag against slb_function_vjp (cotangent 1) at 251^2 points."""
+    from safe_learning_b200 import functions as F
+    par = W.make_pendulum(num_points=251, M=8)
+    pl = par["plant"]
+    plant = sl.InvertedPendulum(normalization=[pl["state_norm"], pl["action_norm"]], **pl["true"])
+    policy = sl.Saturation(sl.LinearSystem(-par["K"]), -1., 1.)
+    V = sl.LyapunovNetwork(2, [64, 64, 64], ["tanh"] * 3, eps=1e-8, seed=21)
+    grid = sl.GridWorld(par["limits"], par["num_points"])
+    fused = sl.Lyapunov(grid, V, plant, par["L_dyn"], sl.Norm1Function(V.gradient_function()), par["tau"],
+                        policy, par["initial"])
+    composed = sl.Lyapunov(grid, V, plant, par["L_dyn"], lambda x: np.abs(V.gradient(x)).sum(1, keepdims=True),
+                           par["tau"], policy, par["initial"])
+    info = _gpu_info(fused.update_safe_set)
+    ms_f = timed(lambda: (fused.update_safe_set(), fused.safe_set), steps=20)
+    ms_c = timed(lambda: (composed.update_safe_set(), composed.safe_set), steps=5, warmup=1)
+    same = bool(np.array_equal(fused.safe_set, composed.safe_set)
+                and fused.feed_dict[fused.c_max] == composed.feed_dict[composed.c_max])
+    print(json.dumps({"bench": "nn_lv_notebook_update_safe_set", "grid": "251x251", "ms_fused": ms_f,
+                      "ms_composed": ms_c, "speedup": ms_c / ms_f, "same_safe_set_and_c_max": same,
+                      "note": "median of CUDA events around update_safe_set + the safe_set read-back", **info}))
+
+    gpar = W.make_pendulum(num_points=256, M=500)
+    base = W.build_product(gpar)
+    for name, lv in (("norm1_grad", sl.Norm1Function(V.gradient_function())), ("constant", 1.0)):
+        lyap = sl.Lyapunov(base.discretization, V, base.dynamics, gpar["L_dyn"], lv, gpar["tau"], base.policy,
+                           initial_set=gpar["initial"])
+        lyap.filter = True
+        ms = timed(lambda: (lyap.update_safe_set(), lyap.safe_set), steps=10)
+        lyap.reset_filter_stats()
+        lyap.compute_negative()
+        st = lyap.filter_stats
+        pts = max(st["points"], 1)
+        print(json.dumps({"bench": "nn_lv_gp_filtered_sweep", "grid": "256x256", "M": 500, "L_V": name,
+                          "ms_update_safe_set": ms,
+                          "stage1": "fp%d" % _stage1(lyap),
+                          "frac_prior": st["prior"] / pts, "frac_head": st["head"] / pts,
+                          "frac_refined": st["refined"] / pts, **info}))
+
+    cpar = W.make_cartpole(num_points=16, M=200)
+    cbase = W.build_product(cpar)
+    CV = cbase.lyapunov_function
+    for name, lv in (("norm1_grad", sl.Norm1Function(CV.gradient_function())), ("L_v=1.0", 1.0)):
+        lyap = sl.Lyapunov(cbase.discretization, CV, cbase.dynamics, cpar["L_dyn"], lv, cpar["tau"],
+                           cbase.policy, initial_set=cpar["initial"])
+        ms = timed(lambda: (lyap.update_safe_set(), lyap.safe_set), steps=10)
+        print(json.dumps({"bench": "nn_lv_c4_update_safe_set", "grid": "16^4", "M": 200, "L_V": name,
+                          "ms_update_safe_set": ms, **info}))
+
+    x = torch.tensor(grid.all_points, device="cuda")
+    g = V.gradient_function()
+    ones = torch.ones((x.shape[0], 1), dtype=torch.float64, device="cuda")
+    ms_eval = timed(lambda: g.evaluate_device(x), steps=50)
+    ms_vjp = timed(lambda: F._function_vjp(V, x, ones), steps=50)
+    print(json.dumps({"bench": "nn_lv_gradient_eval", "points": int(x.shape[0]),
+                      "ms_eval_function_gradient_flag": ms_eval, "ms_function_vjp": ms_vjp,
+                      "bit_identical": bool(torch.equal(g.evaluate_device(x), F._function_vjp(V, x, ones)[0])),
+                      **info}))
+
+
+def _stage1(lyap):
+    from safe_learning_b200 import _native as nat
+    return nat.load().slb_filter_stage1(lyap.sweep_descriptor())
 
 
 if __name__ == "__main__":
