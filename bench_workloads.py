@@ -303,3 +303,50 @@ def build_oracle(par, deterministic=False):
     if par["name"].startswith("cartpole"):
         return _cartpole_objects(ns, par, "oracle")
     return _pendulum_objects(ns, par, "oracle", deterministic)
+
+
+def notebook_policy_case(ns, M, batch=1000, seed=0, torch_dynamics=False):
+    """examples/inverted_pendulum.ipynb cell 17 at batch size `batch`: a NeuralNetwork([32, 32, 1], relu,
+    relu, tanh) policy trained by SGD on -mean(future_values(states, lyapunov=...)) against a FunctionStack
+    of two GPs with the notebook's kernel (cell 6) and the wrong model as linear prior mean, M of
+    make_pendulum's training points (M = 0: the prior-only stack the notebook starts from), a 55x55
+    Triangulation(project=True) value function V = -x^T P x, the Lyapunov function -V and the Lipschitz term
+    of cell 14, L_V = MaxAbsFunction(V.gradient_function()).  With `torch_dynamics` the PolicyIteration
+    gets the stack's torch_predict expression as a plain callable instead of the stack itself.
+    Returns a dict with rl, lyapunov, policy, dynamics, states (device tensor) and step(optimizer)."""
+    import torch
+    par = make_pendulum(num_points=55, M=max(M, 1), seed=seed)
+    X, Y = par["X"][:M], par["Y"][:M]
+    specs = notebook_pendulum_kernels([[0.05, 0.1, 0.02], [0.08, 0.12, 0.05]])
+    gps = []
+    for j in range(2):
+        gp = ns.GPRCached(X, Y[:, [j]], build_kernel(ns, specs[j]),
+                          mean_function=ns.LinearSystem(par["prior_rows"][j][None, :]),
+                          noise_variance=par["noise_variance"])
+        gps.append(ns.GaussianProcess(gp, beta=2.0))
+    dynamics = ns.FunctionStack(gps)
+    grid = ns.GridWorld(par["limits"], par["num_points"])
+    pts = grid.all_points
+    value = ns.Triangulation(grid, -np.sum(pts.dot(par["P"]) * pts, axis=1, keepdims=True), project=True)
+    policy = ns.NeuralNetwork([32, 32, 1], ["relu", "relu", "tanh"], seed=seed + 7)
+    reward = -ns.QuadraticFunction(np.diag([1.0, 1.0, 0.1]))
+    l_v = ns.MaxAbsFunction(value.gradient_function())
+    lyapunov = ns.Lyapunov(grid, -value, dynamics, par["L_dyn"], l_v, par["tau"], policy,
+                           initial_set=par["initial"])
+    if torch_dynamics:
+        def dyn(states, actions):
+            return dynamics._torch_expression(torch.cat((states, actions), dim=1))
+    else:
+        dyn = dynamics
+    rl = ns.PolicyIteration(policy, dyn, reward, value, gamma=0.98)
+    states = torch.tensor(np.random.default_rng(seed + 11).uniform(-1, 1, (batch, 2)), device="cuda")
+
+    def step(opt, lagrange_multiplier=1.0):
+        opt.zero_grad()
+        loss = -torch.mean(rl.future_values(states, lyapunov=lyapunov, lagrange_multiplier=lagrange_multiplier))
+        loss.backward()
+        opt.step()
+        return loss.detach()
+
+    return dict(rl=rl, lyapunov=lyapunov, policy=policy, dynamics=dynamics, value=value, states=states,
+                step=step, grid=grid, l_dyn=par["L_dyn"], tau=par["tau"], initial=par["initial"])

@@ -367,6 +367,19 @@ int slb_pivoted_subset(void* stream, const double* kernel_dev, int32_t M, int32_
  *      err = beta*sqrt(var) (want_var == 0) or the latent variance (want_var != 0). ------- */
 int slb_gp_predict(void* stream, const slb_gp_stack* gp, const double* points_dev, int64_t n,
                    double* mean_dev, double* err_dev, int32_t want_var);
+/* ---- reverse mode of slb_gp_predict (want_var == 0), the reference's tf.gradients through the GP
+ *      posterior (examples/inverted_pendulum.ipynb cells 9, 17):
+ *        grad_points_dev [n, d_in] = grad_mean^T d mean / d points + grad_err^T d (beta sigma) / d points,
+ *      OVERWRITTEN; grad_mean_dev / grad_err_dev [n, D], either may be NULL (not both).  With grad_err NULL
+ *      the call does no O(M^2) work: the mean gradient needs only slb_gp_output.gamma, O(M d_in) per point.
+ *      Where a variance is 0 the err gradient follows torch's sqrt backward (division by 2 sqrt(var) = 0:
+ *      inf or NaN).  Every sum runs in a fixed order without atomics: two calls give bit-identical results.
+ *      n == 0 launches nothing.  workspace_dev: >= slb_gp_vjp_workspace(gp, n) bytes (0 for every stack
+ *      here); the size function returns -1 for a stack it rejects. */
+int64_t slb_gp_vjp_workspace(const slb_gp_stack* gp, int64_t n);
+int slb_gp_vjp(void* stream, const slb_gp_stack* gp, const double* points_dev, int64_t n,
+               const double* grad_mean_dev, const double* grad_err_dev, double* grad_points_dev,
+               void* workspace_dev);
 
 /* ---- the fused Lyapunov sweep over flat grid indices [idx_begin, idx_end):
  *      index -> x (functions.py:714-731) -> u = policy(x) -> [x,u] -> GP mean / beta*sigma

@@ -29,7 +29,8 @@ UNITS += [("gp_sweep.o", "gp_sweep.cu", [], ["gp_args.h"]),
           ("value_opt.o", "value_opt.cu", [], ["bulk_copy.cuh", "exp2_tab512.cuh", "gp_mean_staged.cuh",
                                                "bellman.cuh"]),
           ("network_grad.o", "network_grad.cu", [], []),
-          ("triangulation_grad.o", "triangulation_grad.cu", [], [])]
+          ("triangulation_grad.o", "triangulation_grad.cu", [], []),
+          ("gp_grad.o", "gp_grad.cu", [], [])]
 SOURCES = sorted({u[1] for u in UNITS})
 
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]

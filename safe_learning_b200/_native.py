@@ -177,6 +177,8 @@ SIGNATURES = {
     "slb_function_vjp_workspace": (C.c_int64, [C.POINTER(SlbFunction), _i64]),
     "slb_function_vjp": (C.c_int, [_vp, C.POINTER(SlbFunction), _dp, _i64, _dp, _dp, _dp, _dp, _vp]),
     "slb_triangulation_rows": (C.c_int, [_vp, C.POINTER(SlbFunction), _dp, _i64, _vp, _dp]),
+    "slb_gp_vjp_workspace": (C.c_int64, [C.POINTER(SlbGpStack), _i64]),
+    "slb_gp_vjp": (C.c_int, [_vp, C.POINTER(SlbGpStack), _dp, _i64, _dp, _dp, _dp, _vp]),
 }
 
 _lib = None

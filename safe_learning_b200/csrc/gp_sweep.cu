@@ -64,6 +64,9 @@ int dispatch_gp_tile(cudaStream_t st, const slb_sweep& cfg, const slb_gp_args& a
 
 }  // namespace
 
+// for the other units whose kernels read the packed factors (gp_grad.cu)
+int slb_wait_for_factors(cudaStream_t st) { return wait_for_factors(st); }
+
 // implemented in light.cu
 int slb_launch_det_sweep(cudaStream_t st, const slb_sweep& cfg, const double* states, int64_t n,
                          int64_t idx_begin, uint8_t* negative, double* values, double* decrease,

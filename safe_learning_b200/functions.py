@@ -217,6 +217,14 @@ class Function(object):
             self._build(points.shape[1])
         return _FusedApply.apply(points, self, *self._trainable_tensors())
 
+    # the same forward as a torch expression of the points, differentiated instead of ``_vjp`` when a
+    # backward runs with create_graph=True; None: a second derivative raises
+    _torch_expression = None
+
+    def _forward_device(self, points):
+        """The forward of ``torch``'s node on contiguous device points."""
+        return self.evaluate_device(points)
+
     def _build(self, input_dim):
         """Create whatever depends on the input width before ``torch`` collects the trainable
         tensors (a network in the reference's convention); nothing here."""
@@ -257,23 +265,51 @@ class Function(object):
 
 class _FusedApply(torch.autograd.Function):
     """Fused CUDA evaluation of a Function object inside torch's autograd graph, with the object's
-    trainable tensors as inputs: the one node behind ``Function.torch``."""
+    trainable tensors as inputs: the one node behind ``Function.torch``.  An object whose forward
+    returns a tuple (the GP posterior: mean and beta * sigma) gives one node with several outputs; its
+    ``_vjp`` receives a tuple of cotangents, None for an output that does not reach the loss."""
 
     @staticmethod
     def forward(ctx, points, fun, *tensors):
-        points = points.detach().contiguous()
         ctx.fun = fun
+        if fun._torch_expression is not None:
+            # the points themselves: a backward with create_graph differentiates the torch expression
+            # on them, which needs their place in the graph
+            ctx.save_for_backward(points, *tensors)
+            ctx.set_materialize_grads(False)
+            return fun._forward_device(points.detach().contiguous())
+        points = points.detach().contiguous()
         ctx.save_for_backward(points, *tensors)      # torch refuses backward after an in-place update
-        return fun.evaluate_device(points)
+        return fun._forward_device(points)
+
+    @staticmethod
+    def backward(ctx, *grad_outs):
+        if torch.is_grad_enabled() and ctx.fun._torch_expression is not None:
+            # create_graph=True through an object that states its forward in torch operations: the
+            # first derivative as a graph, so that a second derivative exists
+            points, outs = ctx.saved_tensors[0], ctx.fun._torch_expression(ctx.saved_tensors[0])
+            outs = outs if isinstance(outs, tuple) else (outs,)
+            used = [(o, g) for o, g in zip(outs, grad_outs) if g is not None and o.requires_grad]
+            gin = None
+            if used:
+                (gin,) = torch.autograd.grad([o for o, _ in used], points, [g for _, g in used],
+                                             create_graph=True, allow_unused=True)
+            if gin is None:
+                gin = torch.zeros_like(points)
+            return (gin, None) + (None,) * (len(ctx.saved_tensors) - 1)
+        return _FusedApply._backward_once(ctx, *grad_outs)
 
     @staticmethod
     @torch.autograd.function.once_differentiable
-    def backward(ctx, grad_out):
+    def _backward_once(ctx, *grad_outs):
         # the VJPs are not differentiable themselves: double backward raises instead of treating the
         # gradient as a constant
         points, ntensors = ctx.saved_tensors[0], len(ctx.saved_tensors) - 1
-        gin, grads = ctx.fun._vjp(points, grad_out.contiguous(), ctx.needs_input_grad[0],
-                                  any(ctx.needs_input_grad[2:]))
+        if len(grad_outs) == 1:
+            grad_out = grad_outs[0].contiguous()
+        else:
+            grad_out = tuple(None if g is None else g.contiguous() for g in grad_outs)
+        gin, grads = ctx.fun._vjp(points, grad_out, ctx.needs_input_grad[0], any(ctx.needs_input_grad[2:]))
         return (gin, None) + tuple(grads or [None] * ntensors)
 
 
@@ -2230,7 +2266,65 @@ def _gp_predict(stack, points, want_var=False):
     return mean, err
 
 
-class GaussianProcess(UncertainFunction):
+def _gp_vjp(stack, points, grad_mean=None, grad_err=None):
+    """One ``slb_gp_vjp`` call: the points' gradient [n, d_in] (device tensor) for the cotangents of
+    the mean and of beta * sigma ([n, D] each, either may be None)."""
+    lib = nat.load()
+    pts = dev.to_device(points).contiguous()
+    if pts.dim() != 2 or pts.shape[1] != stack.input_dim:
+        raise DimensionError("GP expects %d input columns, got %s"
+                             % (stack.input_dim, tuple(pts.shape)))
+    n, D = pts.shape[0], stack.num_outputs
+    gm = None if grad_mean is None else dev.to_device(grad_mean).reshape(n, D).contiguous()
+    ge = None if grad_err is None else dev.to_device(grad_err).reshape(n, D).contiguous()
+    gin = dev.empty((n, stack.input_dim))
+    if n == 0:                        # (empty tensors have no data pointer to pass)
+        return gin
+    size = lib.slb_gp_vjp_workspace(stack, n)
+    if size < 0:
+        raise nat.NativeLibraryError("slb_gp_vjp_workspace: %s" % nat.last_error())
+    ws = torch.empty(size, dtype=torch.uint8, device=pts.device) if size else None
+    nat.check(lib.slb_gp_vjp(dev.stream(), stack, pts.data_ptr(), n, dev.ptr(gm), dev.ptr(ge),
+                             gin.data_ptr(), dev.ptr(ws)), "slb_gp_vjp")
+    return gin
+
+
+class _GaussianProcessNode(UncertainFunction):
+    """What ``GaussianProcess`` and ``FunctionStack`` share as one node of torch's autograd graph."""
+
+    def _members(self):
+        raise NotImplementedError
+
+    def torch(self, points):
+        """Stacked (mean, beta * sigma) [n, D] each, differentiable with respect to ``points``
+        (``functions.py:278-291, 507-515``): one autograd node whose forward is ``slb_gp_predict``
+        (equal to ``predict_device`` bit for bit) and whose backward is one ``slb_gp_vjp`` call; an
+        output that does not reach the loss costs nothing (a mean-only objective is O(M d_in) per
+        point).  A backward with create_graph=True differentiates ``GPRCached.torch_predict`` instead,
+        so second derivatives exist."""
+        return _FusedApply.apply(points, self)
+
+    def _forward_device(self, points):
+        return self.predict_device(points)
+
+    def _torch_expression(self, points):
+        """(mean, beta * sigma) in torch operations on the cached factor (``torch_predict``)."""
+        parts = [f.gaussian_process.torch_predict(points) for f in self._members()]
+        return (torch.cat([m for m, _ in parts], dim=1),
+                torch.cat([f.beta * torch.sqrt(v) for f, (_, v) in zip(self._members(), parts)], dim=1))
+
+    def vjp_device(self, points, grad_mean=None, grad_err=None):
+        """grad_mean^T d mean / d points + grad_err^T d (beta sigma) / d points, [n, d_in]."""
+        return _gp_vjp(self.gp_stack(), points, grad_mean, grad_err)
+
+    def _vjp(self, points, grad_out, want_in, want_params):
+        if not want_in:
+            return None, []
+        grad_mean, grad_err = grad_out
+        return _gp_vjp(self.gp_stack(), points.detach(), grad_mean, grad_err), []
+
+
+class GaussianProcess(_GaussianProcessNode):
     """``(mean, beta * sqrt(var))`` of a one-output GP (``functions.py:461-546``)."""
 
     def __init__(self, gaussian_process, beta=2., name="gaussian_process"):
@@ -2274,10 +2368,8 @@ class GaussianProcess(UncertainFunction):
     def predict_device(self, points, want_var=False):
         return _gp_predict(self.gp_stack(), points, want_var)
 
-    def torch(self, points):
-        """(mean, beta * sigma) as differentiable torch tensors [n, 1] (``functions.py:507-515``)."""
-        mean, var = self.gaussian_process.torch_predict(points)
-        return mean, self.beta * torch.sqrt(var)
+    def _members(self):
+        return [self]
 
     def update_feed_dict(self):
         """Reference hook (``functions.py:517-523``): hyper-parameters travel in the
@@ -2289,7 +2381,7 @@ class GaussianProcess(UncertainFunction):
         self.gaussian_process.append_data(x, y)
 
 
-class FunctionStack(UncertainFunction):
+class FunctionStack(_GaussianProcessNode):
     """Stack of one-output GPs, one per state dimension (``functions.py:254-307``)."""
 
     def __init__(self, functions, name="function_stack"):
@@ -2338,10 +2430,8 @@ class FunctionStack(UncertainFunction):
     def predict_device(self, points, want_var=False):
         return _gp_predict(self.gp_stack(), points, want_var)
 
-    def torch(self, points):
-        """Stacked (mean, beta * sigma), [n, D] each, differentiable (``functions.py:278-291``)."""
-        parts = [f.torch(points) for f in self.functions]
-        return torch.cat([p[0] for p in parts], dim=1), torch.cat([p[1] for p in parts], dim=1)
+    def _members(self):
+        return self.functions
 
     def add_data_point(self, x, y):
         for fun, yi in zip(self.functions, np.asarray(y).squeeze()):

@@ -17,7 +17,7 @@ import torch
 from . import _device as dev
 from . import _native as nat
 from .functions import (Function, FunctionStack, GaussianProcess, ScaledFunction, Triangulation,
-                        UncertainFunction)
+                        TriangulationGradient, UncertainFunction, _PostOp)
 
 __all__ = ["PolicyIteration", "OptimizationError"]
 
@@ -40,6 +40,13 @@ def _fusable(fn):
     except (NotImplementedError, TypeError, ValueError):
         return False
     return True
+
+
+def _on_triangulation_gradient(fn):
+    """True when ``fn`` is a ``TriangulationGradient`` under post-op wrappers."""
+    while isinstance(fn, _PostOp):
+        fn = fn.fun
+    return isinstance(fn, TriangulationGradient)
 
 
 def _triangulation_of(value_function):
@@ -100,8 +107,10 @@ class PolicyIteration(object):
         differentiates this graph with ``tf.gradients`` to optimise a parametric policy under the
         Lyapunov penalty, ``examples/inverted_pendulum.ipynb`` cell 17): every fused function
         object is one autograd node (CUDA evaluation forward, its device Jacobian backward,
-        ``Function.torch``), the GP mean / variance are torch operations on the cached Cholesky
-        factor.  ``policy`` may be any callable on tensors (e.g. a ``torch.nn.Module``), and
+        ``Function.torch``), and so is the GP posterior (``slb_gp_predict`` forward, ``slb_gp_vjp``
+        backward).  A Lipschitz term built on a ``TriangulationGradient`` (``MaxAbsFunction(
+        V.gradient_function())``, cell 14) passes no gradient, as in the reference.  ``policy`` may
+        be any callable on tensors (e.g. a ``torch.nn.Module``), and
         ``dynamics`` / ``reward_function`` any callable ``fn(states, actions)`` on tensors, as in the
         reference; gradients flow to ``actions`` / the policy's parameters (network weights,
         Triangulation ``vertex_values``) and to ``states`` if they require them."""
@@ -129,7 +138,14 @@ class PolicyIteration(object):
             v_fn, lv = lyapunov.lyapunov_function, lyapunov._lipschitz_lyapunov
             decrease = v_fn.torch(mean) - v_fn.torch(states)
             if err is not None:
-                lv_mu = lv.torch(mean) if isinstance(lv, Function) else float(lv)
+                if _on_triangulation_gradient(lv):
+                    # the reference's Triangulation.gradient is a py_func without a gradient
+                    # (functions.py:1501-1510): the factor is a constant of the next states
+                    lv_mu = lv.evaluate_device(mean.detach())
+                elif isinstance(lv, Function):
+                    lv_mu = lv.torch(mean)
+                else:
+                    lv_mu = float(lv)
                 decrease = decrease + (lv_mu * err).sum(dim=1, keepdim=True)
             threshold = dev.to_device(np.broadcast_to(
                 lyapunov.threshold(states.detach().cpu().numpy()), (states.shape[0], 1)).copy())

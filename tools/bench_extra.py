@@ -24,8 +24,12 @@
   nn_lv     L_V = |dV/dx|_1 of a LyapunovNetwork fused into the sweeps (Norm1Function(V.gradient_function())):
             the notebook's 251^2 update_safe_set fused against composed, a 256^2 GP sweep (M = 500) and the
             C4 shape against a constant L_V, and the gradient evaluation against slb_function_vjp
+  gp_vjp    reverse mode of the GP posterior (slb_gp_vjp): inverted_pendulum.ipynb cell 17's policy step
+            (batch 1000, notebook-kernel FunctionStack at M = 0, 50, 200) through the GP node against
+            torch_predict as a plain dynamics callable, and the VJP alone on C2's GPs (plain RBF, M = 500,
+            two factors) for 10^3, 10^4 and 65536 points against the forward and torch autograd
 
-    python tools/bench_extra.py [bellman] [det] [c5] [shared] [roa] [reward_rollout] [value_opt] [train] [nn_lv]
+    python tools/bench_extra.py [bellman] [det] [c5] [shared] [roa] [reward_rollout] [value_opt] [train] [nn_lv] [gp_vjp]
 """
 import json
 import os
@@ -675,6 +679,55 @@ def nn_lv():
                       "ms_eval_function_gradient_flag": ms_eval, "ms_function_vjp": ms_vjp,
                       "bit_identical": bool(torch.equal(g.evaluate_device(x), F._function_vjp(V, x, ones)[0])),
                       **info}))
+
+
+def gp_vjp():
+    """(1) examples/inverted_pendulum.ipynb cell 17: one SGD step on -mean(future_values(states, lyapunov=...))
+    for a NeuralNetwork([32, 32, 1]) policy, 1000 states, the notebook-kernel FunctionStack at M = 0, 50, 200, a
+    55x55 Triangulation value function and L_V = MaxAbsFunction(V.gradient_function())
+    (bench_workloads.notebook_policy_case), with GaussianProcess.torch's node against torch_predict;
+    (2) slb_gp_vjp alone on C2's stack (make_pendulum, plain RBF, M = 500, two factors): both cotangents and
+    mean only, against slb_gp_predict and torch autograd through torch_predict.  FLOPs: the algorithmic
+    count of the forward-mode err term, (1 + d_in) M (M + 1) per point and factor (one FMA per L^-1 entry
+    and right-hand side), over the DMMA peak of DESIGN.md section 6."""
+    info = None
+    for M in (0, 50, 200):
+        ms = {}
+        for label, torch_dynamics in (("node", False), ("torch_predict", True)):
+            case = W.notebook_policy_case(sl, M, torch_dynamics=torch_dynamics)
+            net = case["policy"]
+            net._build(2)
+            opt = torch.optim.SGD(net.parameters, lr=1e-3)
+            if info is None:
+                info = _gpu_info(lambda: case["step"](opt))
+            ms[label] = timed(lambda: case["step"](opt), steps=20, warmup=3)
+        print(json.dumps({"bench": "gp_vjp_cell17_policy_step", "batch": 1000, "M": M,
+                          "ms_node": ms["node"], "ms_torch_predict": ms["torch_predict"],
+                          "speedup": ms["torch_predict"] / ms["node"],
+                          "note": "median of CUDA events around zero_grad + forward + backward + SGD step", **info}))
+
+    par = W.make_pendulum(num_points=64, M=500)
+    stack = W.build_product(par).dynamics
+    din, M, nf = 3, 500, stack.gp_stack().num_factors
+    for n in (1000, 10000, 65536):
+        rng = np.random.default_rng(n)
+        x = torch.tensor(rng.uniform(-1, 1, (n, din)), device="cuda")
+        g = torch.tensor(rng.normal(size=(n, 2)), device="cuda")
+        ms_both = timed(lambda: stack.vjp_device(x, g, g), steps=20)
+        ms_mean = timed(lambda: stack.vjp_device(x, g, None), steps=20)
+        ms_fwd = timed(lambda: stack.predict_device(x), steps=20)
+
+        def autograd():
+            xg = x.clone().requires_grad_(True)
+            mean, err = stack._torch_expression(xg)
+            torch.autograd.grad((mean * g).sum() + (err * g).sum(), xg)
+
+        ms_torch = timed(autograd, steps=10)
+        flops = float(n) * nf * (1 + din) * M * (M + 1)
+        print(json.dumps({"bench": "gp_vjp_c2", "points": n, "M": M, "factors": nf, "ms_vjp": ms_both,
+                          "ms_vjp_mean_only": ms_mean, "ms_forward": ms_fwd, "ms_torch_autograd": ms_torch,
+                          "gflop_err_term": flops / 1e9, "tflops": flops / ms_both / 1e9,
+                          "share_of_dmma_peak": flops / ms_both / 1e9 / PEAK_TF, **info}))
 
 
 def _stage1(lyap):
