@@ -468,15 +468,31 @@ SLB_DEV void eval_cartpole(const slb_function& f, const double* in, double* out)
     for (int c = 0; c < 4; ++c) out[c] = s[c];
 }
 
-// ---- LyapunovNetwork (examples/utilities.py:85-104): net <- act(net . kernel_i^T), V = |net|^2.
-// cparams: [0] number of layers, [1 + i] output width of layer i, [9 + i] activation of layer i
-// (0 tanh, 1 relu, 2 identity); `matrix` holds the layer kernels [out_i, in_i] back to back
-// (kernel_i = [W^T W + eps I; W_extra], built on the host).  Widths up to SLB_NN_MAX_WIDTH.
+// ---- the fused networks: LyapunovNetwork (examples/utilities.py:85-104: h <- act(h . K_l^T), V = |h|^2)
+// and NeuralNetwork (functions.py:1702-1729: dense layers, output multiplied by output_scale).
+// Descriptor layout, written by _TrainableNetwork._network_descriptor (functions.py) and read only through
+// the accessors below: cparams [0] layers, [1 + l] output width of layer l, [9 + l] activation of layer l
+// (0 tanh, 1 relu, 2 identity), [17] the MLP's output_scale, [18] the MLP's use_bias.  `matrix` packs per
+// layer its weight [out, in] (one row per output; LyapunovNetwork's kernel [W^T W + eps I; W_extra], built
+// on the host), then its bias [out] if it has one.
+#define SLB_NN_MAX_LAYERS 8
 #define SLB_NN_MAX_WIDTH 64
+#define SLB_NN_HD __host__ __device__ __forceinline__
 
-// The activations of both networks (0 tanh, 1 relu, 2 identity) and their derivatives from the
-// activation's output h (tanh' = 1 - h^2, ReLU' = [h > 0], so 0 at exactly 0, as TF's).  The VJP kernel
-// (network_grad.cu) and network_input_gradient below compile these same expressions.
+SLB_NN_HD int nn_layers(const slb_function& f) { return (int)f.cparams[0]; }
+SLB_NN_HD int nn_out(const slb_function& f, int l) { return (int)f.cparams[1 + l]; }     // layer l's width
+// width l of the network: l = 0 its input, l >= 1 the output of layer l - 1
+SLB_NN_HD int nn_width(const slb_function& f, int l) { return l == 0 ? f.in_dim : nn_out(f, l - 1); }
+SLB_NN_HD int nn_act(const slb_function& f, int l) { return (int)f.cparams[9 + l]; }
+// with use_bias the MLP's hidden layers carry a bias; its output layer and LyapunovNetwork have none
+SLB_NN_HD bool nn_use_bias(const slb_function& f) { return f.kind == SLB_FN_MLP && f.cparams[18] != 0.0; }
+SLB_NN_HD bool nn_bias(const slb_function& f, int l) { return nn_use_bias(f) && l + 1 < nn_layers(f); }
+SLB_NN_HD double nn_scale(const slb_function& f) { return f.cparams[17]; }     // MLP only
+// doubles of a layer wi -> wo in the packed parameters: its weight [wo, wi], then its bias [wo] if it has one
+SLB_NN_HD int64_t nn_layer_size(int wi, int wo, bool bias) { return (int64_t)wo * wi + (bias ? wo : 0); }
+
+// The activations (0 tanh, 1 relu, 2 identity) and their derivatives from the activation's output h
+// (tanh' = 1 - h^2, ReLU' = [h > 0], so 0 at exactly 0, as TF's).
 SLB_DEV double activate(double acc, int act) {
     return act == 0 ? tanh(acc) : (act == 1 ? fmax(acc, 0.0) : acc);
 }
@@ -485,102 +501,89 @@ SLB_DEV double activate_grad(double h, int act) {
     return act == 0 ? 1.0 - h * h : (act == 1 ? (h > 0.0 ? 1.0 : 0.0) : 1.0);
 }
 
-SLB_DEV void eval_lyapunov_nn(const slb_function& f, const double* in, double* out) {
-    double h[SLB_NN_MAX_WIDTH], g[SLB_NN_MAX_WIDTH];
-    int width = f.in_dim;
-    for (int k = 0; k < width; ++k) h[k] = in[k];
-    const double* K = f.matrix;
-    const int layers = (int)f.cparams[0];
-    for (int l = 0; l < layers; ++l) {
-        const int od = (int)f.cparams[1 + l];
-        const int act = (int)f.cparams[9 + l];
-        for (int o = 0; o < od; ++o) {
-            const double* row = K + (size_t)o * width;
-            double acc = f64mul(h[0], row[0]);
-            for (int k = 1; k < width; ++k) acc = f64add(acc, f64mul(h[k], row[k]));
-            g[o] = act == 0 ? tanh(acc) : (act == 1 ? fmax(acc, 0.0) : acc);
-        }
-        K += (size_t)od * width;
-        width = od;
-        for (int k = 0; k < width; ++k) h[k] = g[k];
-    }
-    double v = f64mul(h[0], h[0]);
-    for (int k = 1; k < width; ++k) v = f64add(v, f64mul(h[k], h[k]));
-    out[0] = v;
+// One unit of a layer: act(x(0) w(0) + ... + x(n-1) w(n-1) [+ bias()]), products and sums rounded in
+// ascending k (f64mul / f64add, never contracted).  The accessors read the unit's operands; bias() is
+// called only when has_bias.  Every forward pass of the networks (eval_network, network_input_gradient's
+// recompute, vjp_network_kernel in network_grad.cu) computes its units here, so their activations and
+// ReLU masks agree bit for bit.
+template <class X, class W, class B>
+SLB_DEV double nn_unit(int n, X x, W w, bool has_bias, B bias, int act) {
+    double acc = f64mul(x(0), w(0));
+    for (int k = 1; k < n; ++k) acc = f64add(acc, f64mul(x(k), w(k)));
+    if (has_bias) acc = f64add(acc, bias());
+    return activate(acc, act);
 }
 
-// ---- NeuralNetwork inference (functions.py:1702-1729): dense layers, bias in the hidden layers
-// only, output layer without bias, result scaled by output_scale.  matrix = per layer the weight
-// [out_i, in_i] (already transposed to row-per-output) followed, for hidden layers with bias, by
-// the bias [out_i].
-SLB_DEV void eval_mlp(const slb_function& f, const double* in, double* out) {
+// a layer wi -> wo at one point: g = act(W h [+ b]) from its packed parameters P
+SLB_DEV void nn_layer(const double* P, int wi, int wo, bool bias, int act, const double* h, double* g) {
+    const double* b = P + (size_t)wo * wi;
+    for (int o = 0; o < wo; ++o) {
+        const double* row = P + (size_t)o * wi;
+        g[o] = nn_unit(wi, [&](int k) { return h[k]; }, [&](int k) { return row[k]; }, bias,
+                       [&] { return b[o]; }, act);
+    }
+}
+
+// KIND = f.kind.  LyapunovNetwork: out[0] = |h|^2; NeuralNetwork: out = h * output_scale (h = the last
+// layer's output).  One instance per kind, so each inlines without the other's epilogue or bias test.
+template <int KIND>
+SLB_DEV void eval_network(const slb_function& f, const double* in, double* out) {
     double h[SLB_NN_MAX_WIDTH], g[SLB_NN_MAX_WIDTH];
     int width = f.in_dim;
     for (int k = 0; k < width; ++k) h[k] = in[k];
     const double* P = f.matrix;
-    const int layers = (int)f.cparams[0];
-    const bool use_bias = f.cparams[18] != 0.0;
+    const int layers = nn_layers(f);
+    const bool use_bias = KIND == SLB_FN_MLP && nn_use_bias(f);
     for (int l = 0; l < layers; ++l) {
-        const int od = (int)f.cparams[1 + l];
-        const int act = (int)f.cparams[9 + l];
-        const bool bias = use_bias && (l + 1 < layers);
-        const double* b = P + (size_t)od * width;
-        for (int o = 0; o < od; ++o) {
-            const double* row = P + (size_t)o * width;
-            double acc = f64mul(h[0], row[0]);
-            for (int k = 1; k < width; ++k) acc = f64add(acc, f64mul(h[k], row[k]));
-            if (bias) acc = f64add(acc, b[o]);
-            g[o] = act == 0 ? tanh(acc) : (act == 1 ? fmax(acc, 0.0) : acc);
-        }
-        P += (size_t)od * width + (bias ? od : 0);
+        const int od = nn_out(f, l);
+        const bool bias = use_bias && l + 1 < layers;
+        nn_layer(P, width, od, bias, nn_act(f, l), h, g);
+        P += nn_layer_size(width, od, bias);
         width = od;
         for (int k = 0; k < width; ++k) h[k] = g[k];
     }
-    for (int k = 0; k < width; ++k) out[k] = f64mul(h[k], f.cparams[17]);
+    if constexpr (KIND == SLB_FN_MLP) {
+        for (int k = 0; k < width; ++k) out[k] = f64mul(h[k], nn_scale(f));
+    } else {
+        double v = f64mul(h[0], h[0]);
+        for (int k = 1; k < width; ++k) v = f64add(v, f64mul(h[k], h[k]));
+        out[0] = v;
+    }
 }
 
 // SLB_FLAG_GRADIENT on SLB_FN_LYAPUNOV_NN or a one-output SLB_FN_MLP: out = d f / d x at one point
 // (in_dim columns).  Reverse mode in vjp_network_kernel's operation order (network_grad.cu) for the
-// cotangent 1: the forward of eval_lyapunov_nn / eval_mlp, delta = 2 h (LyapunovNetwork) or output_scale
-// (MLP) times activate_grad(h), then per input k the fma chain over the layer's outputs in ascending
-// order from 0.0.  The result equals slb_function_vjp(grad_out = 1).grad_in bit for bit.
+// cotangent 1: the forward through nn_unit, delta = 2 h (LyapunovNetwork) or output_scale (MLP) times
+// activate_grad(h), then per input k the fma chain over the layer's outputs in ascending order from 0.0.
+// The result equals slb_function_vjp(grad_out = 1).grad_in bit for bit.
 // Four width-64 arrays per thread: the activations are not stored, the forward is recomputed up to
 // layer l + 1 for the backward step through layer l (L (L + 1) / 2 layer evaluations; 6 for three
 // layers).  Never inlined, so the kernels that inline eval_fn carry one call site, not this body.
 static __device__ __noinline__ int network_input_gradient(const slb_function& f, const double* in, double* out) {
     double h[SLB_NN_MAX_WIDTH], g[SLB_NN_MAX_WIDTH];          // forward: a layer's input and output
     double d[SLB_NN_MAX_WIDTH], e[SLB_NN_MAX_WIDTH];          // backward: delta of layer l, dV/d(its input)
-    const int layers = (int)f.cparams[0];
-    const bool mlp = f.kind == SLB_FN_MLP;
-    const bool use_bias = mlp && f.cparams[18] != 0.0;
+    const int layers = nn_layers(f);
+    const bool mlp = f.kind == SLB_FN_MLP, use_bias = nn_use_bias(f);
     for (int l = layers - 1; l >= 0; --l) {
-        // forward through layers 0..l: h = the output of layer l, W = its weight [wo, wi]
+        // forward through layers 0..l: h = the output of layer l, W = its weight [width, wi]
         int width = f.in_dim;
         for (int k = 0; k < width; ++k) h[k] = in[k];
         const double* P = f.matrix;
         const double* W = P;
         int wi = width;
         for (int j = 0; j <= l; ++j) {
-            const int od = (int)f.cparams[1 + j];
-            const int act = (int)f.cparams[9 + j];
-            const bool bias = use_bias && (j + 1 < layers);
-            const double* b = P + (size_t)od * width;
-            for (int o = 0; o < od; ++o) {
-                const double* row = P + (size_t)o * width;
-                double acc = f64mul(h[0], row[0]);
-                for (int k = 1; k < width; ++k) acc = f64add(acc, f64mul(h[k], row[k]));
-                if (bias) acc = f64add(acc, b[o]);
-                g[o] = activate(acc, act);
-            }
+            const int od = nn_out(f, j);
+            const bool bias = use_bias && j + 1 < layers;
+            nn_layer(P, width, od, bias, nn_act(f, j), h, g);
             W = P;
             wi = width;
-            P += (size_t)od * width + (bias ? od : 0);
+            P += nn_layer_size(width, od, bias);
             width = od;
             for (int k = 0; k < width; ++k) h[k] = g[k];
         }
-        const int act = (int)f.cparams[9 + l];
+        const int act = nn_act(f, l);
         if (l == layers - 1) {
-            for (int o = 0; o < width; ++o) d[o] = (mlp ? f.cparams[17] : 2.0 * h[o]) * activate_grad(h[o], act);
+            for (int o = 0; o < width; ++o) d[o] = (mlp ? nn_scale(f) : 2.0 * h[o]) * activate_grad(h[o], act);
         } else {
             for (int o = 0; o < width; ++o) d[o] = e[o] * activate_grad(h[o], act);
         }
@@ -650,13 +653,13 @@ SLB_EVAL_ATTR int eval_fn(const slb_function& f, const double* in, double* out) 
 #ifndef SLB_NO_NETWORK_GRADIENT
         if (f.flags & SLB_FLAG_GRADIENT) { od = network_input_gradient(f, in, out); break; }
 #endif
-        eval_lyapunov_nn(f, in, out); od = 1;
+        eval_network<SLB_FN_LYAPUNOV_NN>(f, in, out); od = 1;
         break;
     case SLB_FN_MLP:
 #ifndef SLB_NO_NETWORK_GRADIENT
         if (f.flags & SLB_FLAG_GRADIENT) { od = network_input_gradient(f, in, out); break; }
 #endif
-        eval_mlp(f, in, out);
+        eval_network<SLB_FN_MLP>(f, in, out);
         break;
     default:
         for (int o = 0; o < od; ++o) out[o] = __longlong_as_double(0x7ff8000000000000ll);

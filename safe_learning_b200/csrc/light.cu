@@ -106,32 +106,26 @@ int slb_validate_function(const slb_function* f, const char* what, int expect_in
     case SLB_FN_CARTPOLE:
         SLB_CHECK(f->in_dim == 5 && f->out_dim == 4, "%s: cart-pole must map 5 -> 4", what);
         break;
-    case SLB_FN_LYAPUNOV_NN: {
-        SLB_CHECK(f->matrix != nullptr, "%s: LyapunovNetwork without kernels", what);
-        const int layers = (int)f->cparams[0];
-        SLB_CHECK(layers >= 1 && layers <= 8, "%s: LyapunovNetwork with %d layers (1..8)", what, layers);
-        SLB_CHECK(f->in_dim >= 1 && f->in_dim <= SLB_MAX_IN && (grad || f->out_dim == 1),
-                  "%s: LyapunovNetwork maps <=%d inputs to 1 output", what, SLB_MAX_IN);
-        for (int l = 0; l < layers; ++l)
-            SLB_CHECK(f->cparams[1 + l] >= 1 && f->cparams[1 + l] <= 64,
-                      "%s: LyapunovNetwork layer %d width %g outside 1..64", what, l, f->cparams[1 + l]);
-        if (grad && validate_network_gradient(f, what, "LyapunovNetwork", 1)) return 1;
-        break;
-    }
-    case SLB_FN_MLP: {
-        SLB_CHECK(f->matrix != nullptr, "%s: NeuralNetwork without parameters", what);
-        const int layers = (int)f->cparams[0];
-        SLB_CHECK(layers >= 1 && layers <= 8, "%s: NeuralNetwork with %d layers (1..8)", what, layers);
-        SLB_CHECK(f->in_dim >= 1 && f->in_dim <= SLB_MAX_IN, "%s: NeuralNetwork input dim %d", what,
-                  f->in_dim);
-        for (int l = 0; l < layers; ++l)
-            SLB_CHECK(f->cparams[1 + l] >= 1 && f->cparams[1 + l] <= 64,
-                      "%s: NeuralNetwork layer %d width %g outside 1..64", what, l, f->cparams[1 + l]);
+    case SLB_FN_LYAPUNOV_NN:
+    case SLB_FN_MLP: {        // LyapunovNetwork has one output, NeuralNetwork its last layer's width
+        const char* name = f->kind == SLB_FN_MLP ? "NeuralNetwork" : "LyapunovNetwork";
+        SLB_CHECK(f->matrix != nullptr, "%s: %s without parameters", what, name);
+        const int layers = nn_layers(*f);
+        SLB_CHECK(layers >= 1 && layers <= SLB_NN_MAX_LAYERS, "%s: %s with %d layers (1..%d)", what, name,
+                  layers, SLB_NN_MAX_LAYERS);
+        SLB_CHECK(f->in_dim >= 1 && f->in_dim <= SLB_MAX_IN, "%s: %s input dim %d outside 1..%d", what, name,
+                  f->in_dim, SLB_MAX_IN);
+        for (int l = 1; l <= layers; ++l)
+            SLB_CHECK(nn_width(*f, l) >= 1 && nn_width(*f, l) <= SLB_NN_MAX_WIDTH,
+                      "%s: %s layer %d width %d outside 1..%d", what, name, l - 1, nn_width(*f, l),
+                      SLB_NN_MAX_WIDTH);
+        const int outputs = f->kind == SLB_FN_MLP ? nn_width(*f, layers) : 1;
         if (grad) {
-            if (validate_network_gradient(f, what, "NeuralNetwork", (int)f->cparams[layers])) return 1;
+            if (validate_network_gradient(f, what, name, outputs)) return 1;
         } else {
-            SLB_CHECK((int)f->cparams[layers] == f->out_dim && f->out_dim <= SLB_MAX_OUT,
-                      "%s: NeuralNetwork output width must equal out_dim (<= %d)", what, SLB_MAX_OUT);
+            SLB_CHECK(f->out_dim == outputs && outputs <= SLB_MAX_OUT,
+                      "%s: %s with %d outputs needs out_dim %d (<= %d), got %d", what, name, outputs, outputs,
+                      SLB_MAX_OUT, f->out_dim);
         }
         break;
     }
@@ -151,10 +145,11 @@ int slb_validate_function(const slb_function* f, const char* what, int expect_in
 // with this number and never with out_dim: a change to eval_fn's return value must be made here too.
 int slb_fn_columns(const slb_function& f) {
     if (f.flags & (SLB_FLAG_NORM1 | SLB_FLAG_MAXABS)) return 1;
-    const bool network = f.kind == SLB_FN_LYAPUNOV_NN || f.kind == SLB_FN_MLP;
-    if (network && (f.flags & SLB_FLAG_GRADIENT) && f.out_dim == f.in_dim) return f.in_dim;
     switch (f.kind) {
-    case SLB_FN_QUADRATIC: case SLB_FN_LYAPUNOV_NN: return 1;
+    case SLB_FN_LYAPUNOV_NN: case SLB_FN_MLP:
+        if ((f.flags & SLB_FLAG_GRADIENT) && f.out_dim == f.in_dim) return f.in_dim;
+        return f.kind == SLB_FN_MLP ? f.out_dim : 1;
+    case SLB_FN_QUADRATIC: return 1;
     case SLB_FN_PENDULUM: return 2;
     case SLB_FN_CARTPOLE: return 4;
     default: return f.out_dim;

@@ -5,9 +5,9 @@
 //
 // Networks (SLB_FN_MLP, SLB_FN_LYAPUNOV_NN): one CTA walks tiles of TP points.  Per tile it
 //   (1) recomputes the forward pass with every layer's activations in shared memory, column-major
-//       [unit][point] with a padded stride, in the operation order of eval_mlp / eval_lyapunov_nn
-//       (sequential k, __dmul_rn / __dadd_rn, the same tanh / fmax): the ReLU masks and tanh values
-//       it differentiates are exactly the forward's, and `out` is bit-identical to slb_eval_function;
+//       [unit][point] with a padded stride, through nn_unit (common.cuh), the unit eval_network computes
+//       with: the ReLU masks and tanh values it differentiates are exactly the forward's, and `out` is
+//       bit-identical to slb_eval_function;
 //   (2) runs the layers backwards: delta = dL/dh * act'(h) (tanh' = 1 - h^2, ReLU' = [h > 0], so 0 at
 //       exactly 0, as TF's), the layer's weight gradient sum_p delta_p a_p^T (and sum_p delta_p for the
 //       bias) accumulated into this CTA's row of the workspace, and dL/da = delta W for the layer below.
@@ -35,7 +35,7 @@ namespace {
 constexpr int TP = 32;            // points per tile (one warp's worth: unit-major loops are conflict-free)
 constexpr int TPS = TP + 1;       // padded column stride of the shared activation tables
 constexpr int NT = 256;           // threads per CTA
-constexpr int MAXL = 8;
+constexpr int MAXL = SLB_NN_MAX_LAYERS;
 constexpr int MAXW = SLB_NN_MAX_WIDTH;
 constexpr size_t SMEM_OPTIN = 227 * 1024;
 
@@ -79,7 +79,7 @@ __global__ void __launch_bounds__(NT) vjp_network_kernel(
             sm[k * TPS + p] = p < np ? x[(p0 + p) * in + k] : 0.0;
         }
         __syncthreads();
-        // ---- forward (eval_mlp / eval_lyapunov_nn order)
+        // ---- forward
         for (int l = 0; l < L; ++l) {
             const int wi = S.width[l], wo = S.width[l + 1], act = S.act[l];
             const double* a_in = sm + S.aoff[l];
@@ -89,10 +89,9 @@ __global__ void __launch_bounds__(NT) vjp_network_kernel(
             for (int i = tid; i < wo * TP; i += NT) {
                 const int o = i / TP, p = i % TP;
                 const double* row = W + (size_t)o * wi;
-                double acc = f64mul(a_in[p], __ldg(row));
-                for (int k = 1; k < wi; ++k) acc = f64add(acc, f64mul(a_in[k * TPS + p], __ldg(row + k)));
-                if (S.bias[l]) acc = f64add(acc, __ldg(b + o));
-                a_out[o * TPS + p] = activate(acc, act);
+                a_out[o * TPS + p] = nn_unit(wi, [&](int k) { return a_in[k * TPS + p]; },
+                                             [&](int k) { return __ldg(row + k); }, S.bias[l],
+                                             [&] { return __ldg(b + o); }, act);
             }
             __syncthreads();
         }
@@ -292,27 +291,25 @@ __global__ void __launch_bounds__(NT) vjp_plant_kernel(const __grid_constant__ s
 void network_shape(const slb_function& f, net_shape* S) {
     memset(S, 0, sizeof(*S));
     S->kind = f.kind;
-    S->layers = (int)f.cparams[0];
-    S->width[0] = f.in_dim;
-    const bool use_bias = f.kind == SLB_FN_MLP && f.cparams[18] != 0.0;
+    S->layers = nn_layers(f);
     int64_t off = 0;
     int32_t aoff = 0;
     S->maxw = 1;
-    for (int l = 0; l < S->layers; ++l) {
-        S->width[l + 1] = (int)f.cparams[1 + l];
-        S->act[l] = (int)f.cparams[9 + l];
-        S->bias[l] = use_bias && l + 1 < S->layers;
-        S->woff[l] = off;
-        off += (int64_t)S->width[l + 1] * S->width[l] + (S->bias[l] ? S->width[l + 1] : 0);
-    }
     for (int l = 0; l <= S->layers; ++l) {
+        S->width[l] = nn_width(f, l);
         S->aoff[l] = aoff;
         aoff += S->width[l] * TPS;
         if (S->width[l] > S->maxw) S->maxw = S->width[l];
     }
+    for (int l = 0; l < S->layers; ++l) {
+        S->act[l] = nn_act(f, l);
+        S->bias[l] = nn_bias(f, l);
+        S->woff[l] = off;
+        off += nn_layer_size(S->width[l], S->width[l + 1], S->bias[l]);
+    }
     S->aoff[S->layers + 1] = aoff;
     S->nparams = off;
-    S->scale = f.kind == SLB_FN_MLP ? f.cparams[17] : 1.0;
+    S->scale = f.kind == SLB_FN_MLP ? nn_scale(f) : 1.0;
 }
 
 size_t network_smem(const net_shape& S) {

@@ -998,6 +998,41 @@ class _TrainableNetwork(DeterministicFunction):
     ``torch(points)`` as one autograd node whose backward is one ``slb_function_vjp`` call for the
     points and every parameter."""
 
+    # activation codes of the fused kernels (csrc/common.cuh)
+    _ACT = {"tanh": 0, "relu": 1, "linear": 2, "identity": 2}
+
+    @classmethod
+    def _activation_names(cls, activations, what):
+        """The kernel's names of ``activations`` (names or functions such as ``numpy.tanh``)."""
+        names = []
+        for act in activations:
+            key = act if isinstance(act, str) else getattr(act, "__name__", "")
+            if key not in cls._ACT:
+                raise NotImplementedError("%s %r is not fused (tanh/relu/linear)" % (what, act))
+            names.append(key)
+        return names
+
+    @staticmethod
+    def _xavier(rng, rows, cols):
+        """A Xavier-uniform ``[rows, cols]`` draw from ``rng`` (``tf.contrib.layers.xavier_initializer``)."""
+        lim = np.sqrt(6.0 / (rows + cols))
+        return rng.uniform(-lim, lim, size=(rows, cols))
+
+    def _network_descriptor(self, kind, widths, activations, output_scale=1.0, use_bias=False):
+        """The descriptor of a fused network (layout in csrc/common.cuh): layer i has output width
+        ``widths[i]`` and activation ``activations[i]``; ``output_scale`` and ``use_bias`` are read for
+        ``FN_MLP`` only."""
+        d = nat.SlbFunction()
+        d.kind, d.in_dim, d.out_dim = kind, self.input_dim, self.output_dim
+        d.cparams[0] = len(widths)
+        for i, (od, act) in enumerate(zip(widths, activations)):
+            d.cparams[1 + i] = od
+            d.cparams[9 + i] = self._ACT[act]
+        d.cparams[17] = output_scale
+        d.cparams[18] = 1.0 if use_bias else 0.0
+        d.matrix = self._packed_device().data_ptr()
+        return d
+
     def _init_params(self):
         self._params = []
         self._names = []
@@ -1086,8 +1121,6 @@ class LyapunovNetwork(_TrainableNetwork):
     layer kernels are formed from them on the host once per parameter version.
     """
 
-    _ACT = {"tanh": 0, "relu": 1, "linear": 2, "identity": 2}
-
     def __init__(self, input_dim, layer_dims, activations, eps=1e-6, initializer=None,
                  name="lyapunov_network", weights=None, seed=0):
         super().__init__(name)
@@ -1101,12 +1134,7 @@ class LyapunovNetwork(_TrainableNetwork):
             raise ValueError("Each layer must maintain or increase the dimension of its input!")
         if max(self.output_dims) > 64 or self.num_layers > 8:
             raise DimensionError("LyapunovNetwork: at most 8 layers of width <= 64 are fused")
-        self.activations = []
-        for act in activations:
-            key = act if isinstance(act, str) else getattr(act, "__name__", "")
-            if key not in self._ACT:
-                raise NotImplementedError("activation %r is not fused (tanh/relu/linear)" % (act,))
-            self.activations.append(key)
+        self.activations = self._activation_names(activations, "activation")
         self.hidden_dims = [int(np.ceil(((self.input_dim if i == 0 else self.output_dims[i - 1])
                                          + 1) / 2)) for i in range(self.num_layers)]
         if weights is None:
@@ -1114,12 +1142,9 @@ class LyapunovNetwork(_TrainableNetwork):
             weights = []
             for i in range(self.num_layers):
                 din = self.input_dim if i == 0 else self.output_dims[i - 1]
-                def xavier(rows, cols):
-                    lim = np.sqrt(6.0 / (rows + cols))
-                    return rng.uniform(-lim, lim, size=(rows, cols))
                 extra = self.output_dims[i] - din
-                weights.append((xavier(self.hidden_dims[i], din),
-                                xavier(extra, din) if extra > 0 else None))
+                weights.append((self._xavier(rng, self.hidden_dims[i], din),
+                                self._xavier(rng, extra, din) if extra > 0 else None))
         self._init_params()
         self.weights = weights
 
@@ -1175,14 +1200,7 @@ class LyapunovNetwork(_TrainableNetwork):
         return dev.to_device(np.concatenate([k.ravel() for k in self.kernels()]))
 
     def descriptor(self):
-        d = nat.SlbFunction()
-        d.kind, d.in_dim, d.out_dim = nat.FN_LYAPUNOV_NN, self.input_dim, 1
-        d.cparams[0] = self.num_layers
-        for i, (od, act) in enumerate(zip(self.output_dims, self.activations)):
-            d.cparams[1 + i] = od
-            d.cparams[9 + i] = self._ACT[act]
-        d.matrix = self._packed_device().data_ptr()
-        return d
+        return self._network_descriptor(nat.FN_LYAPUNOV_NN, self.output_dims, self.activations)
 
     def _unpack_grads(self, gflat):
         """dL/dK_i -> the leaves: dW_posdef = W (G + G^T) over the top in_i rows, dW_extra = G below."""
@@ -1226,13 +1244,8 @@ class NeuralNetwork(_TrainableNetwork):
                  name="neural_network", weights=None, biases=None, seed=0):
         super().__init__(name)
         self.layers = [int(v) for v in layers]
-        self.nonlinearities = []
-        for act in nonlinearities:
-            key = "linear" if act is None else (act if isinstance(act, str)
-                                                else getattr(act, "__name__", ""))
-            if key not in LyapunovNetwork._ACT:
-                raise NotImplementedError("nonlinearity %r is not fused (tanh/relu/None)" % (act,))
-            self.nonlinearities.append(key)
+        self.nonlinearities = self._activation_names(
+            ["linear" if act is None else act for act in nonlinearities], "nonlinearity")
         if len(self.nonlinearities) == len(self.layers):
             widths = list(self.layers)                       # reference convention: input inferred
         elif len(self.nonlinearities) == len(self.layers) - 1:
@@ -1268,10 +1281,7 @@ class NeuralNetwork(_TrainableNetwork):
         dims = [self.input_dim] + self._widths
         rng = np.random.default_rng(self._seed)
         if weights is None:
-            weights = []
-            for din, dout in zip(dims[:-1], dims[1:]):
-                lim = np.sqrt(6.0 / (din + dout))
-                weights.append(rng.uniform(-lim, lim, size=(din, dout)))
+            weights = [self._xavier(rng, din, dout) for din, dout in zip(dims[:-1], dims[1:])]
         if biases is None:
             biases = [np.zeros(d) for d in dims[1:-1]]
         self._dims = dims
@@ -1376,16 +1386,8 @@ class NeuralNetwork(_TrainableNetwork):
             raise DimensionError("NeuralNetwork(%s): the input width is set by the first evaluation;"
                                  " call build(input_dim) or evaluate it once before fusing it"
                                  % self.layers)
-        d = nat.SlbFunction()
-        d.kind, d.in_dim, d.out_dim = nat.FN_MLP, self.input_dim, self.output_dim
-        d.cparams[0] = len(self._widths)
-        for i, (od, act) in enumerate(zip(self._widths, self.nonlinearities)):
-            d.cparams[1 + i] = od
-            d.cparams[9 + i] = LyapunovNetwork._ACT[act]
-        d.cparams[17] = self.output_scale
-        d.cparams[18] = 1.0 if self.use_bias else 0.0
-        d.matrix = self._packed_device().data_ptr()
-        return d
+        return self._network_descriptor(nat.FN_MLP, self._widths, self.nonlinearities, self.output_scale,
+                                        self.use_bias)
 
     def evaluate_device(self, points):
         pts = dev.to_device(points)
