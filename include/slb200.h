@@ -410,6 +410,17 @@ int slb_filter_stage1(const slb_sweep* cfg);
 int slb_lyapunov_sweep_filtered(void* stream, const slb_sweep* cfg, int64_t idx_begin,
                                 int64_t idx_end, uint8_t* negative_dev, double* values_dev,
                                 void* workspace_dev, int64_t* stats_dev);
+/* diagnostics: the refine pass of slb_lyapunov_sweep_filtered alone, on a caller's point list:
+ * list_dev [*count_dev] (device) holds indices relative to idx_begin, each in [0, n_max), and
+ * 0 <= n_max <= the pass length of slb_filter_workspace.  Both tile-size launches, the row / factor
+ * split and its workspace run exactly as in the filtered sweep (the split tickets are zeroed first).
+ * At the listed points it writes negative and values (NULL: not written) as slb_lyapunov_sweep would,
+ * and, unless NULL, mean_dev / err_dev [n_max, D] (err = beta sigma); every other entry is untouched.
+ * workspace_dev: >= slb_filter_workspace(n_max) bytes. */
+int slb_debug_refine(void* stream, const slb_sweep* cfg, int64_t idx_begin, int64_t n_max,
+                     const int64_t* list_dev, const unsigned long long* count_dev,
+                     uint8_t* negative_dev, double* values_dev, double* mean_dev, double* err_dev,
+                     void* workspace_dev);
 /* same on an explicit state list states_dev [n, d] (get_safe_sample-style callers) */
 int slb_lyapunov_points(void* stream, const slb_sweep* cfg, const double* states_dev, int64_t n,
                         uint8_t* negative_dev, double* values_dev, double* decrease_dev,

@@ -148,6 +148,8 @@ SIGNATURES = {
     "slb_filter_workspace": (C.c_int64, [_i64]),
     "slb_lyapunov_sweep_filtered": (C.c_int, [_vp, C.POINTER(SlbSweep), _i64, _i64, _dp, _dp, _vp,
                                               _vp]),
+    "slb_debug_refine": (C.c_int, [_vp, C.POINTER(SlbSweep), _i64, _i64, _vp, _vp, _vp, _dp, _dp, _dp,
+                                   _vp]),
     "slb_first_fail_workspace": (C.c_int64, [_i64]),
     "slb_first_fail_x": (C.c_int, [_vp, _dp, _dp, _dp, _i64, _i64, _vp, _vp,
                                    C.POINTER(SlbExchange)]),

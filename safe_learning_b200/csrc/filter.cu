@@ -865,7 +865,7 @@ int launch_filter(cudaStream_t st, const slb_sweep& cfg, const filter_args& a, s
 // gp_sweep.cu: the full posterior on the compacted list (count read on the device)
 int slb_launch_refine(cudaStream_t st, const slb_sweep& cfg, int64_t n_max, int64_t idx_begin,
                       const int64_t* list, const unsigned long long* count, uint8_t* negative,
-                      double* values, double* split_partial, int* split_ticket);
+                      double* values, double* mean, double* err, double* split_partial, int* split_ticket);
 
 extern "C" {
 
@@ -958,10 +958,32 @@ int slb_lyapunov_sweep_filtered(void* stream, const slb_sweep* cfg, int64_t idx_
         if (!(g_filter_stages & 2)) continue;
         rc = slb_launch_refine(st, *cfg, n, idx_begin + off, a.list_b, a.counts + 1,
                                negative_dev + off, values_dev ? values_dev + off : nullptr,
-                               partial, tickets);
+                               nullptr, nullptr, partial, tickets);
         if (rc) return rc;
     }
     return 0;
+}
+
+int slb_debug_refine(void* stream, const slb_sweep* cfg, int64_t idx_begin, int64_t n_max,
+                     const int64_t* list_dev, const unsigned long long* count_dev,
+                     uint8_t* negative_dev, double* values_dev, double* mean_dev, double* err_dev,
+                     void* workspace_dev) {
+    SLB_CHECK(cfg != nullptr, "slb_debug_refine: null config");
+    SLB_CHECK(cfg->gp.num_outputs > 0, "slb_debug_refine needs GP dynamics (the refine pass is the GP posterior)");
+    SLB_CHECK(n_max >= 0 && n_max <= CHUNK, "slb_debug_refine: n_max %lld outside [0, %lld]", (long long)n_max,
+              (long long)CHUNK);
+    SLB_CHECK(list_dev != nullptr && count_dev != nullptr && negative_dev != nullptr && workspace_dev != nullptr,
+              "slb_debug_refine: null list, count, negative or workspace");
+    int m;
+    if (slb_validate_sweep(cfg, false, &m)) return 1;
+    if (slb_validate_range("slb_debug_refine", idx_begin, idx_begin + n_max, cfg->grid.nindex)) return 1;
+    // the same workspace layout, and the same zeroed tickets, as one pass of the filtered sweep
+    cudaStream_t st = (cudaStream_t)stream;
+    char* ws = static_cast<char*>(workspace_dev);
+    SLB_CUDA(cudaMemsetAsync(ws + 64, 0, SLB_SPLIT_TICKET_BYTES, st));
+    return slb_launch_refine(st, *cfg, n_max, idx_begin, list_dev, count_dev, negative_dev, values_dev, mean_dev,
+                             err_dev, reinterpret_cast<double*>(ws + 64 + SLB_SPLIT_TICKET_BYTES),
+                             reinterpret_cast<int*>(ws + 64));
 }
 
 }  // extern "C"
