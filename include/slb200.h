@@ -314,6 +314,12 @@ void        slb_note_graph_replay(int64_t kernels);
  * %globaltimer (ns) at tile start / end, cycles spent waiting at block barriers, 0;
  * pass NULL to switch it off (default) */
 int         slb_debug_phase_timing(void* buffer_dev);
+/* diagnostics: when buffer_dev != NULL (uint64 [133][8], zeroed by the caller), every later filtered
+ * sweep raises entry [c][m] to the %globaltimer (ns) at which the last warp of head-stage CTA c passed
+ * mark m = {entry, head tables landed, bound of factor 0, bound of every factor, screened decision,
+ * fp64 means of the round, final decision, exit}, and [132][0] to the time the last warp of the first
+ * stage left (tools/head_stage_timeline.py); pass NULL to switch it off (default) */
+int         slb_debug_head_timing(void* buffer_dev);
 /* Records an event (owned by the library, one per device) on `stream` that every later launch reading
  * the packed factors (slb_gp_factor.Wpack: the full posterior of slb_gp_predict / slb_lyapunov_sweep /
  * slb_lyapunov_points and the refine pass of slb_lyapunov_sweep_filtered) waits for on ITS stream.  A
@@ -331,7 +337,9 @@ int         slb_restore_tables(void* dst_dev, const void* src_host, int64_t spli
                                void* stream, void* side_stream);
 /* diagnostics (timing of the individual stages of slb_lyapunov_sweep_filtered; the flags are only
  * complete with bits 0 and 1 set -- 3, the default, or 7): bit 0 runs the head stage, bit 1 the
- * refine pass; bit 2 forces the fp64 mean stage where the fp32 screening stage would run */
+ * refine pass; bit 2 forces the fp64 mean stage where the fp32 screening stage would run; bit 3
+ * forces the head stage's split schedule (a warp per group and factor, means on the spare warps),
+ * bit 4 its round loop (a warp per group), which it otherwise chooses from the list length */
 int         slb_debug_filter_stages(int32_t mask);
 /* diagnostics: while both pointers are non-NULL, the fp32 screening stage of
  * slb_lyapunov_sweep_filtered also writes, for every point of the swept range (row = index relative to

@@ -74,7 +74,20 @@ struct filter_args {
     int prefetch_factors;              // head stage: warm L2 with the packed factors for the refine pass
     double* probe_mu;                  // slb_debug_screening_probe: nullptr or [n, D] screened means ...
     double* probe_dm;                  // ... and their certified error bounds (inf: point left to fp64)
+    unsigned long long* timing;        // slb_debug_head_timing: nullptr or [HEAD_CTAS + 1][8] %globaltimer
+    int head_schedule;                 // head stage: 0 chosen from the list length, 1 split, 2 round loop
 };
+
+// slb_debug_head_timing: timing[slot] = the latest %globaltimer (ns) at which a warp passed a mark.
+// Head CTA c writes row c at the marks below, stage 1 writes row HEAD_CTAS, slot 0 when it leaves.
+enum { HM_ENTRY, HM_TABLES, HM_BOUND0, HM_BOUND, HM_SCREENED, HM_MEANS, HM_DECIDED, HM_EXIT };
+SLB_DEV void timing_mark(const filter_args& a, int slot) {
+    if (a.timing == nullptr || (threadIdx.x & 31) != 0) return;
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    atomicMax(a.timing + slot, t);
+}
+SLB_DEV void head_mark(const filter_args& a, int mark) { timing_mark(a, blockIdx.x * 8 + mark); }
 
 // outcome for err_j = beta_j sigma_j with sigma_j in [0, shi_j]:  +1 decided negative (True),
 // 0 decided not negative (False), -1 undecided.  term_j = L_V(mu)_j beta_j sigma_j lies between 0 and
@@ -251,6 +264,7 @@ filter_mean_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
         count_stat(valid && !undecided, a.stats + 0);
         count_stat(valid, a.stats + 3);
     }
+    timing_mark(a, HEAD_CTAS * 8);
 }
 
 // ---- stage 1, fp32 screening variant ---------------------------------------------------------------
@@ -355,6 +369,7 @@ filter_mean32_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a)
         count_stat(valid && !undecided, a.stats + 0);
         count_stat(valid, a.stats + 3);
     }
+    timing_mark(a, HEAD_CTAS * 8);
 }
 
 // ---- stage 2: variance given the head subset, one warp per HP undecided points ---------------------
@@ -419,19 +434,21 @@ SLB_DEV void head_mean_factor(const double* __restrict__ xf, int Mp, const doubl
 // decide from their screened means (`slots`: s = 8 w + p is entry p of warp w's group), by ALL warps of the
 // CTA -- L = 512 / (number of entries) lanes per point, so a CTA with few of them (short lists: the stage's
 // duration is the latency of one group) still spreads the M exps per point and factor over its threads.
-// Results: mu_s / merr_s [slot][SLB_MAX_OUT] in shared memory.
+// Results: mu_s / merr_s [slot][SLB_MAX_OUT] in shared memory.  The threads [tid0, tid0 + nthreads) of
+// the CTA (whole warps) take part; `slots` nullptr: the entries are slots 0 .. nneed - 1.
 template <int DIN>
 SLB_DEV void head_round_means(const slb_sweep& cfg, const filter_args& a, const int* slots, int nneed,
                               int64_t grp0, int64_t count, const double* mbuf, const double* tab512,
-                              double* mu_s, double* merr_s) {
+                              double* mu_s, double* merr_s, int tid0, int nthreads) {
     const int nf = cfg.gp.num_factors, D = cfg.gp.num_outputs;
-    const int L = nneed <= 16 ? 32 : nneed <= 32 ? 16 : nneed <= 64 ? 8 : 4;
+    int L = 32;                                // 512 threads: 32 lanes up to 16 entries, ..., 4 beyond 64
+    while (L > 4 && nneed * L > nthreads) L >>= 1;
     const int r = threadIdx.x & (L - 1);
     const int per_warp = 32 / L;
     const int nloop = (nneed + per_warp - 1) / per_warp * per_warp;   // whole warps take part in the shuffles
-    for (int i = threadIdx.x / L; i < nloop; i += HT / L) {
+    for (int i = ((int)threadIdx.x - tid0) / L; i < nloop; i += nthreads / L) {
         const bool live = i < nneed;
-        const int slot = live ? slots[i] : 0;
+        const int slot = live ? (slots != nullptr ? slots[i] : i) : 0;
         const int64_t k = (grp0 + (int64_t)(slot / HP) * gridDim.x) * HP + (slot % HP);
         double z[DIN];
 #pragma unroll
@@ -472,15 +489,13 @@ SLB_DEV void head_round_means(const slb_sweep& cfg, const filter_args& a, const 
     }
 }
 
-// one group of P list entries [g P, g P + P) on one warp
-template <int DIN, int P, bool ALL_STAGED>
-SLB_DEV void head_group_bound(const slb_sweep& cfg, const filter_args& a, int64_t grp, int64_t count,
-                              const double* exptab, double* kw, const double* wbuf, const double* xbuf,
-                              filter_side& t, int64_t& rel, bool& mine, double* shi) {
+// lane p < P owns list entry grp * P + p: its terms, its index, the prior bound of every output's sigma and
+// finally its decision
+template <int DIN, int P>
+SLB_DEV void head_group_entries(const slb_sweep& cfg, const filter_args& a, int64_t grp, int64_t count,
+                                filter_side& t, int64_t& rel, bool& mine, double* shi) {
     const int lane = threadIdx.x & 31;
-    const int nf = cfg.gp.num_factors;
     const int D = cfg.gp.num_outputs;
-    // lane p < P owns list entry grp * P + p: its terms, its index and finally its decision
     const int64_t k = grp * P + min(lane, P - 1);
     mine = lane < P && k < count;
     t = filter_side{};
@@ -491,121 +506,150 @@ SLB_DEV void head_group_bound(const slb_sweep& cfg, const filter_args& a, int64_
         shi[j] = mine ? sqrt(F.kernel.num_prims > 0 ? kernel_expr_diag<DIN>(F.kernel, t.z) : F.variance)
                       : 0.0;
     }
-    for (int f = 0; f < nf; ++f) {
-        const slb_gp_factor& F = cfg.gp.factors[f];
-        const int rows = F.head_rows;
-        if (rows <= 0) continue;
-        const bool general = F.kernel.num_prims > 0;
-        const double s2 = f64mul(F.scale, F.scale);
-        // ALL_STAGED: the tables are known to be in shared memory (LDS instead of generic loads)
-        const bool staged = ALL_STAGED || f < a.head_factors_staged;
-        const double* xh = xbuf + (size_t)f * HR * DIN;
-        if (!ALL_STAGED && !staged) xh = F.Xhead;
-        // kernel values of every point of the group against subset points lane and lane + 32
-        // (functions.py:438); entries beyond the list carry zeros (never decided)
-        double zown[DIN];                       // this lane's point in the factor's units (one division
-#pragma unroll                                  // per lane and dimension instead of one per point)
-        for (int c = 0; c < DIN; ++c) zown[c] = general ? t.z[c] : t.z[c] / F.lengthscales[c];
+}
+
+// sigma of factor f (head_rows > 0) given its head subset, for the P entries of a group on one warp
+// (lane p: entry p's; the other lanes' values are meaningless)
+template <int DIN, int P, bool ALL_STAGED>
+SLB_DEV double head_factor_sdev(const slb_sweep& cfg, const filter_args& a, int f, const filter_side& t,
+                                bool mine, const double* exptab, double* kw, const double* wbuf,
+                                const double* xbuf, uint64_t* bar) {
+    const int lane = threadIdx.x & 31;
+    const slb_gp_factor& F = cfg.gp.factors[f];
+    const int rows = F.head_rows;
+    const bool general = F.kernel.num_prims > 0;
+    const double s2 = f64mul(F.scale, F.scale);
+    // ALL_STAGED: the tables are known to be in shared memory (LDS instead of generic loads)
+    const bool staged = ALL_STAGED || f < a.head_factors_staged;
+    const double* xh = xbuf + (size_t)f * HR * DIN;
+    if (!ALL_STAGED && !staged) xh = F.Xhead;
+    // kernel values of every point of the group against subset points lane and lane + 32
+    // (functions.py:438); entries beyond the list carry zeros (never decided)
+    double zown[DIN];                       // this lane's point in the factor's units (one division
+#pragma unroll                              // per lane and dimension instead of one per point)
+    for (int c = 0; c < DIN; ++c) zown[c] = general ? t.z[c] : t.z[c] / F.lengthscales[c];
 #pragma unroll
-        for (int p = 0; p < P; ++p) {
-            double zs[DIN];
+    for (int p = 0; p < P; ++p) {
+        double zs[DIN];
 #pragma unroll
-            for (int c = 0; c < DIN; ++c) zs[c] = __shfl_sync(0xffffffffu, zown[c], p);
+        for (int c = 0; c < DIN; ++c) zs[c] = __shfl_sync(0xffffffffu, zown[c], p);
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int j = lane + 32 * h;
-                double kv = 0.0;
-                if (j < rows) {
-                    const double* xr = xh + j * DIN;
-                    if (general) {
-                        kv = kernel_expr_cross<DIN>(F.kernel, zs, xr, exptab);
-                    } else {
-                        double a2 = 0.0;
+        for (int h = 0; h < 2; ++h) {
+            const int j = lane + 32 * h;
+            double kv = 0.0;
+            if (j < rows) {
+                const double* xr = xh + j * DIN;
+                if (general) {
+                    kv = kernel_expr_cross<DIN>(F.kernel, zs, xr, exptab);
+                } else {
+                    double a2 = 0.0;
 #pragma unroll
-                        for (int c = 0; c < DIN; ++c) { const double df = zs[c] - xr[c]; a2 = fma(df, df, a2); }
-                        kv = F.variance * exp_neg_tab(-0.5 * a2, exptab);
-                    }
-                    kv = s2 * kv;
+                    for (int c = 0; c < DIN; ++c) { const double df = zs[c] - xr[c]; a2 = fma(df, df, a2); }
+                    kv = F.variance * exp_neg_tab(-0.5 * a2, exptab);
                 }
-                kw[j * P + p] = kv;
+                kv = s2 * kv;
             }
+            kw[j * P + p] = kv;
         }
-        __syncwarp();
-        double ssp = 0.0;                       // lane p: sum_i a_i^2 of point p
-        if constexpr (P == HP) {
-            // a = W k on the fp64 tensor pipe: W (64 x 64, lower triangular) pre-packed in DMMA
-            // A-fragment order (row block b, k-step s: slb_gp_factor.Wheadp), the HP = 8 points are
-            // the n dimension, k values [row][point] in shared memory are the B fragments as they
-            // lie.  Only the blocks on or below the diagonal (s <= 2 b + 1) are multiplied: 72 DMMAs.
-            const double* __restrict__ Wp = wbuf + (size_t)f * HR * HR;
-            if (!ALL_STAGED && !staged) Wp = F.Wheadp;
-            double acc[8][2];
-#pragma unroll
-            for (int b = 0; b < 8; ++b) { acc[b][0] = 0.0; acc[b][1] = 0.0; }
-#pragma unroll
-            for (int sk = 0; sk < 16; ++sk) {
-                const double bf = kw[(4 * sk + (lane & 3)) * HP + (lane >> 2)];
-#pragma unroll
-                for (int b = sk / 2; b < 8; ++b) {
-                    const double af = Wp[(b * 16 + sk) * 32 + lane];
-                    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
-                                 : "+d"(acc[b][0]), "+d"(acc[b][1]) : "d"(af), "d"(bf));
-                }
-            }
-            __syncwarp();
-            // lane T holds rows 8 b + T/4 of points 2 (T%4), 2 (T%4) + 1: square, sum over b, then over
-            // the 8 lanes that share T%4; lane p fetches point p's sum
-            double v0 = 0.0, v1 = 0.0;
-#pragma unroll
-            for (int b = 0; b < 8; ++b) { v0 = fma(acc[b][0], acc[b][0], v0); v1 = fma(acc[b][1], acc[b][1], v1); }
-#pragma unroll
-            for (int off = 4; off < 32; off <<= 1) {
-                v0 += __shfl_xor_sync(0xffffffffu, v0, off);
-                v1 += __shfl_xor_sync(0xffffffffu, v1, off);
-            }
-            const double s0 = __shfl_sync(0xffffffffu, v0, (lane >> 1) & 3);
-            const double s1 = __shfl_sync(0xffffffffu, v1, (lane >> 1) & 3);
-            ssp = (lane & 1) ? s1 : s0;
-        } else {
-        // short groups: two partial sums per row and point (even / odd columns) halve the dependent
-        // FMA chain; 8-point groups already carry 16 independent chains
-        constexpr int NS = P <= 2 ? 2 : 1;
-        double al[2][P], ah[2][P];
-#pragma unroll
-        for (int p = 0; p < P; ++p) { al[0][p] = al[1][p] = 0.0; ah[0][p] = ah[1][p] = 0.0; }
-        const double* Wt = F.Whead;            // column-major table (global / L2): reference path
-#pragma unroll 4
-        for (int j = 0; j < HR; ++j) {
-            const double wl = Wt[j * HR + lane], wh = Wt[j * HR + 32 + lane];
-            double kj[P];
-#pragma unroll
-            for (int p = 0; p < P; p += 2) {
-                const double2 v = *reinterpret_cast<const double2*>(kw + j * P + p);
-                kj[p] = v.x; kj[p + 1] = v.y;
-            }
-#pragma unroll
-            for (int p = 0; p < P; ++p) {
-                al[j & (NS - 1)][p] = fma(wl, kj[p], al[j & (NS - 1)][p]);
-                ah[j & (NS - 1)][p] = fma(wh, kj[p], ah[j & (NS - 1)][p]);
-            }
-        }
-        __syncwarp();
-        // sum a^2 per point over the 64 rows: lane p ends up with point p's
-#pragma unroll
-        for (int p = 0; p < P; ++p) {
-            const double lo = al[0][p] + al[1][p], hi = ah[0][p] + ah[1][p];
-            double ss = fma(lo, lo, hi * hi);
-#pragma unroll
-            for (int off = 16; off > 0; off >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, off);
-            if (lane == p) ssp = ss;
-        }
-        }
-        double kss = F.kss;
-        if (general && mine) kss = s2 * kernel_expr_diag<DIN>(F.kernel, t.z);
-        const double sdev = sqrt(f64sub(kss, ssp) / s2);          // NaN if negative
-        for (int j = 0; j < D; ++j)
-            if (cfg.gp.outputs[j].factor == f) shi[j] = sdev;
     }
+    __syncwarp();
+    double ssp = 0.0;                       // lane p: sum_i a_i^2 of point p
+    if constexpr (P == HP) {
+        // a = W k on the fp64 tensor pipe: W (64 x 64, lower triangular) pre-packed in DMMA
+        // A-fragment order (row block b, k-step s: slb_gp_factor.Wheadp), the HP = 8 points are
+        // the n dimension, k values [row][point] in shared memory are the B fragments as they
+        // lie.  Only the blocks on or below the diagonal (s <= 2 b + 1) are multiplied: 72 DMMAs.
+        const double* __restrict__ Wp = wbuf + (size_t)f * HR * HR;
+        if (!ALL_STAGED && !staged) Wp = F.Wheadp;
+        else slb_bulk::mbar_wait(bar + 1, 0);       // the packed factors have landed
+        double acc[8][2];
+#pragma unroll
+        for (int b = 0; b < 8; ++b) { acc[b][0] = 0.0; acc[b][1] = 0.0; }
+#pragma unroll
+        for (int sk = 0; sk < 16; ++sk) {
+            const double bf = kw[(4 * sk + (lane & 3)) * HP + (lane >> 2)];
+#pragma unroll
+            for (int b = sk / 2; b < 8; ++b) {
+                const double af = Wp[(b * 16 + sk) * 32 + lane];
+                asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
+                             : "+d"(acc[b][0]), "+d"(acc[b][1]) : "d"(af), "d"(bf));
+            }
+        }
+        __syncwarp();
+        // lane T holds rows 8 b + T/4 of points 2 (T%4), 2 (T%4) + 1: square, sum over b, then over
+        // the 8 lanes that share T%4; lane p fetches point p's sum
+        double v0 = 0.0, v1 = 0.0;
+#pragma unroll
+        for (int b = 0; b < 8; ++b) { v0 = fma(acc[b][0], acc[b][0], v0); v1 = fma(acc[b][1], acc[b][1], v1); }
+#pragma unroll
+        for (int off = 4; off < 32; off <<= 1) {
+            v0 += __shfl_xor_sync(0xffffffffu, v0, off);
+            v1 += __shfl_xor_sync(0xffffffffu, v1, off);
+        }
+        const double s0 = __shfl_sync(0xffffffffu, v0, (lane >> 1) & 3);
+        const double s1 = __shfl_sync(0xffffffffu, v1, (lane >> 1) & 3);
+        ssp = (lane & 1) ? s1 : s0;
+    } else {
+    // short groups: two partial sums per row and point (even / odd columns) halve the dependent
+    // FMA chain; 8-point groups already carry 16 independent chains
+    constexpr int NS = P <= 2 ? 2 : 1;
+    double al[2][P], ah[2][P];
+#pragma unroll
+    for (int p = 0; p < P; ++p) { al[0][p] = al[1][p] = 0.0; ah[0][p] = ah[1][p] = 0.0; }
+    const double* Wt = F.Whead;            // column-major table (global / L2): reference path
+#pragma unroll 4
+    for (int j = 0; j < HR; ++j) {
+        const double wl = Wt[j * HR + lane], wh = Wt[j * HR + 32 + lane];
+        double kj[P];
+#pragma unroll
+        for (int p = 0; p < P; p += 2) {
+            const double2 v = *reinterpret_cast<const double2*>(kw + j * P + p);
+            kj[p] = v.x; kj[p + 1] = v.y;
+        }
+#pragma unroll
+        for (int p = 0; p < P; ++p) {
+            al[j & (NS - 1)][p] = fma(wl, kj[p], al[j & (NS - 1)][p]);
+            ah[j & (NS - 1)][p] = fma(wh, kj[p], ah[j & (NS - 1)][p]);
+        }
+    }
+    __syncwarp();
+    // sum a^2 per point over the 64 rows: lane p ends up with point p's
+#pragma unroll
+    for (int p = 0; p < P; ++p) {
+        const double lo = al[0][p] + al[1][p], hi = ah[0][p] + ah[1][p];
+        double ss = fma(lo, lo, hi * hi);
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, off);
+        if (lane == p) ssp = ss;
+    }
+    }
+    double kss = F.kss;
+    if (general && mine) kss = s2 * kernel_expr_diag<DIN>(F.kernel, t.z);
+    const double sdev = sqrt(f64sub(kss, ssp) / s2);          // NaN if negative
+    return sdev;
+}
+
+// one group of P list entries [g P, g P + P) on one warp, factor after factor
+template <int DIN, int P, bool ALL_STAGED>
+SLB_DEV void head_group_bound(const slb_sweep& cfg, const filter_args& a, int64_t grp, int64_t count,
+                              const double* exptab, double* kw, const double* wbuf, const double* xbuf,
+                              uint64_t* bar, filter_side& t, int64_t& rel, bool& mine, double* shi) {
+    head_group_entries<DIN, P>(cfg, a, grp, count, t, rel, mine, shi);
+    slb_bulk::mbar_wait(bar + 0, 0);            // exp tables and subset inputs have landed
+    head_mark(a, HM_TABLES);
+    for (int f = 0; f < cfg.gp.num_factors; ++f) {
+        if (cfg.gp.factors[f].head_rows <= 0) continue;
+        const double sdev = head_factor_sdev<DIN, P, ALL_STAGED>(cfg, a, f, t, mine, exptab, kw, wbuf, xbuf, bar);
+        for (int j = 0; j < cfg.gp.num_outputs; ++j)
+            if (cfg.gp.outputs[j].factor == f) shi[j] = sdev;
+        if (f == 0) head_mark(a, HM_BOUND0);
+    }
+    head_mark(a, HM_BOUND);
+}
+
+// every copy lands in this CTA's shared memory before the CTA may leave
+SLB_DEV void head_wait_landings(uint64_t* bar) {
+    for (int b = 0; b < 3; ++b) slb_bulk::mbar_wait(bar + b, 0);
 }
 
 // a lane's final outcome: the flag of a decided point, list B for an undecided one (warp-collective)
@@ -627,20 +671,61 @@ template <int DIN>
 __global__ void __launch_bounds__(HT, 1)
 filter_head_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
+    if (threadIdx.x == 0) head_mark(a, HM_ENTRY);
     prefetch_descriptor_operands(cfg);
-    uint64_t* bar = reinterpret_cast<uint64_t*>(smem_raw);             // [1]
-    unsigned* s_stat = reinterpret_cast<unsigned*>(smem_raw + 8);      // decided / undecided by this CTA
-    double* tab512 = reinterpret_cast<double*>(smem_raw + 16);         // [512] (screened lists: exp_neg_fast)
+    // three landings, each waited for just before its first use: (a) the exp tables and the subsets'
+    // inputs (kernel values), (b) the packed head factors (DMMA), (c) screened lists: [Xf | gamma_f]
+    uint64_t* bar = reinterpret_cast<uint64_t*>(smem_raw);             // [3]
+    unsigned* s_stat = reinterpret_cast<unsigned*>(smem_raw + 24);     // decided / undecided by this CTA
+    double* tab512 = reinterpret_cast<double*>(smem_raw + 32);         // [512] (screened lists: exp_neg_fast)
     double* exptab = tab512 + 512;                                     // [64]
     double* kbuf = exptab + 64;                                        // [HW][HR][HP]
-    double* wbuf = kbuf + HW * HR * HP;                                // [staged][HR * HR]
+    double* sd_s = kbuf + HW * HR * HP;                                // split schedule: [HW * HP][SLB_MAX_OUT]
+    double* wbuf = sd_s + HW * HP * SLB_MAX_OUT;                       // [staged][HR * HR]
     const int nf = cfg.gp.num_factors;
     double* xbuf = wbuf + (size_t)a.head_factors_staged * HR * HR;     // [staged][HR * DIN]
     double* mbuf = xbuf + (size_t)a.head_factors_staged * HR * DIN;    // screened: [Xf | gamma_f ...] per factor
-    // ---- everything that does not depend on stage 1's lists first.  The refine pass that follows
-    // streams every factor's packed L^-1 (1 MB at M = 500); if it is not L2-resident by then (first
-    // sweep after a cache update, or evicted in between) its CTAs start with HBM round trips in
-    // lockstep: prefetch it.
+    if (threadIdx.x == 0) {
+        for (int b = 0; b < 3; ++b) slb_bulk::mbar_init(bar + b, 1);
+        slb_bulk::fence_barrier_init();
+        slb_bulk::fence_proxy_async();
+        unsigned xbytes = 576 * sizeof(double), wbytes = 0;
+        for (int f = 0; f < a.head_factors_staged; ++f)
+            if (cfg.gp.factors[f].head_rows > 0) {
+                xbytes += (unsigned)(HR * DIN) * sizeof(double);
+                wbytes += (unsigned)(HR * HR) * sizeof(double);
+            }
+        slb_bulk::mbar_arrive_expect_tx(bar + 0, xbytes);
+        slb_bulk::copy_g2s(tab512, g_exp_tables, 576 * sizeof(double), bar + 0);
+        for (int f = 0; f < a.head_factors_staged; ++f)
+            if (cfg.gp.factors[f].head_rows > 0)
+                slb_bulk::copy_g2s(xbuf + (size_t)f * HR * DIN, cfg.gp.factors[f].Xhead,
+                                   HR * DIN * sizeof(double), bar + 0);
+        slb_bulk::mbar_arrive_expect_tx(bar + 1, wbytes);
+        for (int f = 0; f < a.head_factors_staged; ++f)
+            if (cfg.gp.factors[f].head_rows > 0)
+                slb_bulk::copy_g2s(wbuf + (size_t)f * HR * HR, cfg.gp.factors[f].Wheadp,
+                                   HR * HR * sizeof(double), bar + 1);
+        slb_bulk::mbar_arrive_expect_tx(bar + 2, a.screened ? (unsigned)a.mean_doubles * sizeof(double) : 0u);
+        if (a.screened) {
+            for (int f = 0; f < nf; ++f) {
+                const slb_gp_factor& F = cfg.gp.factors[f];
+                const int Mp = padded_rows(F.M);
+                if (Mp == 0) continue;
+                double* dst = mbuf + a.mean_off[f];
+                slb_bulk::copy_g2s(dst, F.Xf, (unsigned)(Mp * (DIN + 1)) * sizeof(double), bar + 2);
+                dst += (size_t)Mp * (DIN + 1);
+                for (int o = 0; o < cfg.gp.num_outputs; ++o) {
+                    if (cfg.gp.outputs[o].factor != f) continue;
+                    slb_bulk::copy_g2s(dst, cfg.gp.outputs[o].gamma_f, (unsigned)Mp * sizeof(double), bar + 2);
+                    dst += Mp;
+                }
+            }
+        }
+    }
+    // ---- behind the staging: the refine pass that follows streams every factor's packed L^-1 (1 MB at
+    // M = 500); if it is not L2-resident by then (first sweep after a cache update, or evicted in
+    // between) its CTAs start with HBM round trips in lockstep: prefetch it.
     if (a.prefetch_factors) {
         for (int f = 0; f < nf; ++f) {
             const slb_gp_factor& F = cfg.gp.factors[f];
@@ -663,119 +748,190 @@ filter_head_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
                 asm volatile("prefetch.global.L2 [%0];" ::"l"(reinterpret_cast<const char*>(G.alpha) + off));
         }
     }
-    if (threadIdx.x == 0) {
-        slb_bulk::mbar_init(bar, 1);
-        slb_bulk::fence_barrier_init();
-        slb_bulk::fence_proxy_async();
-        unsigned bytes = 576 * sizeof(double);
-        for (int f = 0; f < a.head_factors_staged; ++f)
-            if (cfg.gp.factors[f].head_rows > 0)
-                bytes += (unsigned)(HR * HR + HR * DIN) * sizeof(double);
-        if (a.screened) bytes += (unsigned)a.mean_doubles * sizeof(double);
-        slb_bulk::mbar_arrive_expect_tx(bar, bytes);
-        slb_bulk::copy_g2s(tab512, g_exp_tables, 576 * sizeof(double), bar);
-        for (int f = 0; f < a.head_factors_staged; ++f) {
-            const slb_gp_factor& F = cfg.gp.factors[f];
-            if (F.head_rows <= 0) continue;
-            slb_bulk::copy_g2s(wbuf + (size_t)f * HR * HR, F.Wheadp, HR * HR * sizeof(double), bar);
-            slb_bulk::copy_g2s(xbuf + (size_t)f * HR * DIN, F.Xhead, HR * DIN * sizeof(double), bar);
-        }
-        if (a.screened) {
-            for (int f = 0; f < nf; ++f) {
-                const slb_gp_factor& F = cfg.gp.factors[f];
-                const int Mp = padded_rows(F.M);
-                if (Mp == 0) continue;
-                double* dst = mbuf + a.mean_off[f];
-                slb_bulk::copy_g2s(dst, F.Xf, (unsigned)(Mp * (DIN + 1)) * sizeof(double), bar);
-                dst += (size_t)Mp * (DIN + 1);
-                for (int o = 0; o < cfg.gp.num_outputs; ++o) {
-                    if (cfg.gp.outputs[o].factor != f) continue;
-                    slb_bulk::copy_g2s(dst, cfg.gp.outputs[o].gamma_f, (unsigned)Mp * sizeof(double), bar);
-                    dst += Mp;
-                }
-            }
-        }
-    }
     if (threadIdx.x < 2) s_stat[threadIdx.x] = 0;
     if (a.screened && threadIdx.x < 2)
         reinterpret_cast<int*>(mbuf + a.mean_doubles + 2 * HW * HP * SLB_MAX_OUT)[threadIdx.x] = 0;
     __syncthreads();
-    slb_bulk::mbar_wait(bar, 0);                  // also before leaving: the copies land in this CTA's memory
     const int64_t count = (int64_t)a.counts[0];
     const int64_t nwarps = (int64_t)gridDim.x * HW;
     const int64_t ngroups = (count + HP - 1) / HP;
     // groups are dealt round-robin over the CTAs (group g: CTA g % gridDim, warp g / gridDim): a short
     // list spreads over all SMs instead of filling the 16 warps of the first few
-    if ((int64_t)blockIdx.x >= ngroups) return;                        // no group for this CTA
+    if ((int64_t)blockIdx.x >= ngroups) {                              // no group for this CTA
+        head_wait_landings(bar);
+        if (threadIdx.x == 0) head_mark(a, HM_EXIT);
+        return;
+    }
     const int warp = threadIdx.x >> 5;
     double* kw = kbuf + warp * HR * HP;
     double* mu_s = mbuf + a.mean_doubles;      // screened: [HW * HP][SLB_MAX_OUT] fp64 means, then their error bounds
     double* merr_s = mu_s + HW * HP * SLB_MAX_OUT;
     int* need_s = reinterpret_cast<int*>(merr_s + HW * HP * SLB_MAX_OUT);   // [2] counters (round parity), slots
-    // round: warp w takes group grp0 + w gridDim (every warp of the CTA makes the same number of rounds)
-    int round = 0;
-    for (int64_t grp0 = blockIdx.x; grp0 < ngroups; grp0 += nwarps, ++round) {
-        const int64_t grp = grp0 + (int64_t)warp * gridDim.x;
-        const bool active = grp < ngroups;
+    // Short lists (one round, and a warp to spare beside one warp per group and factor: C2) are latency
+    // bound: the split schedule gives every (group, factor) pair a warp of its own, and the spare warps
+    // compute the fp64 means of all the round's entries meanwhile (used only where the screened box
+    // leaves an entry open).  Longer lists keep the round loop below, factor after factor on one warp.
+    const int ng_first = (int)min((int64_t)HW, (ngroups - blockIdx.x + gridDim.x - 1) / gridDim.x);
+    const bool split = a.head_schedule == 1 ||
+                       (a.head_schedule == 0 && ngroups <= nwarps && ng_first * nf < HW);
+    if (split) {
         const int lane = threadIdx.x & 31;
-        filter_side t;
-        int64_t rel = 0;
-        bool mine = false, need = false;
-        double shi[SLB_MAX_OUT];
-        double vx = 0.0;
-        int outcome = 0;
-        if (active) {
-            if (a.head_factors_staged == nf)
-                head_group_bound<DIN, HP, true>(cfg, a, grp, count, exptab, kw, wbuf, xbuf, t, rel, mine, shi);
-            else
-                head_group_bound<DIN, HP, false>(cfg, a, grp, count, exptab, kw, wbuf, xbuf, t, rel, mine, shi);
-            if (a.screened) {
-                // first with the screened mean and its error box (stage 1 left them in the entry): most
-                // entries are decided by the tighter variance bound alone
-                double mu[SLB_MAX_OUT], dm[SLB_MAX_OUT], zero[SLB_MAX_OUT];
-                for (int j = 0; j < SLB_MAX_OUT; ++j) { mu[j] = t.coef[j]; dm[j] = t.dm[j]; zero[j] = 0.0; }
-                vx = t.dec0;
-                mean_decision_terms(cfg, t, vx, mu, zero);
-                t.guard += screening_slack(cfg, mu, dm, shi);
-                outcome = mine ? decide(t, shi, cfg.gp.num_outputs) : 0;
-                need = mine && outcome < 0;
-                if (need) need_s[2 + atomicAdd(need_s + (round & 1), 1)] = warp * HP + lane;
-            } else {
-                outcome = mine ? decide(t, shi, cfg.gp.num_outputs) : 0;
-            }
-        }
-        if (a.screened) {
-            if (threadIdx.x == 0) need_s[(round + 1) & 1] = 0;       // the next round's counter
-            __syncthreads();
-            const int nneed = need_s[round & 1];
-            if (nneed > 0) {
-                // the rest gets its mean in fp64 (all warps), then the same comparison as the fp64 path
-                head_round_means<DIN>(cfg, a, need_s + 2, nneed, grp0, count, mbuf, tab512, mu_s, merr_s);
-                __syncthreads();
-                if (need) {
-                    double mu[SLB_MAX_OUT], merr[SLB_MAX_OUT];
-                    const int slot = warp * HP + lane;
-                    for (int j = 0; j < SLB_MAX_OUT; ++j) {
-                        mu[j] = mu_s[slot * SLB_MAX_OUT + j];
-                        merr[j] = merr_s[slot * SLB_MAX_OUT + j];
+        for (int64_t grp0 = blockIdx.x; grp0 < ngroups; grp0 += nwarps) {
+            // this CTA's groups of the round: grp0 + i gridDim, i < ngr (group i's decisions on warp i)
+            const int ngr = (int)min((int64_t)HW, (ngroups - grp0 + gridDim.x - 1) / gridDim.x);
+            const int npairs = ngr * nf;
+            const int nbw = min(npairs, HW);
+            const bool early_means = a.screened && nbw < HW;
+            if (warp < nbw) {
+                slb_bulk::mbar_wait(bar + 0, 0);
+                head_mark(a, HM_TABLES);
+                for (int p = warp; p < npairs; p += nbw) {
+                    const int i = p / nf, f = p % nf;
+                    if (cfg.gp.factors[f].head_rows <= 0) continue;
+                    const int64_t k = (grp0 + (int64_t)i * gridDim.x) * HP + min(lane, HP - 1);
+                    const bool mine = lane < HP && k < count;
+                    filter_side tz = {};
+                    if (mine) {
+#pragma unroll
+                        for (int c = 0; c < DIN; ++c) tz.z[c] = a.side_a[k].z[c];
                     }
-                    mean_decision_terms(cfg, t, vx, mu, merr);
-                    outcome = decide(t, shi, cfg.gp.num_outputs);
+                    const double sd =
+                        a.head_factors_staged == nf
+                            ? head_factor_sdev<DIN, HP, true>(cfg, a, f, tz, mine, exptab, kw, wbuf, xbuf, bar)
+                            : head_factor_sdev<DIN, HP, false>(cfg, a, f, tz, mine, exptab, kw, wbuf, xbuf, bar);
+                    if (lane < HP) sd_s[(i * HP + lane) * SLB_MAX_OUT + f] = sd;
+                    if (f == 0) head_mark(a, HM_BOUND0);
+                }
+                head_mark(a, HM_BOUND);
+            } else if (early_means) {
+                slb_bulk::mbar_wait(bar + 0, 0);
+                slb_bulk::mbar_wait(bar + 2, 0);
+                head_round_means<DIN>(cfg, a, nullptr, ngr * HP, grp0, count, mbuf, tab512, mu_s, merr_s,
+                                      nbw * 32, HT - nbw * 32);
+                head_mark(a, HM_MEANS);
+            }
+            __syncthreads();
+            if (a.screened && !early_means) {             // no warp to spare: the means after the bounds
+                slb_bulk::mbar_wait(bar + 0, 0);
+                slb_bulk::mbar_wait(bar + 2, 0);
+                head_round_means<DIN>(cfg, a, nullptr, ngr * HP, grp0, count, mbuf, tab512, mu_s, merr_s, 0, HT);
+                head_mark(a, HM_MEANS);
+                __syncthreads();
+            }
+            if (warp < ngr) {
+                filter_side t;
+                int64_t rel;
+                bool mine;
+                double shi[SLB_MAX_OUT];
+                head_group_entries<DIN, HP>(cfg, a, grp0 + (int64_t)warp * gridDim.x, count, t, rel, mine, shi);
+                const int slot = warp * HP + min(lane, HP - 1);
+                for (int j = 0; j < cfg.gp.num_outputs; ++j) {
+                    const int f = cfg.gp.outputs[j].factor;
+                    if (cfg.gp.factors[f].head_rows > 0) shi[j] = sd_s[slot * SLB_MAX_OUT + f];
+                }
+                int outcome = 0;
+                if (a.screened) {
+                    // the same two comparisons as the round loop: the screened box, then the fp64 mean
+                    double mu[SLB_MAX_OUT], dm[SLB_MAX_OUT], zero[SLB_MAX_OUT];
+                    for (int j = 0; j < SLB_MAX_OUT; ++j) { mu[j] = t.coef[j]; dm[j] = t.dm[j]; zero[j] = 0.0; }
+                    const double vx = t.dec0;
+                    mean_decision_terms(cfg, t, vx, mu, zero);
+                    t.guard += screening_slack(cfg, mu, dm, shi);
+                    outcome = mine ? decide(t, shi, cfg.gp.num_outputs) : 0;
+                    head_mark(a, HM_SCREENED);
+                    if (mine && outcome < 0) {
+                        double merr[SLB_MAX_OUT];
+                        for (int j = 0; j < SLB_MAX_OUT; ++j) {
+                            mu[j] = mu_s[slot * SLB_MAX_OUT + j];
+                            merr[j] = merr_s[slot * SLB_MAX_OUT + j];
+                        }
+                        mean_decision_terms(cfg, t, vx, mu, merr);
+                        outcome = decide(t, shi, cfg.gp.num_outputs);
+                    }
+                } else {
+                    outcome = mine ? decide(t, shi, cfg.gp.num_outputs) : 0;
+                }
+                head_mark(a, HM_DECIDED);
+                head_group_finish(a, mine, outcome, rel, s_stat);
+            }
+            __syncthreads();                              // sd_s, mu_s are the next round's
+        }
+    } else {
+        // round: warp w takes group grp0 + w gridDim (every warp of the CTA makes the same number of rounds)
+        int round = 0;
+        for (int64_t grp0 = blockIdx.x; grp0 < ngroups; grp0 += nwarps, ++round) {
+            const int64_t grp = grp0 + (int64_t)warp * gridDim.x;
+            const bool active = grp < ngroups;
+            const int lane = threadIdx.x & 31;
+            filter_side t;
+            int64_t rel = 0;
+            bool mine = false, need = false;
+            double shi[SLB_MAX_OUT];
+            double vx = 0.0;
+            int outcome = 0;
+            if (active) {
+                if (a.head_factors_staged == nf)
+                    head_group_bound<DIN, HP, true>(cfg, a, grp, count, exptab, kw, wbuf, xbuf, bar, t, rel, mine, shi);
+                else
+                    head_group_bound<DIN, HP, false>(cfg, a, grp, count, exptab, kw, wbuf, xbuf, bar, t, rel, mine, shi);
+                if (a.screened) {
+                    // first with the screened mean and its error box (stage 1 left them in the entry): most
+                    // entries are decided by the tighter variance bound alone
+                    double mu[SLB_MAX_OUT], dm[SLB_MAX_OUT], zero[SLB_MAX_OUT];
+                    for (int j = 0; j < SLB_MAX_OUT; ++j) { mu[j] = t.coef[j]; dm[j] = t.dm[j]; zero[j] = 0.0; }
+                    vx = t.dec0;
+                    mean_decision_terms(cfg, t, vx, mu, zero);
+                    t.guard += screening_slack(cfg, mu, dm, shi);
+                    outcome = mine ? decide(t, shi, cfg.gp.num_outputs) : 0;
+                    need = mine && outcome < 0;
+                    if (need) need_s[2 + atomicAdd(need_s + (round & 1), 1)] = warp * HP + lane;
+                    head_mark(a, HM_SCREENED);
+                } else {
+                    outcome = mine ? decide(t, shi, cfg.gp.num_outputs) : 0;
                 }
             }
+            if (a.screened) {
+                if (threadIdx.x == 0) need_s[(round + 1) & 1] = 0;       // the next round's counter
+                __syncthreads();
+                const int nneed = need_s[round & 1];
+                if (nneed > 0) {
+                    // the rest gets its mean in fp64 (all warps), then the same comparison as the fp64 path
+                    slb_bulk::mbar_wait(bar + 2, 0);
+                    head_round_means<DIN>(cfg, a, need_s + 2, nneed, grp0, count, mbuf, tab512, mu_s, merr_s, 0, HT);
+                    head_mark(a, HM_MEANS);
+                    __syncthreads();
+                    if (need) {
+                        double mu[SLB_MAX_OUT], merr[SLB_MAX_OUT];
+                        const int slot = warp * HP + lane;
+                        for (int j = 0; j < SLB_MAX_OUT; ++j) {
+                            mu[j] = mu_s[slot * SLB_MAX_OUT + j];
+                            merr[j] = merr_s[slot * SLB_MAX_OUT + j];
+                        }
+                        mean_decision_terms(cfg, t, vx, mu, merr);
+                        outcome = decide(t, shi, cfg.gp.num_outputs);
+                    }
+                }
+            }
+            if (active) {
+                head_mark(a, HM_DECIDED);
+                head_group_finish(a, mine, outcome, rel, s_stat);
+            }
         }
-        if (active) head_group_finish(a, mine, outcome, rel, s_stat);
     }
     // one pair of global atomics per CTA (one per point serialised on the counter's L2 line)
+    head_wait_landings(bar);
     __syncthreads();
     if (a.stats != nullptr && threadIdx.x < 2 && s_stat[threadIdx.x] != 0)
         atomicAdd(a.stats + 1 + threadIdx.x, (unsigned long long)s_stat[threadIdx.x]);
+    if (threadIdx.x == 0) head_mark(a, HM_EXIT);
 }
 
 double* g_probe_mu = nullptr;          // slb_debug_screening_probe
 double* g_probe_dm = nullptr;
+unsigned long long* g_head_timing = nullptr;   // slb_debug_head_timing
 int g_filter_stages = 3;               // slb_debug_filter_stages: bit 0 head stage, bit 1 refine pass,
-                                       // bit 2 forces the fp64 mean stage (no fp32 screening)
+                                       // bit 2 forces the fp64 mean stage (no fp32 screening), bit 3 /
+                                       // bit 4 force the head stage's split schedule / round loop
 
 // The fp32 screening kernel needs closed-form bounds of V and L_V over a box of means
 // (screening_slack): plain RBF factors, V = QUADRATIC (optional scale) on the GP outputs, L_V constant
@@ -800,7 +956,7 @@ bool screening_applicable(const slb_sweep& cfg) {
 // when the fp32 screening kernel is stage 1 -- every factor's [Xf | gamma_f] next to them.  Screening
 // is only used when all of it fits (otherwise the fp64 mean stage runs, whose list entries are complete).
 void head_layout(const slb_sweep& cfg, int din, filter_args& ah, size_t& head_smem) {
-    const size_t head_fixed = 16 + (576 + HW * HR * HP) * sizeof(double);
+    const size_t head_fixed = 32 + (576 + HW * HR * HP + HW * HP * SLB_MAX_OUT) * sizeof(double);
     const size_t per_factor = (size_t)(HR * HR + HR * din) * sizeof(double);
     ah.head_factors_staged = cfg.gp.num_factors;
     while (ah.head_factors_staged > 0 && head_fixed + ah.head_factors_staged * per_factor > 226 * 1024)
@@ -809,6 +965,7 @@ void head_layout(const slb_sweep& cfg, int din, filter_args& ah, size_t& head_sm
     ah.screened = 0;
     ah.mean_doubles = 0;
     ah.prefetch_factors = (g_filter_stages & 2) ? 1 : 0;
+    ah.head_schedule = (g_filter_stages >> 3) & 3;
     if (screening_applicable(cfg) && ah.head_factors_staged == cfg.gp.num_factors) {
         int off = 0;
         for (int f = 0; f < cfg.gp.num_factors; ++f) {
@@ -847,11 +1004,14 @@ int launch_filter(cudaStream_t st, const slb_sweep& cfg, const filter_args& a, s
     head_layout(cfg, DIN, ah, head_smem);
     ah.probe_mu = g_probe_mu;
     ah.probe_dm = g_probe_dm;
+    ah.timing = g_head_timing;
     if (ah.screened) {
         const size_t smem32 = mean32_smem_bytes(DIN, a.max_outputs_per_factor, a.chunk_rows, FT / 32);
         filter_mean32_kernel<DIN><<<(unsigned)blocks, FT, smem32, st>>>(cfg, ah);
     } else {
-        filter_mean_kernel<DIN><<<(unsigned)blocks, FT, smem, st>>>(cfg, a);
+        filter_args a1 = a;
+        a1.timing = g_head_timing;
+        filter_mean_kernel<DIN><<<(unsigned)blocks, FT, smem, st>>>(cfg, a1);
     }
     SLB_LAUNCH_CHECK();
     if (!(g_filter_stages & 1)) return 0;
@@ -886,6 +1046,11 @@ int slb_filter_stage1(const slb_sweep* cfg) {
 int slb_debug_screening_probe(double* mu_dev, double* dm_dev) {
     g_probe_mu = (mu_dev != nullptr && dm_dev != nullptr) ? mu_dev : nullptr;
     g_probe_dm = g_probe_mu != nullptr ? dm_dev : nullptr;
+    return 0;
+}
+
+int slb_debug_head_timing(void* buffer_dev) {
+    g_head_timing = static_cast<unsigned long long*>(buffer_dev);
     return 0;
 }
 
