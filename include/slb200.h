@@ -339,9 +339,10 @@ int         slb_restore_tables(void* dst_dev, const void* src_host, int64_t spli
  * complete with bits 0 and 1 set -- 3, the default, or 7): bit 0 runs the head stage, bit 1 the
  * refine pass; bit 2 forces the fp64 mean stage where the fp32 screening stage would run; bit 3
  * forces the head stage's split schedule (a warp per group and factor, means on the spare warps),
- * bit 4 its round loop (a warp per group), which it otherwise chooses from the list length */
+ * bit 4 its round loop (a warp per group), which it otherwise chooses from the list length; bit 5
+ * forces the fp32 screening kernel where the factored grid mean would run (slb_filter_mean_scheme) */
 int         slb_debug_filter_stages(int32_t mask);
-/* diagnostics: while both pointers are non-NULL, the fp32 screening stage of
+/* diagnostics: while both pointers are non-NULL, the fp32 screening stage (or the factored grid mean) of
  * slb_lyapunov_sweep_filtered also writes, for every point of the swept range (row = index relative to
  * idx_begin of the LAST pass), its screened mean [n, D] and the certified bound of its error [n, D]
  * (+inf where the point is left to the fp64 stages); tests hold |mean - fp64 mean| <= bound */
@@ -415,6 +416,17 @@ int64_t slb_filter_workspace(int64_t n);
  * the head stage's shared memory) with an fp64 mean only for the points its error box leaves open;
  * 64 = the fp64 mean kernel; 0 = no GP */
 int slb_filter_stage1(const slb_sweep* cfg);
+/* how that first stage computes the mean: SLB_MEAN_FP64 per point (the fp64 mean kernel);
+ * SLB_MEAN_FP32_SCREENED per point in fp32 with a certified bound (stage 1 = 32); SLB_MEAN_GRID_FACTORED
+ * (also stage 1 = 32: the same screened list entries) per tile of a 2-D grid from per-axis tables of
+ * kernel values contracted in fp64, with an fp64-class certified bound -- plain RBF factors on
+ * [x0, x1, u] and a LINEAR one-output policy with at most SATURATE and SCALE; bit 5 of
+ * slb_debug_filter_stages forces the fp32 screening kernel instead.  SLB_MEAN_NONE: no GP. */
+#define SLB_MEAN_NONE 0
+#define SLB_MEAN_FP64 1
+#define SLB_MEAN_FP32_SCREENED 2
+#define SLB_MEAN_GRID_FACTORED 3
+int slb_filter_mean_scheme(const slb_sweep* cfg);
 int slb_lyapunov_sweep_filtered(void* stream, const slb_sweep* cfg, int64_t idx_begin,
                                 int64_t idx_end, uint8_t* negative_dev, double* values_dev,
                                 void* workspace_dev, int64_t* stats_dev);

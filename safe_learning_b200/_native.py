@@ -29,6 +29,8 @@ ABI_VERSION = 6
 # slb_value_solve: stats slots and status codes (include/slb200.h)
 VALUE_STATS = 16
 VALUE_CONVERGED, VALUE_MAX_ITERS, VALUE_NEGATIVE_WEIGHT, VALUE_NOT_CONTRACTIVE, VALUE_NAN = range(5)
+# slb_filter_mean_scheme: how stage 1 of the filtered sweep computes the GP mean (include/slb200.h)
+MEAN_NONE, MEAN_FP64, MEAN_FP32_SCREENED, MEAN_GRID_FACTORED = range(4)
 
 UINT64_MAX = (1 << 64) - 1
 INT64_MAX = (1 << 63) - 1
@@ -138,6 +140,7 @@ SIGNATURES = {
     "slb_debug_filter_stages": (C.c_int, [_i32]),
     "slb_debug_screening_probe": (C.c_int, [_dp, _dp]),
     "slb_filter_stage1": (C.c_int, [C.POINTER(SlbSweep)]),
+    "slb_filter_mean_scheme": (C.c_int, [C.POINTER(SlbSweep)]),
     "slb_packed_len": (C.c_int64, [_i32]),
     "slb_pack_factor": (C.c_int, [_vp, _dp, _i32, _dp]),
     "slb_pivoted_subset": (C.c_int, [_vp, _dp, _i32, _i32, _vp, _dp]),

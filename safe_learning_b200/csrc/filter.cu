@@ -76,6 +76,9 @@ struct filter_args {
     double* probe_dm;                  // ... and their certified error bounds (inf: point left to fp64)
     unsigned long long* timing;        // slb_debug_head_timing: nullptr or [HEAD_CTAS + 1][8] %globaltimer
     int head_schedule;                 // head stage: 0 chosen from the list length, 1 split, 2 round loop
+    int grid_means;                    // stage 1 was the factored grid kernel: a list A entry whose bounds
+                                       // dm are all finite carries an fp64-class mean (no recompute);
+                                       // counts[2] is the number of the other entries
 };
 
 // slb_debug_head_timing: timing[slot] = the latest %globaltimer (ns) at which a warp passed a mark.
@@ -372,6 +375,366 @@ filter_mean32_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a)
     timing_mark(a, HEAD_CTAS * 8);
 }
 
+// ---- stage 1, factored grid mean ----------------------------------------------------------------------
+// On a 2-D grid with plain RBF factors on z = [x0, x1, u] and the policy u = clip(a x0 + b x1, lo, hi)
+// (a LINEAR map, optionally saturated and scaled), the kernel values of a tile of grid points factor
+// into per-axis tables and the mean of the tile is a small matrix product on the fp64 tensor pipe.
+// In a factor's units (w = z / l; xs_j the staged training rows) and on a region where the policy is
+// affine, w2 = alpha w0 + beta w1 + const (alpha = a' l0 / l2, beta = b' l1 / l2, a' b' the scaled
+// row; alpha = beta = 0 where u is saturated, a constant).  Centre the tile at cw (cw2 the affine value
+// there), xi = w0 - cw0, eta = w1 - cw1, D_j = cw - xs_j; the exponent -|w - xs_j|^2 / 2 expands to
+//     -|D_j|^2 / 2  -  xi p_j  -  eta q_j  -  (xi^2 + eta^2 + (alpha xi + beta eta)^2) / 2,
+//     p_j = D_j0 + alpha D_j2,  q_j = D_j1 + beta D_j2,
+// so  mean_o[i, k] = Q[i, k] sum_j (gamma_oj exp(-|D_j|^2 / 2) E0[i, j]) E1[k, j],
+//     E0[i, j] = exp(-xi_i p_j),  E1[k, j] = exp(-eta_k q_j),  Q = exp(-(...) / 2) <= 1:
+// The tables run on the uniform offsets xi_i = (i - 8) h0, h0 = unit0 / l0 (eta likewise): a column of
+// E0 is g^(i - 8), g = exp(-h0 p_j), from two exponentials and 15 products -- 5 M exponentials per tile
+// and regime (two per table column, one weight) instead of GR GC M -- and GR GC M fp64 FMAs in DMMA
+// m8n8k4 (warp w: the 8 x 8 block (w / GCB, w % GCB) of the tile; its C fragment is its lanes' points).
+// A tile computes every regime its points are in (saturated low / high, affine), each point keeps its
+// own.  The summation order is fixed: two runs are bit-identical.
+// Certified bound (u = 2^-53, rho = max|xi| sqrt(1 + alpha^2) + max|eta| sqrt(1 + beta^2) >= |w - cw|,
+// s_j = |D_j|, Sg = gamma_l1 >= sum_j |gamma_oj|):
+//   each term: the weight and Q from one exp_neg_fast each (EPS_K relative; its reduction x = n ln2 / 512
+//     + r is the same for positive arguments, |x| <= 294 here), each table entry a power |o| <= 8 of one
+//     (8 (EPS_K + 2 u)), three products; arguments from D (one rounding each), K, p, q (fma chains), h p
+//     and xi = fl(o h): relative error <= 18 EPS_K + u (3.5 (s_j + rho)^2 + 43) of the exact k_j;
+//     k_j <= exp(-max(s_j - rho, 0)^2 / 2), so its contribution is <= (18 EPS_K + u (3.5 (sqrt(rho^2 + 2)
+//     + rho)^2 + 43)) |gamma_j|;
+//   the M-term sum (two DMMA chains): <= (Mp + 4) u sum_j |gamma_j| k_j (the tables' product exceeds k_j
+//     by 1 / Q, the final product with Q takes it back);
+//   the point itself: the grid's w0 = fl(x0 / l0) is within dev (computed, + 2 u |xi|) of cw0 + xi (w1
+//     likewise; on the affine region w2 moves by |alpha| dev + |beta| dev with them); the policy's
+//     fl(fl(x0 a) + fl(x1 b)) scaled, alpha, beta and cw2 are within 10 u (|alpha| W0 + |beta| W1) of
+//     the affine w2 (W = max |w| over the tile); |d k_j / d w_c| <= 1, so each enters times sum |gamma|;
+//   dropped rows (|D_j|^2 > GRID_K_DROP: weight 0): each k_j <= exp(-(sqrt(K_DROP) - rho)^2 / 2);
+//     products that leave the fp64 range downwards: < 1e-150 (Mp + 1) absolute (|table args| <=
+//     rho sqrt(K_DROP) <= 294);
+//   the other evaluation orders of the same mean (gamma itself and the a . alpha form of the full
+//     posterior, its expanded distance): 7e-16 (M + 8) + 4.5e-16 (|w|^2 / 2 + hmax), as mean_output_finish.
+// dm = 1.05 (sum of the above) Sg / |scale|.  A tile and regime with rho > GRID_RHO_MAX or a non-finite
+// constant leaves its points to the fp64 route (dm = inf), like points the prologue finds insane.
+constexpr int GR = 16, GC = 16;        // grid rows (axis 0) x columns (axis 1, contiguous) per CTA tile
+constexpr int GCB = GC / 8;            // column blocks
+constexpr int GT = GR * GC / 2;        // threads: one warp per 8 x 8 block, two points per thread (two CTAs
+                                       // per SM: one's barriers and round trips hide behind the other)
+constexpr int GJ = 128;                // training rows per chunk of the tables
+constexpr int GNO = 4;                 // outputs per factor (screening_applicable: at most 4 outputs)
+constexpr double GRID_RHO_MAX = 12.0;
+constexpr double GRID_K_DROP = 600.0;
+constexpr int GFS = 36;                // doubles per fragment (32 used): the recurrence's column stores hit
+                                       // every bank pair once, the contraction's loads stay contiguous
+constexpr int GTAB = (GR / 8) * (GJ / 4) * GFS;   // one table of a chunk, in fragments
+constexpr int GSMEM_PRE_TAB = 2 * GTAB + GNO * GJ + 2 * GJ + 2 * (GR + GC);   // doubles before the exp table
+static_assert(GR == 16 && GC == 16, "the recurrence runs 8 steps each way from the tile's centre");
+
+inline size_t grid_mean_smem_bytes() {
+    return (size_t)(GSMEM_PRE_TAB + 512) * sizeof(double);
+}
+
+// one factor with NO outputs (compile-time: accumulators in registers) for the tile; writes mu / dm of
+// the thread's two points for the factor's outputs
+template <int NO>
+SLB_DEV void grid_mean_factor(const slb_sweep& cfg, int f, const int* outs, double* smem, const double* tab,
+                              int64_t row0,
+                              int64_t col0, const double (*z)[3], const int* reg, double (*mu)[GNO],
+                              double (*dm)[GNO]) {
+    const slb_gp_factor& F = cfg.gp.factors[f];
+    const slb_grid& g = cfg.grid;
+    const slb_function& pol = cfg.policy;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int rb = warp / GCB, cb = warp % GCB;
+    double* e0f = smem;                        // [GR / 8][J / 4][GFS]: DMMA A fragments
+    double* e1f = e0f + GTAB;                  // [GC / 8][J / 4][GFS]: DMMA B fragments
+    double* wg = e1f + GTAB;                   // [NO][GJ] gamma_oj exp(-|D_j|^2 / 2)
+    double* pq = wg + GNO * GJ;                // [2][GJ]
+    double* xi = pq + 2 * GJ;                  // [GR] xi of the tables: (i - GR / 2) h0
+    double* eta = xi + GR;                     // [GC]
+    double* dev = eta + GC;                    // [GR + GC] |w - cw - xi| of the grid's own points
+    const double l0 = F.lengthscales[0], l1 = F.lengthscales[1], l2 = F.lengthscales[2];
+    // the centre: grid point (GR / 2, GC / 2) of the tile, in the factor's units
+    const double cw0 = f64add(f64mul((double)(row0 + GR / 2), g.unit_maxes[0]), g.offset[0]) / l0;
+    const double cw1 = f64add(f64mul((double)(col0 + GC / 2), g.unit_maxes[1]), g.offset[1]) / l1;
+    __syncthreads();                           // the previous factor is done with the tables
+    // the tables run on the uniform offsets xi_i = (i - GR / 2) h0, h0 = unit / l0 (a recurrence along the
+    // axis); the grid's own points are within dev of them (a perturbation of the point, in the bound)
+    const double h0 = g.unit_maxes[0] / l0, h1 = g.unit_maxes[1] / l1;
+    if (threadIdx.x < GR + GC) {
+        const int c = threadIdx.x < GR ? 0 : 1;
+        const int i = c == 0 ? threadIdx.x : threadIdx.x - GR;
+        const int64_t gi = (c == 0 ? row0 : col0) + i;
+        const double x = f64add(f64mul((double)gi, g.unit_maxes[c]), g.offset[c]);   // grid_index_to_state
+        const double ideal = (double)(i - GR / 2) * (c == 0 ? h0 : h1);
+        xi[threadIdx.x] = ideal;
+        dev[threadIdx.x] = fabs((x / (c == 0 ? l0 : l1) - (c == 0 ? cw0 : cw1)) - ideal);
+    }
+    __syncthreads();
+    double mxi = 0.0, meta = 0.0, pert = 0.0;
+#pragma unroll
+    for (int r = 0; r < GR; ++r) mxi = fmax(mxi, fabs(xi[r]));
+#pragma unroll
+    for (int k = 0; k < GC; ++k) meta = fmax(meta, fabs(eta[k]));
+#pragma unroll
+    for (int k = 0; k < GR + GC; ++k) pert = fmax(pert, dev[k]);
+    const int ti = rb * 8 + (lane >> 2);
+    const int tk0 = cb * 8 + 2 * (lane & 3);
+    const int Mp = padded_rows(F.M);
+    const double u53 = 1.1102230246251565e-16;
+    const double sc = (pol.flags & SLB_FLAG_SCALE) ? pol.out_scale : 1.0;
+    for (int r = 0; r < 3; ++r) {
+        if (!__syncthreads_or(reg[0] == r || reg[1] == r)) continue;
+        double alpha = 0.0, beta = 0.0, cw2;
+        if (r == 2) {
+            alpha = f64mul(f64mul(__ldg(pol.matrix + 0), sc), l0) / l2;
+            beta = f64mul(f64mul(__ldg(pol.matrix + 1), sc), l1) / l2;
+            cw2 = fma(alpha, cw0, f64mul(beta, cw1));
+        } else {
+            const double lim = r == 0 ? pol.lower : pol.upper;
+            cw2 = ((pol.flags & SLB_FLAG_SCALE) ? f64mul(lim, pol.out_scale) : lim) / l2;
+        }
+        const double rho = mxi * sqrt(fma(alpha, alpha, 1.0)) + meta * sqrt(fma(beta, beta, 1.0));
+        const bool ok = rho <= GRID_RHO_MAX && fabs(cw0) < 1e100 && fabs(cw1) < 1e100 && fabs(cw2) < 1e100 &&
+                        fabs(alpha) < 1e100 && fabs(beta) < 1e100;
+        double acc[NO][2][2];
+#pragma unroll
+        for (int q = 0; q < NO; ++q) { acc[q][0][0] = acc[q][0][1] = acc[q][1][0] = acc[q][1][1] = 0.0; }
+        // the thread's training row of a chunk (GT == GJ), loaded one chunk ahead: its L2 round trip runs
+        // behind the previous chunk's tables and contraction
+        static_assert(GT == GJ, "one training row per thread and chunk");
+        double nx[3] = {0.0, 0.0, 0.0}, ng[NO];
+#pragma unroll
+        for (int q = 0; q < NO; ++q) ng[q] = 0.0;
+        if (ok && (int)threadIdx.x < Mp) {
+            const double2 x01 = *reinterpret_cast<const double2*>(F.Xf + (size_t)threadIdx.x * 4);
+            nx[0] = x01.x; nx[1] = x01.y; nx[2] = F.Xf[(size_t)threadIdx.x * 4 + 2];
+#pragma unroll
+            for (int q = 0; q < NO; ++q) ng[q] = cfg.gp.outputs[outs[q]].gamma_f[threadIdx.x];
+        }
+        for (int j0 = 0; ok && j0 < Mp; j0 += GJ) {
+            const int J = min(GJ, Mp - j0), J4 = J >> 2;
+            __syncthreads();                   // the previous chunk's tables are consumed
+            if ((int)threadIdx.x < J) {
+                const double d0 = cw0 - nx[0], d1 = cw1 - nx[1], d2 = cw2 - nx[2];
+                const double K = fma(d0, d0, fma(d1, d1, d2 * d2));
+                const bool keep = K <= GRID_K_DROP;          // dropped rows: weight 0, tables of ones
+                bool far;
+                const double w = keep ? exp_neg_fast(-0.5 * K, tab, far) : 0.0;
+                pq[threadIdx.x] = keep ? fma(alpha, d2, d0) : 0.0;
+                pq[GJ + threadIdx.x] = keep ? fma(beta, d2, d1) : 0.0;
+#pragma unroll
+                for (int q = 0; q < NO; ++q) wg[q * GJ + threadIdx.x] = ng[q] * w;
+            }
+            const int jn = j0 + GJ + (int)threadIdx.x;
+            if (jn < Mp) {
+                const double2 x01 = *reinterpret_cast<const double2*>(F.Xf + (size_t)jn * 4);
+                nx[0] = x01.x; nx[1] = x01.y; nx[2] = F.Xf[(size_t)jn * 4 + 2];
+#pragma unroll
+                for (int q = 0; q < NO; ++q) ng[q] = cfg.gp.outputs[outs[q]].gamma_f[jn];
+            }
+            __syncthreads();
+            // one table column (training row jj, axis c) per task: exp(-o h p) = g^o for the offsets
+            // o = -8 .. 7 from two exps g = exp(-h p), 1 / g = exp(h p) and products outwards from o = 0
+            for (int task = threadIdx.x; task < 2 * J; task += GT) {
+                const int c = task >= J ? 1 : 0, jj = task - c * J;
+                const double t = (c ? h1 : h0) * pq[c * GJ + jj];
+                bool far;
+                const double gd = exp_neg_fast(-t, tab, far), gu = exp_neg_fast(t, tab, far);
+                double* col = (c ? e1f : e0f) + (jj >> 2) * GFS + (jj & 3);   // + block (m / 8) J4 GFS + (m % 8) 4
+                col[J4 * GFS] = 1.0;                                          // m = 8: o = 0
+                double v = 1.0;
+#pragma unroll
+                for (int o = 1; o < 8; ++o) { v *= gd; col[J4 * GFS + o * 4] = v; }      // m = 8 + o
+                v = 1.0;
+#pragma unroll
+                for (int o = 1; o <= 8; ++o) { v *= gu; col[(8 - o) * 4] = v; }          // m = 8 - o
+            }
+            __syncthreads();
+            const double* pa = e0f + rb * J4 * GFS + lane;
+            const double* pb = e1f + cb * J4 * GFS + lane;
+#pragma unroll 2
+            for (int s = 0; s < J4; s += 2) {            // J4 is even (rows padded to 8)
+                double af[2][NO], bf[2];
+#pragma unroll
+                for (int t = 0; t < 2; ++t) {
+                    const double a0 = pa[(s + t) * GFS];
+                    bf[t] = pb[(s + t) * GFS];
+#pragma unroll
+                    for (int q = 0; q < NO; ++q) af[t][q] = a0 * wg[q * GJ + 4 * (s + t) + (lane & 3)];
+                }
+#pragma unroll
+                for (int q = 0; q < NO; ++q) {
+                    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
+                                 : "+d"(acc[q][0][0]), "+d"(acc[q][0][1]) : "d"(af[0][q]), "d"(bf[0]));
+                    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
+                                 : "+d"(acc[q][1][0]), "+d"(acc[q][1][1]) : "d"(af[1][q]), "d"(bf[1]));
+                }
+            }
+        }
+        // the bound of this tile and regime (relative to gamma_l1, see above)
+        const double W0 = fabs(cw0) + mxi, W1 = fabs(cw1) + meta;
+        const double W2 = r == 2 ? fabs(alpha) * W0 + fabs(beta) * W1 : fabs(cw2);
+        const double sq = sqrt(rho * rho + 2.0) + rho, kd = sqrt(GRID_K_DROP) - rho;
+        const double eps = 1.05 * (18.2 * EPS_K + u53 * (1.01 * (3.5 * sq * sq + 43.0) + 1.02 * (Mp + 4)) +
+                                   1.01 * pert * (r == 2 ? 2.0 + fabs(alpha) + fabs(beta) : 2.0) +
+                                   u53 * (2.0 * (mxi + meta) + (r == 2 ? 10.0 * W2 : 2.0 * W2)) +
+                                   4.5e-16 * (0.5 * (W0 * W0 + W1 * W1 + W2 * W2) + F.hmax) + 7e-16 * (F.M + 8) +
+                                   exp(-0.5 * kd * kd));
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            if (reg[h] != r) continue;
+            const double x0 = xi[ti], e1 = eta[tk0 + h];
+            const double v = fma(alpha, x0, beta * e1);
+            bool far;
+            const double Q = exp_neg_fast(-0.5 * fma(x0, x0, fma(e1, e1, v * v)), tab, far);
+#pragma unroll
+            for (int q = 0; q < NO; ++q) {
+                const slb_gp_output& G = cfg.gp.outputs[outs[q]];
+                double mx = 0.0;
+                if (G.prior_mean != nullptr) {
+                    mx = f64mul(z[h][0], G.prior_mean[0]);
+#pragma unroll
+                    for (int c = 1; c < 3; ++c) mx = f64add(mx, f64mul(z[h][c], G.prior_mean[c]));
+                    mx = f64mul(F.scale, mx);
+                }
+                const double m = f64add(f64mul(acc[q][0][h] + acc[q][1][h], Q), mx) / F.scale;
+                const double bound = ok && eps < 1e-3
+                                         ? (eps * G.gamma_l1 + 1e-150 * (Mp + 1)) / fabs(F.scale) + 1e-300
+                                         : __longlong_as_double(0x7ff0000000000000ll);
+#pragma unroll
+                for (int o = 0; o < GNO; ++o)
+                    if (o == outs[q]) { mu[h][o] = m; dm[h][o] = bound; }
+            }
+        }
+    }
+}
+
+template <int DIN>
+__global__ void __launch_bounds__(GT, 2)
+filter_grid_mean_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
+    static_assert(DIN == 3, "the factored grid mean is written for z = [x0, x1, u]");
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    double* smem = reinterpret_cast<double*>(smem_raw);
+    double* tab = smem + GSMEM_PRE_TAB;                                  // [512] of exp_neg_fast
+    for (int i = threadIdx.x; i < 512; i += GT) tab[i] = g_exp_tables[i];   // visible after the first barrier
+    prefetch_descriptor_operands(cfg);
+    // the training rows and weights every tile reads chunk by chunk: into L2 while the prologue runs
+    for (int f = 0; f < cfg.gp.num_factors; ++f) {
+        const size_t bytes = (size_t)padded_rows(cfg.gp.factors[f].M) * 4 * sizeof(double);
+        for (size_t off = (size_t)threadIdx.x * 128; off < bytes; off += (size_t)GT * 128)
+            asm volatile("prefetch.global.L2 [%0];" ::"l"(reinterpret_cast<const char*>(cfg.gp.factors[f].Xf) + off));
+    }
+    for (int o = 0; o < cfg.gp.num_outputs; ++o) {
+        const size_t bytes = (size_t)padded_rows(cfg.gp.factors[cfg.gp.outputs[o].factor].M) * sizeof(double);
+        for (size_t off = (size_t)threadIdx.x * 128; off < bytes; off += (size_t)GT * 128)
+            asm volatile("prefetch.global.L2 [%0];" ::"l"(reinterpret_cast<const char*>(cfg.gp.outputs[o].gamma_f) + off));
+    }
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int64_t n0 = cfg.grid.num_points[0], n1 = cfg.grid.num_points[1];
+    const int64_t ntc = (n1 + GC - 1) / GC;
+    const int64_t row0 = a.idx_begin / n1 + (int64_t)(blockIdx.x / ntc) * GR;
+    const int64_t col0 = (int64_t)(blockIdx.x % ntc) * GC;
+    const int D = cfg.gp.num_outputs;
+    const slb_function& pol = cfg.policy;
+
+    // ---- the thread's two points (its lanes' C-fragment positions): x, V(x), threshold(x), u = policy(x)
+    const int64_t gi = row0 + (warp / GCB) * 8 + (lane >> 2);
+    double z[2][3], vx[2], thr[2];
+    bool valid[2], sane[2];
+    int64_t rel[2];
+    int reg[2];
+    const double ulo = (pol.flags & SLB_FLAG_SCALE) ? f64mul(pol.lower, pol.out_scale) : pol.lower;
+    const double uhi = (pol.flags & SLB_FLAG_SCALE) ? f64mul(pol.upper, pol.out_scale) : pol.upper;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int64_t gk = col0 + (warp % GCB) * 8 + 2 * (lane & 3) + h;
+        const int64_t flat = gi * n1 + gk;
+        valid[h] = gi < n0 && gk < n1 && flat >= a.idx_begin && flat < a.idx_begin + a.n;
+        rel[h] = valid[h] ? flat - a.idx_begin : 0;   // every thread stays for the block barriers
+        double x[SLB_MAX_IN];
+        grid_index_to_state(cfg.grid, a.idx_begin + rel[h], x);
+        lyapunov_state_terms(cfg, x, a.idx_begin + rel[h], &vx[h], &thr[h]);
+        double u[SLB_MAX_OUT];
+        eval_fn_small(pol, x, u);
+        z[h][0] = x[0]; z[h][1] = x[1]; z[h][2] = u[0];
+        sane[h] = fabs(x[0]) < 1e100 && fabs(x[1]) < 1e100 && fabs(u[0]) < 1e100;
+        // the regime is the clip the policy computed: saturated points carry the constant itself
+        reg[h] = !(valid[h] && sane[h]) ? -1
+                 : (pol.flags & SLB_FLAG_SATURATE) && u[0] == ulo ? 0
+                 : (pol.flags & SLB_FLAG_SATURATE) && u[0] == uhi ? 1 : 2;
+    }
+
+    // ---- posterior means, factor by factor
+    double mu[2][GNO], dm[2][GNO];
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int o = 0; o < GNO; ++o) { mu[h][o] = 0.0; dm[h][o] = __longlong_as_double(0x7ff0000000000000ll); }
+    for (int f = 0; f < cfg.gp.num_factors; ++f) {
+        int outs[SLB_MAX_OUT];
+        int no = 0;
+        for (int o = 0; o < D; ++o)
+            if (cfg.gp.outputs[o].factor == f) outs[no++] = o;
+        switch (no) {
+        case 1: grid_mean_factor<1>(cfg, f, outs, smem, tab, row0, col0, z, reg, mu, dm); break;
+        case 2: grid_mean_factor<2>(cfg, f, outs, smem, tab, row0, col0, z, reg, mu, dm); break;
+        case 3: grid_mean_factor<3>(cfg, f, outs, smem, tab, row0, col0, z, reg, mu, dm); break;
+        case 4: grid_mean_factor<4>(cfg, f, outs, smem, tab, row0, col0, z, reg, mu, dm); break;
+        default: break;
+        }
+    }
+
+    // ---- per point: the comparison over mu +- dm and sigma_j in [0, prior sigma_j] (as filter_mean32_kernel)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        double m[SLB_MAX_OUT], d[SLB_MAX_OUT], zero[SLB_MAX_OUT];
+        bool fp64 = true;
+#pragma unroll
+        for (int j = 0; j < SLB_MAX_OUT; ++j) {
+            m[j] = j < GNO ? mu[h][j] : 0.0;
+            d[j] = j < GNO ? dm[h][j] : 0.0;
+            zero[j] = 0.0;
+            if (j < D) fp64 &= d[j] < __longlong_as_double(0x7ff0000000000000ll);
+        }
+        if (a.probe_mu != nullptr && valid[h]) {
+            for (int o = 0; o < D; ++o) {
+                a.probe_mu[rel[h] * D + o] = m[o];
+                a.probe_dm[rel[h] * D + o] = sane[h] ? d[o] : __longlong_as_double(0x7ff0000000000000ll);
+            }
+        }
+        filter_side t;
+        t.thr = thr[h];
+        mean_decision_terms(cfg, t, vx[h], m, zero);
+        double shi[SLB_MAX_OUT];
+        for (int j = 0; j < D; ++j) shi[j] = sqrt(cfg.gp.factors[cfg.gp.outputs[j].factor].variance);
+        t.guard += screening_slack(cfg, m, d, shi);
+        const int outcome = sane[h] ? decide(t, shi, D) : -1;
+        const bool undecided = valid[h] && outcome < 0;
+        if (valid[h]) {
+            a.negative[rel[h]] = outcome > 0 ? 1 : 0;
+            if (a.values != nullptr) a.values[rel[h]] = vx[h];
+        }
+        const long long slot = list_append(undecided, a.counts + 0);
+        if (undecided) {
+            filter_side* dst = a.side_a + slot;
+            dst->dec0 = vx[h];                    // the screened layout: the head stage rebuilds the rest
+            dst->thr = thr[h];
+#pragma unroll
+            for (int c = 0; c < DIN; ++c) dst->z[c] = z[h][c];
+            for (int j = 0; j < D; ++j) {
+                dst->coef[j] = m[j];
+                dst->dm[j] = sane[h] ? d[j] : __longlong_as_double(0x7ff0000000000000ll);
+            }
+            a.list_a[slot] = rel[h];
+        }
+        count_stat(undecided && !(sane[h] && fp64), a.counts + 2);
+        if (a.stats != nullptr) {
+            count_stat(valid[h] && !undecided, a.stats + 0);
+            count_stat(valid[h], a.stats + 3);
+        }
+    }
+    timing_mark(a, HEAD_CTAS * 8);
+}
+
 // ---- stage 2: variance given the head subset, one warp per HP undecided points ---------------------
 // One CTA per SM, 8 warps.  The head factors W = L_S^-1 (column-major, zero padded, 32 KB each) and
 // the subset's inputs are staged ONCE per CTA in shared memory by TMA bulk copies (read from
@@ -647,6 +1010,15 @@ SLB_DEV void head_group_bound(const slb_sweep& cfg, const filter_args& a, int64_
     head_mark(a, HM_BOUND);
 }
 
+// an entry of the factored grid kernel with finite bounds carries an fp64-class mean: the head stage
+// decides it from its box, or sends it to the refine pass, without recomputing the mean
+SLB_DEV bool fp64_class_entry(const filter_args& a, const filter_side& t, int D) {
+    if (!a.grid_means) return false;
+    bool finite = true;
+    for (int j = 0; j < D; ++j) finite &= t.dm[j] < __longlong_as_double(0x7ff0000000000000ll);
+    return finite;
+}
+
 // every copy lands in this CTA's shared memory before the CTA may leave
 SLB_DEV void head_wait_landings(uint64_t* bar) {
     for (int b = 0; b < 3; ++b) slb_bulk::mbar_wait(bar + b, 0);
@@ -685,6 +1057,9 @@ filter_head_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
     const int nf = cfg.gp.num_factors;
     double* xbuf = wbuf + (size_t)a.head_factors_staged * HR * HR;     // [staged][HR * DIN]
     double* mbuf = xbuf + (size_t)a.head_factors_staged * HR * DIN;    // screened: [Xf | gamma_f ...] per factor
+    // fp64 means are recomputed here only for entries without an fp64-class one (all of them after the
+    // fp32 screening kernel, those the grid kernel left with dm = inf: counts[2])
+    const bool means = a.screened && (!a.grid_means || a.counts[2] != 0);
     if (threadIdx.x == 0) {
         for (int b = 0; b < 3; ++b) slb_bulk::mbar_init(bar + b, 1);
         slb_bulk::fence_barrier_init();
@@ -706,8 +1081,8 @@ filter_head_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
             if (cfg.gp.factors[f].head_rows > 0)
                 slb_bulk::copy_g2s(wbuf + (size_t)f * HR * HR, cfg.gp.factors[f].Wheadp,
                                    HR * HR * sizeof(double), bar + 1);
-        slb_bulk::mbar_arrive_expect_tx(bar + 2, a.screened ? (unsigned)a.mean_doubles * sizeof(double) : 0u);
-        if (a.screened) {
+        slb_bulk::mbar_arrive_expect_tx(bar + 2, means ? (unsigned)a.mean_doubles * sizeof(double) : 0u);
+        if (means) {
             for (int f = 0; f < nf; ++f) {
                 const slb_gp_factor& F = cfg.gp.factors[f];
                 const int Mp = padded_rows(F.M);
@@ -781,7 +1156,7 @@ filter_head_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
             const int ngr = (int)min((int64_t)HW, (ngroups - grp0 + gridDim.x - 1) / gridDim.x);
             const int npairs = ngr * nf;
             const int nbw = min(npairs, HW);
-            const bool early_means = a.screened && nbw < HW;
+            const bool early_means = means && nbw < HW;
             if (warp < nbw) {
                 slb_bulk::mbar_wait(bar + 0, 0);
                 head_mark(a, HM_TABLES);
@@ -811,7 +1186,7 @@ filter_head_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
                 head_mark(a, HM_MEANS);
             }
             __syncthreads();
-            if (a.screened && !early_means) {             // no warp to spare: the means after the bounds
+            if (means && !early_means) {                  // no warp to spare: the means after the bounds
                 slb_bulk::mbar_wait(bar + 0, 0);
                 slb_bulk::mbar_wait(bar + 2, 0);
                 head_round_means<DIN>(cfg, a, nullptr, ngr * HP, grp0, count, mbuf, tab512, mu_s, merr_s, 0, HT);
@@ -839,7 +1214,7 @@ filter_head_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
                     t.guard += screening_slack(cfg, mu, dm, shi);
                     outcome = mine ? decide(t, shi, cfg.gp.num_outputs) : 0;
                     head_mark(a, HM_SCREENED);
-                    if (mine && outcome < 0) {
+                    if (mine && outcome < 0 && !fp64_class_entry(a, t, cfg.gp.num_outputs)) {
                         double merr[SLB_MAX_OUT];
                         for (int j = 0; j < SLB_MAX_OUT; ++j) {
                             mu[j] = mu_s[slot * SLB_MAX_OUT + j];
@@ -883,7 +1258,7 @@ filter_head_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
                     mean_decision_terms(cfg, t, vx, mu, zero);
                     t.guard += screening_slack(cfg, mu, dm, shi);
                     outcome = mine ? decide(t, shi, cfg.gp.num_outputs) : 0;
-                    need = mine && outcome < 0;
+                    need = mine && outcome < 0 && !fp64_class_entry(a, t, cfg.gp.num_outputs);
                     if (need) need_s[2 + atomicAdd(need_s + (round & 1), 1)] = warp * HP + lane;
                     head_mark(a, HM_SCREENED);
                 } else {
@@ -931,7 +1306,8 @@ double* g_probe_dm = nullptr;
 unsigned long long* g_head_timing = nullptr;   // slb_debug_head_timing
 int g_filter_stages = 3;               // slb_debug_filter_stages: bit 0 head stage, bit 1 refine pass,
                                        // bit 2 forces the fp64 mean stage (no fp32 screening), bit 3 /
-                                       // bit 4 force the head stage's split schedule / round loop
+                                       // bit 4 force the head stage's split schedule / round loop,
+                                       // bit 5 the fp32 screening kernel where the grid kernel would run
 
 // The fp32 screening kernel needs closed-form bounds of V and L_V over a box of means
 // (screening_slack): plain RBF factors, V = QUADRATIC (optional scale) on the GP outputs, L_V constant
@@ -950,6 +1326,17 @@ bool screening_applicable(const slb_sweep& cfg) {
     if (L.flags & ~(uint32_t)(SLB_FLAG_ABS | SLB_FLAG_NORM1 | SLB_FLAG_SCALE)) return false;
     if (L.out_dim > 4) return false;
     return (L.flags & SLB_FLAG_NORM1) || L.out_dim == 1 || L.out_dim == D;
+}
+
+// The factored grid kernel replaces the fp32 screening kernel (same list A layout) where kernel values
+// factor over the grid axes: a 2-D grid, z = [x0, x1, u] with plain RBF factors (screening_applicable)
+// and u = a x0 + b x1, optionally saturated and scaled.
+bool grid_mean_applicable(const slb_sweep& cfg) {
+    if (g_filter_stages & 32) return false;
+    const slb_function& P = cfg.policy;
+    return screening_applicable(cfg) && cfg.grid.ndim == 2 && cfg.gp.input_dim == 3 &&
+           P.kind == SLB_FN_LINEAR && P.in_dim == 2 && P.out_dim == 1 && P.matrix != nullptr &&
+           !(P.flags & ~(uint32_t)(SLB_FLAG_SATURATE | SLB_FLAG_SCALE));
 }
 
 // Shared-memory plan of the head stage (one CTA per SM): which factors' head tables are staged, and --
@@ -982,6 +1369,7 @@ void head_layout(const slb_sweep& cfg, int din, filter_args& ah, size_t& head_sm
             head_smem += extra;
         }
     }
+    ah.grid_means = ah.screened && grid_mean_applicable(cfg) ? 1 : 0;
 }
 
 template <int DIN>
@@ -996,6 +1384,10 @@ int launch_filter(cudaStream_t st, const slb_sweep& cfg, const filter_args& a, s
                                       cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
         SLB_CUDA(cudaFuncSetAttribute(filter_head_kernel<DIN>,
                                       cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        if constexpr (DIN == 3)
+            SLB_CUDA(cudaFuncSetAttribute(filter_grid_mean_kernel<DIN>,
+                                          cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                          (int)grid_mean_smem_bytes()));
         if (device >= 0 && device < 64) configured[device].store(true, std::memory_order_release);
     }
     const int64_t blocks = (a.n + FT - 1) / FT;
@@ -1005,7 +1397,15 @@ int launch_filter(cudaStream_t st, const slb_sweep& cfg, const filter_args& a, s
     ah.probe_mu = g_probe_mu;
     ah.probe_dm = g_probe_dm;
     ah.timing = g_head_timing;
-    if (ah.screened) {
+    if (ah.grid_means) {                          // d_in = 3 (grid_mean_applicable)
+        if constexpr (DIN == 3) {
+            // tiles of GR rows x GC columns over the rows the range touches (it may start and end mid-row)
+            const int64_t n1 = cfg.grid.num_points[1];
+            const int64_t r0 = a.idx_begin / n1, r1 = (a.idx_begin + a.n - 1) / n1;
+            const int64_t tiles = ((r1 - r0) / GR + 1) * ((n1 + GC - 1) / GC);
+            filter_grid_mean_kernel<DIN><<<(unsigned)tiles, GT, grid_mean_smem_bytes(), st>>>(cfg, ah);
+        }
+    } else if (ah.screened) {
         const size_t smem32 = mean32_smem_bytes(DIN, a.max_outputs_per_factor, a.chunk_rows, FT / 32);
         filter_mean32_kernel<DIN><<<(unsigned)blocks, FT, smem32, st>>>(cfg, ah);
     } else {
@@ -1041,6 +1441,15 @@ int slb_filter_stage1(const slb_sweep* cfg) {
     size_t smem = 0;
     head_layout(*cfg, cfg->gp.input_dim, a, smem);
     return a.screened ? 32 : 64;
+}
+
+int slb_filter_mean_scheme(const slb_sweep* cfg) {
+    if (cfg == nullptr || cfg->gp.num_outputs <= 0) return SLB_MEAN_NONE;
+    filter_args a;
+    memset(&a, 0, sizeof(a));
+    size_t smem = 0;
+    head_layout(*cfg, cfg->gp.input_dim, a, smem);
+    return a.grid_means ? SLB_MEAN_GRID_FACTORED : a.screened ? SLB_MEAN_FP32_SCREENED : SLB_MEAN_FP64;
 }
 
 int slb_debug_screening_probe(double* mu_dev, double* dm_dev) {
