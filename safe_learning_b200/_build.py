@@ -22,7 +22,8 @@ HEADER = os.path.join(HERE, "..", "include", "slb200.h")
 UNITS = [("gp_tile_%d_%d.o" % (d, tp), "gp_tile_inst.cu", ["-DSLB_TILE_DIN=%d" % d, "-DSLB_TP=%d" % tp],
           ["gp_tile.cuh", "gp_args.h"]) for d in range(1, 7) for tp in (64, 32)]
 UNITS += [("gp_sweep.o", "gp_sweep.cu", [], ["gp_args.h"]),
-          ("filter.o", "filter.cu", [], ["bulk_copy.cuh", "exp2_tab512.cuh", "gp_mean_staged.cuh", "gp_args.h"]),
+          ("filter.o", "filter.cu", [], ["bulk_copy.cuh", "exp2_tab512.cuh", "gp_mean_staged.cuh", "gp_mean_grid.cuh",
+                                         "gp_args.h"]),
           ("light.o", "light.cu", [], ["bulk_copy.cuh", "exp2_tab512.cuh", "gp_mean_staged.cuh", "bellman.cuh"]),
           ("bellman_tile.o", "bellman_tile.cu", [], []),
           ("rollout.o", "rollout.cu", [], []),

@@ -5,14 +5,28 @@
 // and all of its cost is sigma_j = sqrt(k** - |L^-1 k|^2): M^2 flops per point and Cholesky factor,
 // against M for the mean mu = k . (L^-T alpha).  But the comparison is monotone in every sigma_j, and
 //     0 <= sigma_j <= sigma_j given ANY subset of the training set <= prior sigma_j.  So:
-//   stage 1  (filter_mean_kernel, thread per point) the posterior mean from all M kernel values
-//            (one exp each -- the cost of a Bellman sweep), V(mu), L_V(mu); decide every point
-//            whose outcome is the same for sigma = 0 and the prior sigma; the rest is compacted
-//            into list A with its terms;
-//   stage 2  (filter_head_kernel, warp per point of list A) the posterior variance given a HEAD
-//            SUBSET of at most SLB_HEAD_RANK training points (chosen by the host in pivoted-
-//            Cholesky order, its own small factor: slb_gp_factor.Whead / Xhead); decide with
-//            the tighter bound;
+//   stage 1  the posterior mean mu of every grid point, V(mu), L_V(mu); decide every point whose outcome
+//            is the same for sigma = 0 and the prior sigma; the rest is compacted into list A.  One of
+//            three mean schemes per sweep (stage1_plan):
+//              SLB_MEAN_FP64  (filter_mean_kernel, thread per point) all M kernel values in fp64, one
+//                exp each -- the cost of a Bellman sweep (gp_mean_staged.cuh).  Runs whenever the other
+//                two cannot: covariance expressions, a V or L_V without a closed-form bound over a box
+//                of means (screening_applicable), head tables that do not fit in shared memory.  Its
+//                list A entries are complete: every term of the comparison (filter_side);
+//              SLB_MEAN_FP32_SCREENED  (filter_mean32_kernel, thread per point) the fp32 mean of
+//                gp_mean_staged.cuh with its certified bound dm;
+//              SLB_MEAN_GRID_FACTORED  (filter_grid_mean_kernel, CTA per 16 x 16 tile) the factored fp64
+//                mean of gp_mean_grid.cuh with its fp64-class bound: 2-D grids, z = [x0, x1, u], a linear
+//                policy (grid_mean_applicable).
+//              The last two decide a point when the outcome is the same over the whole box mu +- dm
+//              (screened_outcome) and leave list A entries in the screened layout: z, threshold, V(x) in
+//              dec0, the screened mean in coef and its bound in dm;
+//   stage 2  (filter_head_kernel, one CTA per SM, a warp per 8 entries of list A) the posterior variance
+//            given a HEAD SUBSET of at most SLB_HEAD_RANK training points (chosen by the host in pivoted-
+//            Cholesky order, its own small factor: slb_gp_factor.Wheadp / Xhead); decide with the
+//            tighter bound -- screened entries first over their box, then, unless their mean is
+//            fp64-class already, with the mean recomputed in fp64 by the whole CTA (head_round_means).
+//            Two schedules: a warp per group, or per (group, factor) pair when the list is short;
 //   rest     compacted into list B for the full fp64 posterior (gp_tile_kernel, gp_sweep.cu).
 // Certification.  A point is only decided when the outcome holds with a guard band that covers
 // (a) 1e-6 relative to the magnitudes involved (five orders above the rounding differences between
@@ -33,6 +47,7 @@
 #include <string.h>
 
 #include "gp_mean_staged.cuh"
+#include "gp_mean_grid.cuh"
 #include "gp_args.h"
 
 namespace {
@@ -40,7 +55,9 @@ namespace {
 constexpr int FT = 64;                 // stage 1: threads per CTA = points per CTA (1024 CTAs at
                                        // 256 x 256, 7 resident per SM)
 constexpr int HR = SLB_HEAD_RANK;
-constexpr int HT = 512;                // stage 2: threads per CTA (16 warps, 8 or 2 list entries each)
+constexpr int HT = 512;                // stage 2: threads per CTA
+constexpr int HW = HT / 32;            // ... its 16 warps
+constexpr int HP = 8;                  // ... list entries per warp and round: the n dimension of a DMMA
 constexpr int HEAD_CTAS = SLB_NUM_SMS;  // one CTA per SM (it stages the head factors in shared memory)
 constexpr int64_t CHUNK = 1 << 22;     // points per pass of the three stages (bounds the workspace)
 constexpr int64_t WS_HEAD = 64 + SLB_SPLIT_TICKET_BYTES + (int64_t)SLB_SPLIT_PARTIAL_BYTES;   // bytes before the lists
@@ -51,6 +68,28 @@ struct filter_side { double dec0, thr, guard, coef[SLB_MAX_OUT], z[SLB_MAX_IN], 
 // fp32 screening stage: dec0 = V(x), coef[j] = screened mean of output j, dm[j] = its certified bound
 // (the head stage rebuilds the mean-dependent terms from them, and from an fp64 mean where needed)
 
+// What stage1_plan decides for a sweep: the mean scheme of stage 1 (which fixes the layout of list A) and
+// the shared memory of a head CTA, as offsets in doubles from its base.  [0, 4) there: three mbarriers
+// and the CTA's two counters.
+struct filter_plan {
+    int mean_scheme;                   // SLB_MEAN_*.  FP64: list A entries are complete.  The other two:
+                                       // the screened layout; GRID_FACTORED: an entry whose bounds dm are
+                                       // all finite carries an fp64-class mean (no recompute), counts[2]
+                                       // is the number of the other entries
+    int factors_staged;                // factors whose head tables fit in shared memory (the others are
+                                       // read from global memory)
+    int mean_off[SLB_MAX_OUT];         // screened: offset of factor f's [Xf | gamma_f ...] block in mbuf
+    int mean_doubles;                  // screened: size of mbuf
+    int tabs;                          // [512] of exp_neg_fast, [64] of exp_neg_tab: one landing
+    int kbuf;                          // [HW][HR][HP] kernel values of a warp's group
+    int sd;                            // split schedule: [HW * HP][SLB_MAX_OUT] sigma by entry and factor
+    int wbuf, xbuf;                    // [staged][HR * HR] packed head factors, [staged][HR * d_in] inputs
+    int mbuf, mu, merr;                // screened: the mean tables, [HW * HP][SLB_MAX_OUT] fp64 means of a
+                                       // round's entries and their error bounds
+    int need;                          // screened: ints, [2] counters (round parity) then the slots to recompute
+    int doubles;                       // all of it: the CTA's dynamic shared memory
+};
+
 struct filter_args {
     int64_t n;
     int64_t idx_begin;
@@ -59,26 +98,16 @@ struct filter_args {
     int64_t* list_a;                   // undecided after stage 1 (index relative to the range)
     filter_side* side_a;               // their terms, same order
     int64_t* list_b;                   // undecided after stage 2 -> full posterior
-    unsigned long long* counts;        // [0] entries of list_a, [1] entries of list_b
+    unsigned long long* counts;        // [0] entries of list_a, [1] entries of list_b, [2] see filter_plan
     unsigned long long* stats;         // nullptr or [4], see slb200.h
     int chunk_rows;                    // training rows per staged slice (multiple of 8)
     int max_outputs_per_factor;
-    int head_factors_staged;           // head stage: factors whose tables fit in shared memory (the
-                                       // others are read from global memory)
-    int screened;                      // stage 1 was the fp32 screening kernel: list A entries carry only
-                                       // z, threshold and V(x) (in dec0); the head stage computes the
-                                       // fp64 mean and the terms that depend on it
-    int mean_off[SLB_MAX_OUT];         // screened: offset (doubles) of factor f's [Xf | gamma_f ...] block
-                                       // in the head stage's shared-memory copy
-    int mean_doubles;                  // screened: size of that copy
+    filter_plan plan;
     int prefetch_factors;              // head stage: warm L2 with the packed factors for the refine pass
     double* probe_mu;                  // slb_debug_screening_probe: nullptr or [n, D] screened means ...
     double* probe_dm;                  // ... and their certified error bounds (inf: point left to fp64)
     unsigned long long* timing;        // slb_debug_head_timing: nullptr or [HEAD_CTAS + 1][8] %globaltimer
     int head_schedule;                 // head stage: 0 chosen from the list length, 1 split, 2 round loop
-    int grid_means;                    // stage 1 was the factored grid kernel: a list A entry whose bounds
-                                       // dm are all finite carries an fp64-class mean (no recompute);
-                                       // counts[2] is the number of the other entries
 };
 
 // slb_debug_head_timing: timing[slot] = the latest %globaltimer (ns) at which a warp passed a mark.
@@ -207,6 +236,92 @@ SLB_DEV double screening_slack(const slb_sweep& cfg, const double* mu, const dou
     return 1.000001 * (dv + dl);
 }
 
+// the comparison over the box mu +- dm and every sigma_j in [0, shi_j]: fills t's mean-dependent terms
+SLB_DEV int screened_outcome(const slb_sweep& cfg, filter_side& t, double vx, const double* mu,
+                             const double* dm, const double* shi) {
+    double zero[SLB_MAX_OUT];
+    for (int j = 0; j < SLB_MAX_OUT; ++j) zero[j] = 0.0;
+    mean_decision_terms(cfg, t, vx, mu, zero);
+    t.guard += screening_slack(cfg, mu, dm, shi);
+    return decide(t, shi, cfg.gp.num_outputs);
+}
+
+// ---- stage 1: what its three kernels share -----------------------------------------------------------
+// x of a grid point, V(x), threshold(x), u = policy(x), z = [x, u]          (lyapunov.py:436, 284-288).
+// Returns whether z is sane: the expanded squared distance needs moderate magnitudes; NaN / huge inputs
+// go to the full path.
+template <int DIN>
+SLB_DEV bool stage1_point(const slb_sweep& cfg, int64_t index, double* z, double* vx, double* thr) {
+    grid_index_to_state(cfg.grid, index, z);
+    lyapunov_state_terms(cfg, z, index, vx, thr);
+    double u[SLB_MAX_OUT];
+    const int m = eval_fn_small(cfg.policy, z, u);
+    for (int c = 0; c < m; ++c) z[cfg.grid.ndim + c] = u[c];
+    bool sane = true;
+#pragma unroll
+    for (int c = 0; c < DIN; ++c) sane &= fabs(z[c]) < 1e100;
+    return sane;
+}
+
+// sigma_j <= prior sigma_j at z, for every output     (functions.py:450 without data)
+template <int DIN>
+SLB_DEV void prior_sigma_bound(const slb_gp_stack& gp, const double* z, double* shi) {
+    for (int j = 0; j < gp.num_outputs; ++j) {
+        const slb_gp_factor& F = gp.factors[gp.outputs[j].factor];
+        shi[j] = sqrt(F.kernel.num_prims > 0 ? kernel_expr_diag<DIN>(F.kernel, z) : F.variance);
+    }
+}
+
+// a point leaves stage 1: its flag and V(x); an undecided one is appended to list A (returns its slot,
+// -1 otherwise: the caller writes the entry's terms)
+SLB_DEV long long stage1_finish(const filter_args& a, bool valid, int64_t rel, int outcome, double vx) {
+    const bool undecided = valid && outcome < 0;
+    if (valid) {
+        a.negative[rel] = outcome > 0 ? 1 : 0;
+        if (a.values != nullptr) a.values[rel] = vx;
+    }
+    const long long slot = list_append(undecided, a.counts + 0);
+    if (undecided) a.list_a[slot] = rel;
+    if (a.stats != nullptr) {
+        count_stat(valid && !undecided, a.stats + 0);
+        count_stat(valid, a.stats + 3);
+    }
+    return slot;
+}
+
+// ... from a screened kernel (t: the point's z and threshold), with its mean mu and certified bound dm: the
+// comparison over the box and the prior sigma, the list A entry in the screened layout (the head stage
+// rebuilds the mean-dependent terms), the probe
+template <int DIN>
+SLB_DEV void stage1_screened_finish(const slb_sweep& cfg, const filter_args& a, bool valid, bool sane,
+                                    int64_t rel, filter_side& t, double vx, const double* mu, const double* dm) {
+    const int D = cfg.gp.num_outputs;
+    if (a.probe_mu != nullptr && valid) {
+        for (int o = 0; o < D; ++o) {
+            a.probe_mu[rel * D + o] = mu[o];
+            a.probe_dm[rel * D + o] = sane ? dm[o] : f64_inf();
+        }
+    }
+    double shi[SLB_MAX_OUT];
+    prior_sigma_bound<DIN>(cfg.gp, t.z, shi);
+    const int screened = screened_outcome(cfg, t, vx, mu, dm, shi);
+    const long long slot = stage1_finish(a, valid, rel, sane ? screened : -1, vx);
+    bool fp64 = sane;                             // every bound finite: an fp64-class mean
+    for (int j = 0; j < D; ++j) fp64 &= dm[j] < f64_inf();
+    if (slot >= 0) {
+        filter_side* dst = a.side_a + slot;
+        dst->dec0 = vx;
+        dst->thr = t.thr;
+#pragma unroll
+        for (int c = 0; c < DIN; ++c) dst->z[c] = t.z[c];
+        for (int j = 0; j < D; ++j) {
+            dst->coef[j] = mu[j];
+            dst->dm[j] = sane ? dm[j] : f64_inf();
+        }
+    }
+    if (a.plan.mean_scheme == SLB_MEAN_GRID_FACTORED) count_stat(slot >= 0 && !fp64, a.counts + 2);
+}
+
 template <int DIN>
 __global__ void __launch_bounds__(FT, 7)
 filter_mean_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
@@ -223,23 +338,9 @@ filter_mean_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
     const int64_t rel0 = (int64_t)blockIdx.x * FT + threadIdx.x;
     const bool valid = rel0 < a.n;
     const int64_t rel = valid ? rel0 : a.n - 1;   // every thread stays for the block barriers
-    const int d = cfg.grid.ndim;
-    const int D = cfg.gp.num_outputs;
-
-    // ---- x, V(x), threshold(x), u = policy(x)           (lyapunov.py:436, 284-288)
     filter_side t;
-    grid_index_to_state(cfg.grid, a.idx_begin + rel, t.z);
     double vx;
-    lyapunov_state_terms(cfg, t.z, a.idx_begin + rel, &vx, &t.thr);
-    {
-        double u[SLB_MAX_OUT];
-        const int m = eval_fn_small(cfg.policy, t.z, u);
-        for (int c = 0; c < m; ++c) t.z[d + c] = u[c];
-    }
-    // the expanded squared distance needs moderate magnitudes; NaN / huge inputs -> full path
-    bool sane = true;
-#pragma unroll
-    for (int c = 0; c < DIN; ++c) sane &= fabs(t.z[c]) < 1e100;
+    const bool sane = stage1_point<DIN>(cfg, a.idx_begin + rel, t.z, &vx, &t.thr);
 
     // ---- posterior mean of every output (functions.py:439-442 as k . L^-T alpha)
     slb_bulk::mbar_wait(bar + 2, 0);              // exp tables have landed
@@ -249,24 +350,10 @@ filter_mean_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
 
     mean_decision_terms(cfg, t, vx, mu, mean_err);
 
-    // ---- sigma_j <= prior sigma_j     (functions.py:450 without data)
     double shi[SLB_MAX_OUT];
-    for (int j = 0; j < D; ++j) {
-        const slb_gp_factor& F = cfg.gp.factors[cfg.gp.outputs[j].factor];
-        shi[j] = sqrt(F.kernel.num_prims > 0 ? kernel_expr_diag<DIN>(F.kernel, t.z) : F.variance);
-    }
-    const int outcome = sane ? decide(t, shi, D) : -1;
-    const bool undecided = valid && outcome < 0;
-    if (valid) {
-        a.negative[rel] = outcome > 0 ? 1 : 0;
-        if (a.values != nullptr) a.values[rel] = vx;
-    }
-    const long long slot = list_append(undecided, a.counts + 0);
-    if (undecided) { a.list_a[slot] = rel; a.side_a[slot] = t; }
-    if (a.stats != nullptr) {
-        count_stat(valid && !undecided, a.stats + 0);
-        count_stat(valid, a.stats + 3);
-    }
+    prior_sigma_bound<DIN>(cfg.gp, t.z, shi);
+    const long long slot = stage1_finish(a, valid, rel, sane ? decide(t, shi, cfg.gp.num_outputs) : -1, vx);
+    if (slot >= 0) a.side_a[slot] = t;
     timing_mark(a, HEAD_CTAS * 8);
 }
 
@@ -283,46 +370,19 @@ filter_mean32_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a)
     extern __shared__ __align__(16) unsigned char smem_raw[];
     __shared__ double s_cen[SLB_MAX_IN];
     prefetch_descriptor_operands(cfg);
-    constexpr int W32 = row32<DIN>::W;
     mean_pipe P;
-    P.bar = reinterpret_cast<uint64_t*>(smem_raw);
-    P.C = a.chunk_rows;
-    P.xstride = P.C * (DIN + 1);
-    P.gstride = P.C * a.max_outputs_per_factor;
-    P.xbuf = reinterpret_cast<double*>(smem_raw + 32);
-    P.gbuf = P.xbuf + 2 * P.xstride;
-    P.t = 0;
     mean32_bufs B;
-    B.red = P.gbuf + 2 * P.gstride;
-    B.xf = reinterpret_cast<float*>(B.red + 8 * (FT / 32) + 8);
-    B.g = B.xf + P.C * W32;
-    if (threadIdx.x == 0) {
-        slb_bulk::mbar_init(P.bar + 0, 1);
-        slb_bulk::mbar_init(P.bar + 1, 1);
-        slb_bulk::fence_barrier_init();
-        slb_bulk::fence_proxy_async();
-    }
+    mean32_bufs_setup<DIN>(B, mean_pipe_setup(P, smem_raw, DIN, a.chunk_rows, a.max_outputs_per_factor, cfg.gp,
+                                              nullptr, nullptr), a.chunk_rows, FT / 32);
+    if (threadIdx.x == 0) mean_pipe_init(P, nullptr);
     mean_pipe_start<DIN>(cfg.gp, P);                                   // slice 0 -> buffer 0
 
     const int64_t rel0 = (int64_t)blockIdx.x * FT + threadIdx.x;
     const bool valid = rel0 < a.n;
     const int64_t rel = valid ? rel0 : a.n - 1;   // every thread stays for the block barriers
-    const int d = cfg.grid.ndim;
-    const int D = cfg.gp.num_outputs;
-
-    // ---- x, V(x), threshold(x), u = policy(x)           (lyapunov.py:436, 284-288)
     filter_side t;
-    grid_index_to_state(cfg.grid, a.idx_begin + rel, t.z);
     double vx;
-    lyapunov_state_terms(cfg, t.z, a.idx_begin + rel, &vx, &t.thr);
-    {
-        double u[SLB_MAX_OUT];
-        const int m = eval_fn_small(cfg.policy, t.z, u);
-        for (int c = 0; c < m; ++c) t.z[d + c] = u[c];
-    }
-    bool sane = true;
-#pragma unroll
-    for (int c = 0; c < DIN; ++c) sane &= fabs(t.z[c]) < 1e100;
+    bool sane = stage1_point<DIN>(cfg, a.idx_begin + rel, t.z, &vx, &t.thr);
     // the CTA's centre: the query point of its middle thread
     if (threadIdx.x == FT / 2) {
 #pragma unroll
@@ -335,279 +395,11 @@ filter_mean32_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a)
 
     double mu[SLB_MAX_OUT], dm[SLB_MAX_OUT];
     gp_mean32_staged<DIN>(cfg.gp, t.z, zcen, mu, dm, sane, P, B);
-    if (a.probe_mu != nullptr && valid) {
-        for (int o = 0; o < D; ++o) {
-            a.probe_mu[rel * D + o] = mu[o];
-            a.probe_dm[rel * D + o] = sane ? dm[o] : __longlong_as_double(0x7ff0000000000000ll);
-        }
-    }
-
-    // ---- the comparison over mu +- dm and sigma_j in [0, prior sigma_j]
-    double zero[SLB_MAX_OUT];
-    for (int j = 0; j < SLB_MAX_OUT; ++j) zero[j] = 0.0;
-    mean_decision_terms(cfg, t, vx, mu, zero);
-    double shi[SLB_MAX_OUT];
-    for (int j = 0; j < D; ++j) shi[j] = sqrt(cfg.gp.factors[cfg.gp.outputs[j].factor].variance);
-    t.guard += screening_slack(cfg, mu, dm, shi);
-    const int outcome = sane ? decide(t, shi, D) : -1;
-    const bool undecided = valid && outcome < 0;
-    if (valid) {
-        a.negative[rel] = outcome > 0 ? 1 : 0;
-        if (a.values != nullptr) a.values[rel] = vx;
-    }
-    const long long slot = list_append(undecided, a.counts + 0);
-    if (undecided) {
-        filter_side* dst = a.side_a + slot;
-        dst->dec0 = vx;                           // the head stage rebuilds the mean-dependent terms
-        dst->thr = t.thr;
-#pragma unroll
-        for (int c = 0; c < DIN; ++c) dst->z[c] = t.z[c];
-        for (int j = 0; j < D; ++j) {
-            dst->coef[j] = mu[j];
-            dst->dm[j] = sane ? dm[j] : __longlong_as_double(0x7ff0000000000000ll);
-        }
-        a.list_a[slot] = rel;
-    }
-    if (a.stats != nullptr) {
-        count_stat(valid && !undecided, a.stats + 0);
-        count_stat(valid, a.stats + 3);
-    }
+    stage1_screened_finish<DIN>(cfg, a, valid, sane, rel, t, vx, mu, dm);
     timing_mark(a, HEAD_CTAS * 8);
 }
 
-// ---- stage 1, factored grid mean ----------------------------------------------------------------------
-// On a 2-D grid with plain RBF factors on z = [x0, x1, u] and the policy u = clip(a x0 + b x1, lo, hi)
-// (a LINEAR map, optionally saturated and scaled), the kernel values of a tile of grid points factor
-// into per-axis tables and the mean of the tile is a small matrix product on the fp64 tensor pipe.
-// In a factor's units (w = z / l; xs_j the staged training rows) and on a region where the policy is
-// affine, w2 = alpha w0 + beta w1 + const (alpha = a' l0 / l2, beta = b' l1 / l2, a' b' the scaled
-// row; alpha = beta = 0 where u is saturated, a constant).  Centre the tile at cw (cw2 the affine value
-// there), xi = w0 - cw0, eta = w1 - cw1, D_j = cw - xs_j; the exponent -|w - xs_j|^2 / 2 expands to
-//     -|D_j|^2 / 2  -  xi p_j  -  eta q_j  -  (xi^2 + eta^2 + (alpha xi + beta eta)^2) / 2,
-//     p_j = D_j0 + alpha D_j2,  q_j = D_j1 + beta D_j2,
-// so  mean_o[i, k] = Q[i, k] sum_j (gamma_oj exp(-|D_j|^2 / 2) E0[i, j]) E1[k, j],
-//     E0[i, j] = exp(-xi_i p_j),  E1[k, j] = exp(-eta_k q_j),  Q = exp(-(...) / 2) <= 1:
-// The tables run on the uniform offsets xi_i = (i - 8) h0, h0 = unit0 / l0 (eta likewise): a column of
-// E0 is g^(i - 8), g = exp(-h0 p_j), from two exponentials and 15 products -- 5 M exponentials per tile
-// and regime (two per table column, one weight) instead of GR GC M -- and GR GC M fp64 FMAs in DMMA
-// m8n8k4 (warp w: the 8 x 8 block (w / GCB, w % GCB) of the tile; its C fragment is its lanes' points).
-// A tile computes every regime its points are in (saturated low / high, affine), each point keeps its
-// own.  The summation order is fixed: two runs are bit-identical.
-// Certified bound (u = 2^-53, rho = max|xi| sqrt(1 + alpha^2) + max|eta| sqrt(1 + beta^2) >= |w - cw|,
-// s_j = |D_j|, Sg = gamma_l1 >= sum_j |gamma_oj|):
-//   each term: the weight and Q from one exp_neg_fast each (EPS_K relative; its reduction x = n ln2 / 512
-//     + r is the same for positive arguments, |x| <= 294 here), each table entry a power |o| <= 8 of one
-//     (8 (EPS_K + 2 u)), three products; arguments from D (one rounding each), K, p, q (fma chains), h p
-//     and xi = fl(o h): relative error <= 18 EPS_K + u (3.5 (s_j + rho)^2 + 43) of the exact k_j;
-//     k_j <= exp(-max(s_j - rho, 0)^2 / 2), so its contribution is <= (18 EPS_K + u (3.5 (sqrt(rho^2 + 2)
-//     + rho)^2 + 43)) |gamma_j|;
-//   the M-term sum (two DMMA chains): <= (Mp + 4) u sum_j |gamma_j| k_j (the tables' product exceeds k_j
-//     by 1 / Q, the final product with Q takes it back);
-//   the point itself: the grid's w0 = fl(x0 / l0) is within dev (computed, + 2 u |xi|) of cw0 + xi (w1
-//     likewise; on the affine region w2 moves by |alpha| dev + |beta| dev with them); the policy's
-//     fl(fl(x0 a) + fl(x1 b)) scaled, alpha, beta and cw2 are within 10 u (|alpha| W0 + |beta| W1) of
-//     the affine w2 (W = max |w| over the tile); |d k_j / d w_c| <= 1, so each enters times sum |gamma|;
-//   dropped rows (|D_j|^2 > GRID_K_DROP: weight 0): each k_j <= exp(-(sqrt(K_DROP) - rho)^2 / 2);
-//     products that leave the fp64 range downwards: < 1e-150 (Mp + 1) absolute (|table args| <=
-//     rho sqrt(K_DROP) <= 294);
-//   the other evaluation orders of the same mean (gamma itself and the a . alpha form of the full
-//     posterior, its expanded distance): 7e-16 (M + 8) + 4.5e-16 (|w|^2 / 2 + hmax), as mean_output_finish.
-// dm = 1.05 (sum of the above) Sg / |scale|.  A tile and regime with rho > GRID_RHO_MAX or a non-finite
-// constant leaves its points to the fp64 route (dm = inf), like points the prologue finds insane.
-constexpr int GR = 16, GC = 16;        // grid rows (axis 0) x columns (axis 1, contiguous) per CTA tile
-constexpr int GCB = GC / 8;            // column blocks
-constexpr int GT = GR * GC / 2;        // threads: one warp per 8 x 8 block, two points per thread (two CTAs
-                                       // per SM: one's barriers and round trips hide behind the other)
-constexpr int GJ = 128;                // training rows per chunk of the tables
-constexpr int GNO = 4;                 // outputs per factor (screening_applicable: at most 4 outputs)
-constexpr double GRID_RHO_MAX = 12.0;
-constexpr double GRID_K_DROP = 600.0;
-constexpr int GFS = 36;                // doubles per fragment (32 used): the recurrence's column stores hit
-                                       // every bank pair once, the contraction's loads stay contiguous
-constexpr int GTAB = (GR / 8) * (GJ / 4) * GFS;   // one table of a chunk, in fragments
-constexpr int GSMEM_PRE_TAB = 2 * GTAB + GNO * GJ + 2 * GJ + 2 * (GR + GC);   // doubles before the exp table
-static_assert(GR == 16 && GC == 16, "the recurrence runs 8 steps each way from the tile's centre");
-
-inline size_t grid_mean_smem_bytes() {
-    return (size_t)(GSMEM_PRE_TAB + 512) * sizeof(double);
-}
-
-// one factor with NO outputs (compile-time: accumulators in registers) for the tile; writes mu / dm of
-// the thread's two points for the factor's outputs
-template <int NO>
-SLB_DEV void grid_mean_factor(const slb_sweep& cfg, int f, const int* outs, double* smem, const double* tab,
-                              int64_t row0,
-                              int64_t col0, const double (*z)[3], const int* reg, double (*mu)[GNO],
-                              double (*dm)[GNO]) {
-    const slb_gp_factor& F = cfg.gp.factors[f];
-    const slb_grid& g = cfg.grid;
-    const slb_function& pol = cfg.policy;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int rb = warp / GCB, cb = warp % GCB;
-    double* e0f = smem;                        // [GR / 8][J / 4][GFS]: DMMA A fragments
-    double* e1f = e0f + GTAB;                  // [GC / 8][J / 4][GFS]: DMMA B fragments
-    double* wg = e1f + GTAB;                   // [NO][GJ] gamma_oj exp(-|D_j|^2 / 2)
-    double* pq = wg + GNO * GJ;                // [2][GJ]
-    double* xi = pq + 2 * GJ;                  // [GR] xi of the tables: (i - GR / 2) h0
-    double* eta = xi + GR;                     // [GC]
-    double* dev = eta + GC;                    // [GR + GC] |w - cw - xi| of the grid's own points
-    const double l0 = F.lengthscales[0], l1 = F.lengthscales[1], l2 = F.lengthscales[2];
-    // the centre: grid point (GR / 2, GC / 2) of the tile, in the factor's units
-    const double cw0 = f64add(f64mul((double)(row0 + GR / 2), g.unit_maxes[0]), g.offset[0]) / l0;
-    const double cw1 = f64add(f64mul((double)(col0 + GC / 2), g.unit_maxes[1]), g.offset[1]) / l1;
-    __syncthreads();                           // the previous factor is done with the tables
-    // the tables run on the uniform offsets xi_i = (i - GR / 2) h0, h0 = unit / l0 (a recurrence along the
-    // axis); the grid's own points are within dev of them (a perturbation of the point, in the bound)
-    const double h0 = g.unit_maxes[0] / l0, h1 = g.unit_maxes[1] / l1;
-    if (threadIdx.x < GR + GC) {
-        const int c = threadIdx.x < GR ? 0 : 1;
-        const int i = c == 0 ? threadIdx.x : threadIdx.x - GR;
-        const int64_t gi = (c == 0 ? row0 : col0) + i;
-        const double x = f64add(f64mul((double)gi, g.unit_maxes[c]), g.offset[c]);   // grid_index_to_state
-        const double ideal = (double)(i - GR / 2) * (c == 0 ? h0 : h1);
-        xi[threadIdx.x] = ideal;
-        dev[threadIdx.x] = fabs((x / (c == 0 ? l0 : l1) - (c == 0 ? cw0 : cw1)) - ideal);
-    }
-    __syncthreads();
-    double mxi = 0.0, meta = 0.0, pert = 0.0;
-#pragma unroll
-    for (int r = 0; r < GR; ++r) mxi = fmax(mxi, fabs(xi[r]));
-#pragma unroll
-    for (int k = 0; k < GC; ++k) meta = fmax(meta, fabs(eta[k]));
-#pragma unroll
-    for (int k = 0; k < GR + GC; ++k) pert = fmax(pert, dev[k]);
-    const int ti = rb * 8 + (lane >> 2);
-    const int tk0 = cb * 8 + 2 * (lane & 3);
-    const int Mp = padded_rows(F.M);
-    const double u53 = 1.1102230246251565e-16;
-    const double sc = (pol.flags & SLB_FLAG_SCALE) ? pol.out_scale : 1.0;
-    for (int r = 0; r < 3; ++r) {
-        if (!__syncthreads_or(reg[0] == r || reg[1] == r)) continue;
-        double alpha = 0.0, beta = 0.0, cw2;
-        if (r == 2) {
-            alpha = f64mul(f64mul(__ldg(pol.matrix + 0), sc), l0) / l2;
-            beta = f64mul(f64mul(__ldg(pol.matrix + 1), sc), l1) / l2;
-            cw2 = fma(alpha, cw0, f64mul(beta, cw1));
-        } else {
-            const double lim = r == 0 ? pol.lower : pol.upper;
-            cw2 = ((pol.flags & SLB_FLAG_SCALE) ? f64mul(lim, pol.out_scale) : lim) / l2;
-        }
-        const double rho = mxi * sqrt(fma(alpha, alpha, 1.0)) + meta * sqrt(fma(beta, beta, 1.0));
-        const bool ok = rho <= GRID_RHO_MAX && fabs(cw0) < 1e100 && fabs(cw1) < 1e100 && fabs(cw2) < 1e100 &&
-                        fabs(alpha) < 1e100 && fabs(beta) < 1e100;
-        double acc[NO][2][2];
-#pragma unroll
-        for (int q = 0; q < NO; ++q) { acc[q][0][0] = acc[q][0][1] = acc[q][1][0] = acc[q][1][1] = 0.0; }
-        // the thread's training row of a chunk (GT == GJ), loaded one chunk ahead: its L2 round trip runs
-        // behind the previous chunk's tables and contraction
-        static_assert(GT == GJ, "one training row per thread and chunk");
-        double nx[3] = {0.0, 0.0, 0.0}, ng[NO];
-#pragma unroll
-        for (int q = 0; q < NO; ++q) ng[q] = 0.0;
-        if (ok && (int)threadIdx.x < Mp) {
-            const double2 x01 = *reinterpret_cast<const double2*>(F.Xf + (size_t)threadIdx.x * 4);
-            nx[0] = x01.x; nx[1] = x01.y; nx[2] = F.Xf[(size_t)threadIdx.x * 4 + 2];
-#pragma unroll
-            for (int q = 0; q < NO; ++q) ng[q] = cfg.gp.outputs[outs[q]].gamma_f[threadIdx.x];
-        }
-        for (int j0 = 0; ok && j0 < Mp; j0 += GJ) {
-            const int J = min(GJ, Mp - j0), J4 = J >> 2;
-            __syncthreads();                   // the previous chunk's tables are consumed
-            if ((int)threadIdx.x < J) {
-                const double d0 = cw0 - nx[0], d1 = cw1 - nx[1], d2 = cw2 - nx[2];
-                const double K = fma(d0, d0, fma(d1, d1, d2 * d2));
-                const bool keep = K <= GRID_K_DROP;          // dropped rows: weight 0, tables of ones
-                bool far;
-                const double w = keep ? exp_neg_fast(-0.5 * K, tab, far) : 0.0;
-                pq[threadIdx.x] = keep ? fma(alpha, d2, d0) : 0.0;
-                pq[GJ + threadIdx.x] = keep ? fma(beta, d2, d1) : 0.0;
-#pragma unroll
-                for (int q = 0; q < NO; ++q) wg[q * GJ + threadIdx.x] = ng[q] * w;
-            }
-            const int jn = j0 + GJ + (int)threadIdx.x;
-            if (jn < Mp) {
-                const double2 x01 = *reinterpret_cast<const double2*>(F.Xf + (size_t)jn * 4);
-                nx[0] = x01.x; nx[1] = x01.y; nx[2] = F.Xf[(size_t)jn * 4 + 2];
-#pragma unroll
-                for (int q = 0; q < NO; ++q) ng[q] = cfg.gp.outputs[outs[q]].gamma_f[jn];
-            }
-            __syncthreads();
-            // one table column (training row jj, axis c) per task: exp(-o h p) = g^o for the offsets
-            // o = -8 .. 7 from two exps g = exp(-h p), 1 / g = exp(h p) and products outwards from o = 0
-            for (int task = threadIdx.x; task < 2 * J; task += GT) {
-                const int c = task >= J ? 1 : 0, jj = task - c * J;
-                const double t = (c ? h1 : h0) * pq[c * GJ + jj];
-                bool far;
-                const double gd = exp_neg_fast(-t, tab, far), gu = exp_neg_fast(t, tab, far);
-                double* col = (c ? e1f : e0f) + (jj >> 2) * GFS + (jj & 3);   // + block (m / 8) J4 GFS + (m % 8) 4
-                col[J4 * GFS] = 1.0;                                          // m = 8: o = 0
-                double v = 1.0;
-#pragma unroll
-                for (int o = 1; o < 8; ++o) { v *= gd; col[J4 * GFS + o * 4] = v; }      // m = 8 + o
-                v = 1.0;
-#pragma unroll
-                for (int o = 1; o <= 8; ++o) { v *= gu; col[(8 - o) * 4] = v; }          // m = 8 - o
-            }
-            __syncthreads();
-            const double* pa = e0f + rb * J4 * GFS + lane;
-            const double* pb = e1f + cb * J4 * GFS + lane;
-#pragma unroll 2
-            for (int s = 0; s < J4; s += 2) {            // J4 is even (rows padded to 8)
-                double af[2][NO], bf[2];
-#pragma unroll
-                for (int t = 0; t < 2; ++t) {
-                    const double a0 = pa[(s + t) * GFS];
-                    bf[t] = pb[(s + t) * GFS];
-#pragma unroll
-                    for (int q = 0; q < NO; ++q) af[t][q] = a0 * wg[q * GJ + 4 * (s + t) + (lane & 3)];
-                }
-#pragma unroll
-                for (int q = 0; q < NO; ++q) {
-                    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
-                                 : "+d"(acc[q][0][0]), "+d"(acc[q][0][1]) : "d"(af[0][q]), "d"(bf[0]));
-                    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
-                                 : "+d"(acc[q][1][0]), "+d"(acc[q][1][1]) : "d"(af[1][q]), "d"(bf[1]));
-                }
-            }
-        }
-        // the bound of this tile and regime (relative to gamma_l1, see above)
-        const double W0 = fabs(cw0) + mxi, W1 = fabs(cw1) + meta;
-        const double W2 = r == 2 ? fabs(alpha) * W0 + fabs(beta) * W1 : fabs(cw2);
-        const double sq = sqrt(rho * rho + 2.0) + rho, kd = sqrt(GRID_K_DROP) - rho;
-        const double eps = 1.05 * (18.2 * EPS_K + u53 * (1.01 * (3.5 * sq * sq + 43.0) + 1.02 * (Mp + 4)) +
-                                   1.01 * pert * (r == 2 ? 2.0 + fabs(alpha) + fabs(beta) : 2.0) +
-                                   u53 * (2.0 * (mxi + meta) + (r == 2 ? 10.0 * W2 : 2.0 * W2)) +
-                                   4.5e-16 * (0.5 * (W0 * W0 + W1 * W1 + W2 * W2) + F.hmax) + 7e-16 * (F.M + 8) +
-                                   exp(-0.5 * kd * kd));
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            if (reg[h] != r) continue;
-            const double x0 = xi[ti], e1 = eta[tk0 + h];
-            const double v = fma(alpha, x0, beta * e1);
-            bool far;
-            const double Q = exp_neg_fast(-0.5 * fma(x0, x0, fma(e1, e1, v * v)), tab, far);
-#pragma unroll
-            for (int q = 0; q < NO; ++q) {
-                const slb_gp_output& G = cfg.gp.outputs[outs[q]];
-                double mx = 0.0;
-                if (G.prior_mean != nullptr) {
-                    mx = f64mul(z[h][0], G.prior_mean[0]);
-#pragma unroll
-                    for (int c = 1; c < 3; ++c) mx = f64add(mx, f64mul(z[h][c], G.prior_mean[c]));
-                    mx = f64mul(F.scale, mx);
-                }
-                const double m = f64add(f64mul(acc[q][0][h] + acc[q][1][h], Q), mx) / F.scale;
-                const double bound = ok && eps < 1e-3
-                                         ? (eps * G.gamma_l1 + 1e-150 * (Mp + 1)) / fabs(F.scale) + 1e-300
-                                         : __longlong_as_double(0x7ff0000000000000ll);
-#pragma unroll
-                for (int o = 0; o < GNO; ++o)
-                    if (o == outs[q]) { mu[h][o] = m; dm[h][o] = bound; }
-            }
-        }
-    }
-}
-
+// ---- stage 1, factored grid mean (gp_mean_grid.cuh): one CTA per GR x GC tile of a 2-D grid -------------
 template <int DIN>
 __global__ void __launch_bounds__(GT, 2)
 filter_grid_mean_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
@@ -633,7 +425,6 @@ filter_grid_mean_kernel(const __grid_constant__ slb_sweep cfg, const filter_args
     const int64_t ntc = (n1 + GC - 1) / GC;
     const int64_t row0 = a.idx_begin / n1 + (int64_t)(blockIdx.x / ntc) * GR;
     const int64_t col0 = (int64_t)(blockIdx.x % ntc) * GC;
-    const int D = cfg.gp.num_outputs;
     const slb_function& pol = cfg.policy;
 
     // ---- the thread's two points (its lanes' C-fragment positions): x, V(x), threshold(x), u = policy(x)
@@ -651,16 +442,13 @@ filter_grid_mean_kernel(const __grid_constant__ slb_sweep cfg, const filter_args
         valid[h] = gi < n0 && gk < n1 && flat >= a.idx_begin && flat < a.idx_begin + a.n;
         rel[h] = valid[h] ? flat - a.idx_begin : 0;   // every thread stays for the block barriers
         double x[SLB_MAX_IN];
-        grid_index_to_state(cfg.grid, a.idx_begin + rel[h], x);
-        lyapunov_state_terms(cfg, x, a.idx_begin + rel[h], &vx[h], &thr[h]);
-        double u[SLB_MAX_OUT];
-        eval_fn_small(pol, x, u);
-        z[h][0] = x[0]; z[h][1] = x[1]; z[h][2] = u[0];
-        sane[h] = fabs(x[0]) < 1e100 && fabs(x[1]) < 1e100 && fabs(u[0]) < 1e100;
+        sane[h] = stage1_point<DIN>(cfg, a.idx_begin + rel[h], x, &vx[h], &thr[h]);
+#pragma unroll
+        for (int c = 0; c < 3; ++c) z[h][c] = x[c];
         // the regime is the clip the policy computed: saturated points carry the constant itself
         reg[h] = !(valid[h] && sane[h]) ? -1
-                 : (pol.flags & SLB_FLAG_SATURATE) && u[0] == ulo ? 0
-                 : (pol.flags & SLB_FLAG_SATURATE) && u[0] == uhi ? 1 : 2;
+                 : (pol.flags & SLB_FLAG_SATURATE) && z[h][2] == ulo ? 0
+                 : (pol.flags & SLB_FLAG_SATURATE) && z[h][2] == uhi ? 1 : 2;
     }
 
     // ---- posterior means, factor by factor
@@ -668,85 +456,39 @@ filter_grid_mean_kernel(const __grid_constant__ slb_sweep cfg, const filter_args
 #pragma unroll
     for (int h = 0; h < 2; ++h)
 #pragma unroll
-        for (int o = 0; o < GNO; ++o) { mu[h][o] = 0.0; dm[h][o] = __longlong_as_double(0x7ff0000000000000ll); }
-    for (int f = 0; f < cfg.gp.num_factors; ++f) {
-        int outs[SLB_MAX_OUT];
-        int no = 0;
-        for (int o = 0; o < D; ++o)
-            if (cfg.gp.outputs[o].factor == f) outs[no++] = o;
-        switch (no) {
-        case 1: grid_mean_factor<1>(cfg, f, outs, smem, tab, row0, col0, z, reg, mu, dm); break;
-        case 2: grid_mean_factor<2>(cfg, f, outs, smem, tab, row0, col0, z, reg, mu, dm); break;
-        case 3: grid_mean_factor<3>(cfg, f, outs, smem, tab, row0, col0, z, reg, mu, dm); break;
-        case 4: grid_mean_factor<4>(cfg, f, outs, smem, tab, row0, col0, z, reg, mu, dm); break;
-        default: break;
-        }
-    }
+        for (int o = 0; o < GNO; ++o) { mu[h][o] = 0.0; dm[h][o] = f64_inf(); }
+    for (int f = 0; f < cfg.gp.num_factors; ++f)
+        for_outputs_on_factor<GNO>(cfg.gp, f, [&](auto no, const int* outs) {
+            grid_mean_factor<decltype(no)::value>(cfg, f, outs, smem, tab, row0, col0, z, reg, mu, dm);
+        });
 
     // ---- per point: the comparison over mu +- dm and sigma_j in [0, prior sigma_j] (as filter_mean32_kernel)
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-        double m[SLB_MAX_OUT], d[SLB_MAX_OUT], zero[SLB_MAX_OUT];
-        bool fp64 = true;
+        double m[SLB_MAX_OUT], d[SLB_MAX_OUT];
 #pragma unroll
         for (int j = 0; j < SLB_MAX_OUT; ++j) {
             m[j] = j < GNO ? mu[h][j] : 0.0;
             d[j] = j < GNO ? dm[h][j] : 0.0;
-            zero[j] = 0.0;
-            if (j < D) fp64 &= d[j] < __longlong_as_double(0x7ff0000000000000ll);
-        }
-        if (a.probe_mu != nullptr && valid[h]) {
-            for (int o = 0; o < D; ++o) {
-                a.probe_mu[rel[h] * D + o] = m[o];
-                a.probe_dm[rel[h] * D + o] = sane[h] ? d[o] : __longlong_as_double(0x7ff0000000000000ll);
-            }
         }
         filter_side t;
         t.thr = thr[h];
-        mean_decision_terms(cfg, t, vx[h], m, zero);
-        double shi[SLB_MAX_OUT];
-        for (int j = 0; j < D; ++j) shi[j] = sqrt(cfg.gp.factors[cfg.gp.outputs[j].factor].variance);
-        t.guard += screening_slack(cfg, m, d, shi);
-        const int outcome = sane[h] ? decide(t, shi, D) : -1;
-        const bool undecided = valid[h] && outcome < 0;
-        if (valid[h]) {
-            a.negative[rel[h]] = outcome > 0 ? 1 : 0;
-            if (a.values != nullptr) a.values[rel[h]] = vx[h];
-        }
-        const long long slot = list_append(undecided, a.counts + 0);
-        if (undecided) {
-            filter_side* dst = a.side_a + slot;
-            dst->dec0 = vx[h];                    // the screened layout: the head stage rebuilds the rest
-            dst->thr = thr[h];
 #pragma unroll
-            for (int c = 0; c < DIN; ++c) dst->z[c] = z[h][c];
-            for (int j = 0; j < D; ++j) {
-                dst->coef[j] = m[j];
-                dst->dm[j] = sane[h] ? d[j] : __longlong_as_double(0x7ff0000000000000ll);
-            }
-            a.list_a[slot] = rel[h];
-        }
-        count_stat(undecided && !(sane[h] && fp64), a.counts + 2);
-        if (a.stats != nullptr) {
-            count_stat(valid[h] && !undecided, a.stats + 0);
-            count_stat(valid[h], a.stats + 3);
-        }
+        for (int c = 0; c < DIN; ++c) t.z[c] = z[h][c];
+        stage1_screened_finish<DIN>(cfg, a, valid[h], sane[h], rel[h], t, vx[h], m, d);
     }
     timing_mark(a, HEAD_CTAS * 8);
 }
 
 // ---- stage 2: variance given the head subset, one warp per HP undecided points ---------------------
-// One CTA per SM, 8 warps.  The head factors W = L_S^-1 (column-major, zero padded, 32 KB each) and
-// the subset's inputs are staged ONCE per CTA in shared memory by TMA bulk copies (read from
-// global memory per point they cost an L2/HBM round trip per column); then every warp walks the list in groups of HP = 8 points.  Lane l owns rows l and l + 32
-// of a = W k for all HP points (16 independent FMA chains): a column of W read from shared memory
-// serves 8 points -- one point per warp makes the stage shared-memory-bandwidth bound.  The kernel values k_j of the HR subset points are
-// computed two per lane and point and exchanged through shared memory ([row][point]: one row's
-// HP values are four broadcast 128-bit loads); lane p < HP makes the decision of point p.
-constexpr int HW = HT / 32;            // warps per CTA
-constexpr int HP = 8;                  // list entries per warp iteration (long lists)
-constexpr int HP_SHORT = 2;            // ... when the list has fewer than HP entries per warp of the grid:
-                                       // the latency of one group is the whole stage then
+// One CTA per SM, HW = 16 warps.  The head factors W = L_S^-1 (packed in DMMA fragment order, 32 KB each)
+// and the subset's inputs are staged ONCE per CTA in shared memory by TMA bulk copies (read from global
+// memory per point they cost an L2/HBM round trip per column); then the warps take the list in groups of
+// HP = 8 entries: a = W k for the eight of them is one chain of DMMAs (the entries are its n dimension), so
+// a fragment of W read from shared memory serves 8 points -- one point per warp makes the stage
+// shared-memory-bandwidth bound.  The kernel values k_j of the HR subset points are computed two per lane
+// and point and exchanged through shared memory ([row][point]: the B fragments as they lie); lane p < HP
+// makes the decision of point p.
 
 // screened lists: fp64 mean of one factor's NO outputs at the lane's point.  L lanes (a power of two,
 // 4..32, consecutive in the warp) share a point: lane r of them takes rows r, r + L, ... of the
@@ -803,7 +545,7 @@ template <int DIN>
 SLB_DEV void head_round_means(const slb_sweep& cfg, const filter_args& a, const int* slots, int nneed,
                               int64_t grp0, int64_t count, const double* mbuf, const double* tab512,
                               double* mu_s, double* merr_s, int tid0, int nthreads) {
-    const int nf = cfg.gp.num_factors, D = cfg.gp.num_outputs;
+    const int nf = cfg.gp.num_factors;
     int L = 32;                                // 512 threads: 32 lanes up to 16 entries, ..., 4 beyond 64
     while (L > 4 && nneed * L > nthreads) L >>= 1;
     const int r = threadIdx.x & (L - 1);
@@ -818,10 +560,6 @@ SLB_DEV void head_round_means(const slb_sweep& cfg, const filter_args& a, const 
         for (int c = 0; c < DIN; ++c) z[c] = (live && k < count) ? a.side_a[k].z[c] : 0.0;
         for (int f = 0; f < nf; ++f) {
             const slb_gp_factor& F = cfg.gp.factors[f];
-            int outs[SLB_MAX_OUT];
-            int no = 0;
-            for (int o = 0; o < D; ++o)
-                if (cfg.gp.outputs[o].factor == f) outs[no++] = o;
             double zs[DIN];
             double zz = 0.0;
 #pragma unroll
@@ -831,49 +569,41 @@ SLB_DEV void head_round_means(const slb_sweep& cfg, const filter_args& a, const 
             }
             zz *= -0.5;
             const int Mp = padded_rows(F.M);
-            const double* xf = mbuf + a.mean_off[f];
-            double dot[SLB_MAX_OUT];
-            switch (no) {
-            case 1: head_mean_factor<DIN, 1>(xf, Mp, zs, zz, r, L, tab512, dot); break;
-            case 2: head_mean_factor<DIN, 2>(xf, Mp, zs, zz, r, L, tab512, dot); break;
-            case 3: head_mean_factor<DIN, 3>(xf, Mp, zs, zz, r, L, tab512, dot); break;
-            case 4: head_mean_factor<DIN, 4>(xf, Mp, zs, zz, r, L, tab512, dot); break;
-            case 5: head_mean_factor<DIN, 5>(xf, Mp, zs, zz, r, L, tab512, dot); break;
-            case 6: head_mean_factor<DIN, 6>(xf, Mp, zs, zz, r, L, tab512, dot); break;
-            default: break;
-            }
-            if (r == 0 && live) {
-                for (int q = 0; q < no; ++q)
-                    mean_output_finish<DIN>(F, cfg.gp.outputs[outs[q]], z, dot[q], zz, 1.0, false,
-                                            &mu_s[slot * SLB_MAX_OUT + outs[q]],
-                                            &merr_s[slot * SLB_MAX_OUT + outs[q]]);
-            }
+            const double* xf = mbuf + a.plan.mean_off[f];
+            for_outputs_on_factor(cfg.gp, f, [&](auto no, const int* outs) {
+                constexpr int NO = decltype(no)::value;
+                double dot[NO];
+                head_mean_factor<DIN, NO>(xf, Mp, zs, zz, r, L, tab512, dot);
+                if (r == 0 && live) {
+#pragma unroll 1                                   // cold, once per entry: one copy of the finish per NO
+                    for (int q = 0; q < NO; ++q)
+                        mean_output_finish<DIN>(F, cfg.gp.outputs[outs[q]], z, dot[q], zz, 1.0, false,
+                                                &mu_s[slot * SLB_MAX_OUT + outs[q]],
+                                                &merr_s[slot * SLB_MAX_OUT + outs[q]]);
+                }
+            });
         }
     }
 }
 
-// lane p < P owns list entry grp * P + p: its terms, its index, the prior bound of every output's sigma and
-// finally its decision
-template <int DIN, int P>
+// lane p < HP owns list entry grp * HP + p: its terms, its index and the prior bound of every output's sigma
+template <int DIN>
 SLB_DEV void head_group_entries(const slb_sweep& cfg, const filter_args& a, int64_t grp, int64_t count,
                                 filter_side& t, int64_t& rel, bool& mine, double* shi) {
     const int lane = threadIdx.x & 31;
-    const int D = cfg.gp.num_outputs;
-    const int64_t k = grp * P + min(lane, P - 1);
-    mine = lane < P && k < count;
+    const int64_t k = grp * HP + min(lane, HP - 1);
+    mine = lane < HP && k < count;
     t = filter_side{};
     rel = 0;
     if (mine) { t = a.side_a[k]; rel = a.list_a[k]; }
-    for (int j = 0; j < D; ++j) {
-        const slb_gp_factor& F = cfg.gp.factors[cfg.gp.outputs[j].factor];
-        shi[j] = mine ? sqrt(F.kernel.num_prims > 0 ? kernel_expr_diag<DIN>(F.kernel, t.z) : F.variance)
-                      : 0.0;
-    }
+    prior_sigma_bound<DIN>(cfg.gp, t.z, shi);
+    if (!mine)
+        for (int j = 0; j < cfg.gp.num_outputs; ++j) shi[j] = 0.0;
 }
 
-// sigma of factor f (head_rows > 0) given its head subset, for the P entries of a group on one warp
+// sigma of factor f (head_rows > 0) given its head subset, for the HP entries of a group on one warp
 // (lane p: entry p's; the other lanes' values are meaningless)
-template <int DIN, int P, bool ALL_STAGED>
+template <int DIN, bool ALL_STAGED>
 SLB_DEV double head_factor_sdev(const slb_sweep& cfg, const filter_args& a, int f, const filter_side& t,
                                 bool mine, const double* exptab, double* kw, const double* wbuf,
                                 const double* xbuf, uint64_t* bar) {
@@ -883,7 +613,7 @@ SLB_DEV double head_factor_sdev(const slb_sweep& cfg, const filter_args& a, int 
     const bool general = F.kernel.num_prims > 0;
     const double s2 = f64mul(F.scale, F.scale);
     // ALL_STAGED: the tables are known to be in shared memory (LDS instead of generic loads)
-    const bool staged = ALL_STAGED || f < a.head_factors_staged;
+    const bool staged = ALL_STAGED || f < a.plan.factors_staged;
     const double* xh = xbuf + (size_t)f * HR * DIN;
     if (!ALL_STAGED && !staged) xh = F.Xhead;
     // kernel values of every point of the group against subset points lane and lane + 32
@@ -892,7 +622,7 @@ SLB_DEV double head_factor_sdev(const slb_sweep& cfg, const filter_args& a, int 
 #pragma unroll                              // per lane and dimension instead of one per point)
     for (int c = 0; c < DIN; ++c) zown[c] = general ? t.z[c] : t.z[c] / F.lengthscales[c];
 #pragma unroll
-    for (int p = 0; p < P; ++p) {
+    for (int p = 0; p < HP; ++p) {
         double zs[DIN];
 #pragma unroll
         for (int c = 0; c < DIN; ++c) zs[c] = __shfl_sync(0xffffffffu, zown[c], p);
@@ -912,97 +642,62 @@ SLB_DEV double head_factor_sdev(const slb_sweep& cfg, const filter_args& a, int 
                 }
                 kv = s2 * kv;
             }
-            kw[j * P + p] = kv;
+            kw[j * HP + p] = kv;
         }
     }
     __syncwarp();
     double ssp = 0.0;                       // lane p: sum_i a_i^2 of point p
-    if constexpr (P == HP) {
-        // a = W k on the fp64 tensor pipe: W (64 x 64, lower triangular) pre-packed in DMMA
-        // A-fragment order (row block b, k-step s: slb_gp_factor.Wheadp), the HP = 8 points are
-        // the n dimension, k values [row][point] in shared memory are the B fragments as they
-        // lie.  Only the blocks on or below the diagonal (s <= 2 b + 1) are multiplied: 72 DMMAs.
-        const double* __restrict__ Wp = wbuf + (size_t)f * HR * HR;
-        if (!ALL_STAGED && !staged) Wp = F.Wheadp;
-        else slb_bulk::mbar_wait(bar + 1, 0);       // the packed factors have landed
-        double acc[8][2];
+    // a = W k on the fp64 tensor pipe: W (64 x 64, lower triangular) pre-packed in DMMA
+    // A-fragment order (row block b, k-step s: slb_gp_factor.Wheadp), the HP = 8 points are
+    // the n dimension, k values [row][point] in shared memory are the B fragments as they
+    // lie.  Only the blocks on or below the diagonal (s <= 2 b + 1) are multiplied: 72 DMMAs.
+    const double* __restrict__ Wp = wbuf + (size_t)f * HR * HR;
+    if (!ALL_STAGED && !staged) Wp = F.Wheadp;
+    else slb_bulk::mbar_wait(bar + 1, 0);       // the packed factors have landed
+    double acc[8][2];
 #pragma unroll
-        for (int b = 0; b < 8; ++b) { acc[b][0] = 0.0; acc[b][1] = 0.0; }
+    for (int b = 0; b < 8; ++b) { acc[b][0] = 0.0; acc[b][1] = 0.0; }
 #pragma unroll
-        for (int sk = 0; sk < 16; ++sk) {
-            const double bf = kw[(4 * sk + (lane & 3)) * HP + (lane >> 2)];
+    for (int sk = 0; sk < 16; ++sk) {
+        const double bf = kw[(4 * sk + (lane & 3)) * HP + (lane >> 2)];
 #pragma unroll
-            for (int b = sk / 2; b < 8; ++b) {
-                const double af = Wp[(b * 16 + sk) * 32 + lane];
-                asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
-                             : "+d"(acc[b][0]), "+d"(acc[b][1]) : "d"(af), "d"(bf));
-            }
-        }
-        __syncwarp();
-        // lane T holds rows 8 b + T/4 of points 2 (T%4), 2 (T%4) + 1: square, sum over b, then over
-        // the 8 lanes that share T%4; lane p fetches point p's sum
-        double v0 = 0.0, v1 = 0.0;
-#pragma unroll
-        for (int b = 0; b < 8; ++b) { v0 = fma(acc[b][0], acc[b][0], v0); v1 = fma(acc[b][1], acc[b][1], v1); }
-#pragma unroll
-        for (int off = 4; off < 32; off <<= 1) {
-            v0 += __shfl_xor_sync(0xffffffffu, v0, off);
-            v1 += __shfl_xor_sync(0xffffffffu, v1, off);
-        }
-        const double s0 = __shfl_sync(0xffffffffu, v0, (lane >> 1) & 3);
-        const double s1 = __shfl_sync(0xffffffffu, v1, (lane >> 1) & 3);
-        ssp = (lane & 1) ? s1 : s0;
-    } else {
-    // short groups: two partial sums per row and point (even / odd columns) halve the dependent
-    // FMA chain; 8-point groups already carry 16 independent chains
-    constexpr int NS = P <= 2 ? 2 : 1;
-    double al[2][P], ah[2][P];
-#pragma unroll
-    for (int p = 0; p < P; ++p) { al[0][p] = al[1][p] = 0.0; ah[0][p] = ah[1][p] = 0.0; }
-    const double* Wt = F.Whead;            // column-major table (global / L2): reference path
-#pragma unroll 4
-    for (int j = 0; j < HR; ++j) {
-        const double wl = Wt[j * HR + lane], wh = Wt[j * HR + 32 + lane];
-        double kj[P];
-#pragma unroll
-        for (int p = 0; p < P; p += 2) {
-            const double2 v = *reinterpret_cast<const double2*>(kw + j * P + p);
-            kj[p] = v.x; kj[p + 1] = v.y;
-        }
-#pragma unroll
-        for (int p = 0; p < P; ++p) {
-            al[j & (NS - 1)][p] = fma(wl, kj[p], al[j & (NS - 1)][p]);
-            ah[j & (NS - 1)][p] = fma(wh, kj[p], ah[j & (NS - 1)][p]);
+        for (int b = sk / 2; b < 8; ++b) {
+            const double af = Wp[(b * 16 + sk) * 32 + lane];
+            asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
+                         : "+d"(acc[b][0]), "+d"(acc[b][1]) : "d"(af), "d"(bf));
         }
     }
     __syncwarp();
-    // sum a^2 per point over the 64 rows: lane p ends up with point p's
+    // lane T holds rows 8 b + T/4 of points 2 (T%4), 2 (T%4) + 1: square, sum over b, then over
+    // the 8 lanes that share T%4; lane p fetches point p's sum
+    double v0 = 0.0, v1 = 0.0;
 #pragma unroll
-    for (int p = 0; p < P; ++p) {
-        const double lo = al[0][p] + al[1][p], hi = ah[0][p] + ah[1][p];
-        double ss = fma(lo, lo, hi * hi);
+    for (int b = 0; b < 8; ++b) { v0 = fma(acc[b][0], acc[b][0], v0); v1 = fma(acc[b][1], acc[b][1], v1); }
 #pragma unroll
-        for (int off = 16; off > 0; off >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, off);
-        if (lane == p) ssp = ss;
+    for (int off = 4; off < 32; off <<= 1) {
+        v0 += __shfl_xor_sync(0xffffffffu, v0, off);
+        v1 += __shfl_xor_sync(0xffffffffu, v1, off);
     }
-    }
+    const double s0 = __shfl_sync(0xffffffffu, v0, (lane >> 1) & 3);
+    const double s1 = __shfl_sync(0xffffffffu, v1, (lane >> 1) & 3);
+    ssp = (lane & 1) ? s1 : s0;
     double kss = F.kss;
     if (general && mine) kss = s2 * kernel_expr_diag<DIN>(F.kernel, t.z);
     const double sdev = sqrt(f64sub(kss, ssp) / s2);          // NaN if negative
     return sdev;
 }
 
-// one group of P list entries [g P, g P + P) on one warp, factor after factor
-template <int DIN, int P, bool ALL_STAGED>
+// one group of HP list entries [g HP, g HP + HP) on one warp, factor after factor
+template <int DIN, bool ALL_STAGED>
 SLB_DEV void head_group_bound(const slb_sweep& cfg, const filter_args& a, int64_t grp, int64_t count,
                               const double* exptab, double* kw, const double* wbuf, const double* xbuf,
                               uint64_t* bar, filter_side& t, int64_t& rel, bool& mine, double* shi) {
-    head_group_entries<DIN, P>(cfg, a, grp, count, t, rel, mine, shi);
+    head_group_entries<DIN>(cfg, a, grp, count, t, rel, mine, shi);
     slb_bulk::mbar_wait(bar + 0, 0);            // exp tables and subset inputs have landed
     head_mark(a, HM_TABLES);
     for (int f = 0; f < cfg.gp.num_factors; ++f) {
         if (cfg.gp.factors[f].head_rows <= 0) continue;
-        const double sdev = head_factor_sdev<DIN, P, ALL_STAGED>(cfg, a, f, t, mine, exptab, kw, wbuf, xbuf, bar);
+        const double sdev = head_factor_sdev<DIN, ALL_STAGED>(cfg, a, f, t, mine, exptab, kw, wbuf, xbuf, bar);
         for (int j = 0; j < cfg.gp.num_outputs; ++j)
             if (cfg.gp.outputs[j].factor == f) shi[j] = sdev;
         if (f == 0) head_mark(a, HM_BOUND0);
@@ -1013,10 +708,41 @@ SLB_DEV void head_group_bound(const slb_sweep& cfg, const filter_args& a, int64_
 // an entry of the factored grid kernel with finite bounds carries an fp64-class mean: the head stage
 // decides it from its box, or sends it to the refine pass, without recomputing the mean
 SLB_DEV bool fp64_class_entry(const filter_args& a, const filter_side& t, int D) {
-    if (!a.grid_means) return false;
+    if (a.plan.mean_scheme != SLB_MEAN_GRID_FACTORED) return false;
     bool finite = true;
-    for (int j = 0; j < D; ++j) finite &= t.dm[j] < __longlong_as_double(0x7ff0000000000000ll);
+    for (int j = 0; j < D; ++j) finite &= t.dm[j] < f64_inf();
     return finite;
+}
+
+// The decision of a list entry from what stage 1 left in it and the bound shi of every sigma, the same in
+// both schedules.  A complete entry (fp64 mean stage): the comparison itself.  A screened entry: over the
+// box of its screened mean first -- most are decided by the tighter variance bound alone; `need`: it is
+// still open and has no fp64-class mean, so head_mean_decision follows with vx = V(x).
+SLB_DEV int head_entry_decision(const slb_sweep& cfg, const filter_args& a, filter_side& t, const double* shi,
+                                bool mine, double& vx, bool& need) {
+    const int D = cfg.gp.num_outputs;
+    need = false;
+    if (a.plan.mean_scheme == SLB_MEAN_FP64) return mine ? decide(t, shi, D) : 0;
+    double mu[SLB_MAX_OUT], dm[SLB_MAX_OUT];
+    for (int j = 0; j < SLB_MAX_OUT; ++j) { mu[j] = t.coef[j]; dm[j] = t.dm[j]; }
+    vx = t.dec0;
+    const int screened = screened_outcome(cfg, t, vx, mu, dm, shi);
+    const int outcome = mine ? screened : 0;
+    need = mine && outcome < 0 && !fp64_class_entry(a, t, D);
+    head_mark(a, HM_SCREENED);
+    return outcome;
+}
+
+// ... and with the fp64 mean head_round_means left for its slot: the comparison of the fp64 mean stage
+SLB_DEV int head_mean_decision(const slb_sweep& cfg, filter_side& t, double vx, const double* shi,
+                               const double* mu_s, const double* merr_s, int slot) {
+    double mu[SLB_MAX_OUT], merr[SLB_MAX_OUT];
+    for (int j = 0; j < SLB_MAX_OUT; ++j) {
+        mu[j] = mu_s[slot * SLB_MAX_OUT + j];
+        merr[j] = merr_s[slot * SLB_MAX_OUT + j];
+    }
+    mean_decision_terms(cfg, t, vx, mu, merr);
+    return decide(t, shi, cfg.gp.num_outputs);
 }
 
 // every copy lands in this CTA's shared memory before the CTA may leave
@@ -1047,47 +773,49 @@ filter_head_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
     prefetch_descriptor_operands(cfg);
     // three landings, each waited for just before its first use: (a) the exp tables and the subsets'
     // inputs (kernel values), (b) the packed head factors (DMMA), (c) screened lists: [Xf | gamma_f]
-    uint64_t* bar = reinterpret_cast<uint64_t*>(smem_raw);             // [3]
-    unsigned* s_stat = reinterpret_cast<unsigned*>(smem_raw + 24);     // decided / undecided by this CTA
-    double* tab512 = reinterpret_cast<double*>(smem_raw + 32);         // [512] (screened lists: exp_neg_fast)
-    double* exptab = tab512 + 512;                                     // [64]
-    double* kbuf = exptab + 64;                                        // [HW][HR][HP]
-    double* sd_s = kbuf + HW * HR * HP;                                // split schedule: [HW * HP][SLB_MAX_OUT]
-    double* wbuf = sd_s + HW * HP * SLB_MAX_OUT;                       // [staged][HR * HR]
+    const filter_plan& lay = a.plan;
+    double* smem = reinterpret_cast<double*>(smem_raw);
+    uint64_t* bar = reinterpret_cast<uint64_t*>(smem);                 // [3]
+    unsigned* s_stat = reinterpret_cast<unsigned*>(smem + 3);          // decided / undecided by this CTA
+    double* tab512 = smem + lay.tabs;                                  // (screened lists: exp_neg_fast)
+    double* exptab = tab512 + 512;
+    double* kbuf = smem + lay.kbuf;
+    double* wbuf = smem + lay.wbuf;
+    double* xbuf = smem + lay.xbuf;
+    double* mbuf = smem + lay.mbuf;
     const int nf = cfg.gp.num_factors;
-    double* xbuf = wbuf + (size_t)a.head_factors_staged * HR * HR;     // [staged][HR * DIN]
-    double* mbuf = xbuf + (size_t)a.head_factors_staged * HR * DIN;    // screened: [Xf | gamma_f ...] per factor
+    const bool screened = lay.mean_scheme != SLB_MEAN_FP64;
     // fp64 means are recomputed here only for entries without an fp64-class one (all of them after the
     // fp32 screening kernel, those the grid kernel left with dm = inf: counts[2])
-    const bool means = a.screened && (!a.grid_means || a.counts[2] != 0);
+    const bool means = screened && (lay.mean_scheme != SLB_MEAN_GRID_FACTORED || a.counts[2] != 0);
     if (threadIdx.x == 0) {
         for (int b = 0; b < 3; ++b) slb_bulk::mbar_init(bar + b, 1);
         slb_bulk::fence_barrier_init();
         slb_bulk::fence_proxy_async();
         unsigned xbytes = 576 * sizeof(double), wbytes = 0;
-        for (int f = 0; f < a.head_factors_staged; ++f)
+        for (int f = 0; f < lay.factors_staged; ++f)
             if (cfg.gp.factors[f].head_rows > 0) {
                 xbytes += (unsigned)(HR * DIN) * sizeof(double);
                 wbytes += (unsigned)(HR * HR) * sizeof(double);
             }
         slb_bulk::mbar_arrive_expect_tx(bar + 0, xbytes);
         slb_bulk::copy_g2s(tab512, g_exp_tables, 576 * sizeof(double), bar + 0);
-        for (int f = 0; f < a.head_factors_staged; ++f)
+        for (int f = 0; f < lay.factors_staged; ++f)
             if (cfg.gp.factors[f].head_rows > 0)
                 slb_bulk::copy_g2s(xbuf + (size_t)f * HR * DIN, cfg.gp.factors[f].Xhead,
                                    HR * DIN * sizeof(double), bar + 0);
         slb_bulk::mbar_arrive_expect_tx(bar + 1, wbytes);
-        for (int f = 0; f < a.head_factors_staged; ++f)
+        for (int f = 0; f < lay.factors_staged; ++f)
             if (cfg.gp.factors[f].head_rows > 0)
                 slb_bulk::copy_g2s(wbuf + (size_t)f * HR * HR, cfg.gp.factors[f].Wheadp,
                                    HR * HR * sizeof(double), bar + 1);
-        slb_bulk::mbar_arrive_expect_tx(bar + 2, means ? (unsigned)a.mean_doubles * sizeof(double) : 0u);
+        slb_bulk::mbar_arrive_expect_tx(bar + 2, means ? (unsigned)lay.mean_doubles * sizeof(double) : 0u);
         if (means) {
             for (int f = 0; f < nf; ++f) {
                 const slb_gp_factor& F = cfg.gp.factors[f];
                 const int Mp = padded_rows(F.M);
                 if (Mp == 0) continue;
-                double* dst = mbuf + a.mean_off[f];
+                double* dst = mbuf + lay.mean_off[f];
                 slb_bulk::copy_g2s(dst, F.Xf, (unsigned)(Mp * (DIN + 1)) * sizeof(double), bar + 2);
                 dst += (size_t)Mp * (DIN + 1);
                 for (int o = 0; o < cfg.gp.num_outputs; ++o) {
@@ -1124,8 +852,7 @@ filter_head_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
         }
     }
     if (threadIdx.x < 2) s_stat[threadIdx.x] = 0;
-    if (a.screened && threadIdx.x < 2)
-        reinterpret_cast<int*>(mbuf + a.mean_doubles + 2 * HW * HP * SLB_MAX_OUT)[threadIdx.x] = 0;
+    if (screened && threadIdx.x < 2) reinterpret_cast<int*>(smem + lay.need)[threadIdx.x] = 0;
     __syncthreads();
     const int64_t count = (int64_t)a.counts[0];
     const int64_t nwarps = (int64_t)gridDim.x * HW;
@@ -1139,9 +866,10 @@ filter_head_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
     }
     const int warp = threadIdx.x >> 5;
     double* kw = kbuf + warp * HR * HP;
-    double* mu_s = mbuf + a.mean_doubles;      // screened: [HW * HP][SLB_MAX_OUT] fp64 means, then their error bounds
-    double* merr_s = mu_s + HW * HP * SLB_MAX_OUT;
-    int* need_s = reinterpret_cast<int*>(merr_s + HW * HP * SLB_MAX_OUT);   // [2] counters (round parity), slots
+    double* sd_s = smem + lay.sd;
+    double* mu_s = smem + lay.mu;
+    double* merr_s = smem + lay.merr;
+    int* need_s = reinterpret_cast<int*>(smem + lay.need);
     // Short lists (one round, and a warp to spare beside one warp per group and factor: C2) are latency
     // bound: the split schedule gives every (group, factor) pair a warp of its own, and the spare warps
     // compute the fp64 means of all the round's entries meanwhile (used only where the screened box
@@ -1171,9 +899,9 @@ filter_head_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
                         for (int c = 0; c < DIN; ++c) tz.z[c] = a.side_a[k].z[c];
                     }
                     const double sd =
-                        a.head_factors_staged == nf
-                            ? head_factor_sdev<DIN, HP, true>(cfg, a, f, tz, mine, exptab, kw, wbuf, xbuf, bar)
-                            : head_factor_sdev<DIN, HP, false>(cfg, a, f, tz, mine, exptab, kw, wbuf, xbuf, bar);
+                        lay.factors_staged == nf
+                            ? head_factor_sdev<DIN, true>(cfg, a, f, tz, mine, exptab, kw, wbuf, xbuf, bar)
+                            : head_factor_sdev<DIN, false>(cfg, a, f, tz, mine, exptab, kw, wbuf, xbuf, bar);
                     if (lane < HP) sd_s[(i * HP + lane) * SLB_MAX_OUT + f] = sd;
                     if (f == 0) head_mark(a, HM_BOUND0);
                 }
@@ -1198,34 +926,16 @@ filter_head_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
                 int64_t rel;
                 bool mine;
                 double shi[SLB_MAX_OUT];
-                head_group_entries<DIN, HP>(cfg, a, grp0 + (int64_t)warp * gridDim.x, count, t, rel, mine, shi);
+                head_group_entries<DIN>(cfg, a, grp0 + (int64_t)warp * gridDim.x, count, t, rel, mine, shi);
                 const int slot = warp * HP + min(lane, HP - 1);
                 for (int j = 0; j < cfg.gp.num_outputs; ++j) {
                     const int f = cfg.gp.outputs[j].factor;
                     if (cfg.gp.factors[f].head_rows > 0) shi[j] = sd_s[slot * SLB_MAX_OUT + f];
                 }
-                int outcome = 0;
-                if (a.screened) {
-                    // the same two comparisons as the round loop: the screened box, then the fp64 mean
-                    double mu[SLB_MAX_OUT], dm[SLB_MAX_OUT], zero[SLB_MAX_OUT];
-                    for (int j = 0; j < SLB_MAX_OUT; ++j) { mu[j] = t.coef[j]; dm[j] = t.dm[j]; zero[j] = 0.0; }
-                    const double vx = t.dec0;
-                    mean_decision_terms(cfg, t, vx, mu, zero);
-                    t.guard += screening_slack(cfg, mu, dm, shi);
-                    outcome = mine ? decide(t, shi, cfg.gp.num_outputs) : 0;
-                    head_mark(a, HM_SCREENED);
-                    if (mine && outcome < 0 && !fp64_class_entry(a, t, cfg.gp.num_outputs)) {
-                        double merr[SLB_MAX_OUT];
-                        for (int j = 0; j < SLB_MAX_OUT; ++j) {
-                            mu[j] = mu_s[slot * SLB_MAX_OUT + j];
-                            merr[j] = merr_s[slot * SLB_MAX_OUT + j];
-                        }
-                        mean_decision_terms(cfg, t, vx, mu, merr);
-                        outcome = decide(t, shi, cfg.gp.num_outputs);
-                    }
-                } else {
-                    outcome = mine ? decide(t, shi, cfg.gp.num_outputs) : 0;
-                }
+                double vx = 0.0;
+                bool need;
+                int outcome = head_entry_decision(cfg, a, t, shi, mine, vx, need);
+                if (need) outcome = head_mean_decision(cfg, t, vx, shi, mu_s, merr_s, slot);
                 head_mark(a, HM_DECIDED);
                 head_group_finish(a, mine, outcome, rel, s_stat);
             }
@@ -1245,27 +955,14 @@ filter_head_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
             double vx = 0.0;
             int outcome = 0;
             if (active) {
-                if (a.head_factors_staged == nf)
-                    head_group_bound<DIN, HP, true>(cfg, a, grp, count, exptab, kw, wbuf, xbuf, bar, t, rel, mine, shi);
+                if (lay.factors_staged == nf)
+                    head_group_bound<DIN, true>(cfg, a, grp, count, exptab, kw, wbuf, xbuf, bar, t, rel, mine, shi);
                 else
-                    head_group_bound<DIN, HP, false>(cfg, a, grp, count, exptab, kw, wbuf, xbuf, bar, t, rel, mine, shi);
-                if (a.screened) {
-                    // first with the screened mean and its error box (stage 1 left them in the entry): most
-                    // entries are decided by the tighter variance bound alone
-                    double mu[SLB_MAX_OUT], dm[SLB_MAX_OUT], zero[SLB_MAX_OUT];
-                    for (int j = 0; j < SLB_MAX_OUT; ++j) { mu[j] = t.coef[j]; dm[j] = t.dm[j]; zero[j] = 0.0; }
-                    vx = t.dec0;
-                    mean_decision_terms(cfg, t, vx, mu, zero);
-                    t.guard += screening_slack(cfg, mu, dm, shi);
-                    outcome = mine ? decide(t, shi, cfg.gp.num_outputs) : 0;
-                    need = mine && outcome < 0 && !fp64_class_entry(a, t, cfg.gp.num_outputs);
-                    if (need) need_s[2 + atomicAdd(need_s + (round & 1), 1)] = warp * HP + lane;
-                    head_mark(a, HM_SCREENED);
-                } else {
-                    outcome = mine ? decide(t, shi, cfg.gp.num_outputs) : 0;
-                }
+                    head_group_bound<DIN, false>(cfg, a, grp, count, exptab, kw, wbuf, xbuf, bar, t, rel, mine, shi);
+                outcome = head_entry_decision(cfg, a, t, shi, mine, vx, need);
+                if (need) need_s[2 + atomicAdd(need_s + (round & 1), 1)] = warp * HP + lane;
             }
-            if (a.screened) {
+            if (screened) {
                 if (threadIdx.x == 0) need_s[(round + 1) & 1] = 0;       // the next round's counter
                 __syncthreads();
                 const int nneed = need_s[round & 1];
@@ -1275,16 +972,7 @@ filter_head_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
                     head_round_means<DIN>(cfg, a, need_s + 2, nneed, grp0, count, mbuf, tab512, mu_s, merr_s, 0, HT);
                     head_mark(a, HM_MEANS);
                     __syncthreads();
-                    if (need) {
-                        double mu[SLB_MAX_OUT], merr[SLB_MAX_OUT];
-                        const int slot = warp * HP + lane;
-                        for (int j = 0; j < SLB_MAX_OUT; ++j) {
-                            mu[j] = mu_s[slot * SLB_MAX_OUT + j];
-                            merr[j] = merr_s[slot * SLB_MAX_OUT + j];
-                        }
-                        mean_decision_terms(cfg, t, vx, mu, merr);
-                        outcome = decide(t, shi, cfg.gp.num_outputs);
-                    }
+                    if (need) outcome = head_mean_decision(cfg, t, vx, shi, mu_s, merr_s, warp * HP + lane);
                 }
             }
             if (active) {
@@ -1339,41 +1027,47 @@ bool grid_mean_applicable(const slb_sweep& cfg) {
            !(P.flags & ~(uint32_t)(SLB_FLAG_SATURATE | SLB_FLAG_SCALE));
 }
 
-// Shared-memory plan of the head stage (one CTA per SM): which factors' head tables are staged, and --
-// when the fp32 screening kernel is stage 1 -- every factor's [Xf | gamma_f] next to them.  Screening
+// Which stage 1 runs and the shared-memory layout of the head stage (one CTA per SM): which factors' head
+// tables are staged, and -- for a screened stage 1 -- every factor's [Xf | gamma_f] next to them.  Screening
 // is only used when all of it fits (otherwise the fp64 mean stage runs, whose list entries are complete).
-void head_layout(const slb_sweep& cfg, int din, filter_args& ah, size_t& head_smem) {
-    const size_t head_fixed = 32 + (576 + HW * HR * HP + HW * HP * SLB_MAX_OUT) * sizeof(double);
-    const size_t per_factor = (size_t)(HR * HR + HR * din) * sizeof(double);
-    ah.head_factors_staged = cfg.gp.num_factors;
-    while (ah.head_factors_staged > 0 && head_fixed + ah.head_factors_staged * per_factor > 226 * 1024)
-        --ah.head_factors_staged;
-    head_smem = head_fixed + ah.head_factors_staged * per_factor;
-    ah.screened = 0;
-    ah.mean_doubles = 0;
-    ah.prefetch_factors = (g_filter_stages & 2) ? 1 : 0;
-    ah.head_schedule = (g_filter_stages >> 3) & 3;
-    if (screening_applicable(cfg) && ah.head_factors_staged == cfg.gp.num_factors) {
-        int off = 0;
-        for (int f = 0; f < cfg.gp.num_factors; ++f) {
-            int no = 0;
-            for (int o = 0; o < cfg.gp.num_outputs; ++o) no += cfg.gp.outputs[o].factor == f;
-            ah.mean_off[f] = off;
-            off += ((cfg.gp.factors[f].M + 7) & ~7) * (din + 1 + no);
-        }
-        const size_t extra = ((size_t)off + 2 * HW * HP * SLB_MAX_OUT) * sizeof(double) +
-                             (size_t)(HW * HP + 4) * sizeof(int);
-        if (head_smem + extra <= 226 * 1024) {
-            ah.screened = 1;
-            ah.mean_doubles = off;
-            head_smem += extra;
-        }
+filter_plan stage1_plan(const slb_sweep& cfg) {
+    const int din = cfg.gp.input_dim, nf = cfg.gp.num_factors;
+    const int budget = 226 * 1024 / (int)sizeof(double);
+    const int slots = HW * HP * SLB_MAX_OUT;
+    filter_plan p = {};
+    p.mean_scheme = SLB_MEAN_FP64;
+    p.factors_staged = nf;
+    while (p.factors_staged > 0 && 4 + 576 + HW * HR * HP + slots + p.factors_staged * (HR * HR + HR * din) > budget)
+        --p.factors_staged;
+    int off = 4;
+    p.tabs = off;   off += 576;
+    p.kbuf = off;   off += HW * HR * HP;
+    p.sd = off;     off += slots;
+    p.wbuf = off;   off += p.factors_staged * HR * HR;
+    p.xbuf = off;   off += p.factors_staged * HR * din;
+    p.doubles = off;
+    if (!screening_applicable(cfg) || p.factors_staged != nf) return p;
+    int tables = 0;
+    for (int f = 0; f < nf; ++f) {
+        int no = 0;
+        for (int o = 0; o < cfg.gp.num_outputs; ++o) no += cfg.gp.outputs[o].factor == f;
+        p.mean_off[f] = tables;
+        tables += ((cfg.gp.factors[f].M + 7) & ~7) * (din + 1 + no);
     }
-    ah.grid_means = ah.screened && grid_mean_applicable(cfg) ? 1 : 0;
+    const int need = (HW * HP + 4) * (int)sizeof(int) / (int)sizeof(double);
+    if (off + tables + 2 * slots + need > budget) return p;
+    p.mean_scheme = grid_mean_applicable(cfg) ? SLB_MEAN_GRID_FACTORED : SLB_MEAN_FP32_SCREENED;
+    p.mean_doubles = tables;
+    p.mbuf = off;   off += tables;
+    p.mu = off;     off += slots;
+    p.merr = off;   off += slots;
+    p.need = off;   off += need;
+    p.doubles = off;
+    return p;
 }
 
 template <int DIN>
-int launch_filter(cudaStream_t st, const slb_sweep& cfg, const filter_args& a, size_t smem) {
+int launch_filter(cudaStream_t st, const slb_sweep& cfg, const filter_args& a) {
     static std::atomic<bool> configured[64];
     int device = 0;
     SLB_CUDA(cudaGetDevice(&device));
@@ -1391,31 +1085,27 @@ int launch_filter(cudaStream_t st, const slb_sweep& cfg, const filter_args& a, s
         if (device >= 0 && device < 64) configured[device].store(true, std::memory_order_release);
     }
     const int64_t blocks = (a.n + FT - 1) / FT;
-    filter_args ah = a;
-    size_t head_smem = 0;
-    head_layout(cfg, DIN, ah, head_smem);
-    ah.probe_mu = g_probe_mu;
-    ah.probe_dm = g_probe_dm;
-    ah.timing = g_head_timing;
-    if (ah.grid_means) {                          // d_in = 3 (grid_mean_applicable)
+    switch (a.plan.mean_scheme) {
+    case SLB_MEAN_GRID_FACTORED:                  // d_in = 3 (grid_mean_applicable)
         if constexpr (DIN == 3) {
             // tiles of GR rows x GC columns over the rows the range touches (it may start and end mid-row)
             const int64_t n1 = cfg.grid.num_points[1];
             const int64_t r0 = a.idx_begin / n1, r1 = (a.idx_begin + a.n - 1) / n1;
             const int64_t tiles = ((r1 - r0) / GR + 1) * ((n1 + GC - 1) / GC);
-            filter_grid_mean_kernel<DIN><<<(unsigned)tiles, GT, grid_mean_smem_bytes(), st>>>(cfg, ah);
+            filter_grid_mean_kernel<DIN><<<(unsigned)tiles, GT, grid_mean_smem_bytes(), st>>>(cfg, a);
         }
-    } else if (ah.screened) {
-        const size_t smem32 = mean32_smem_bytes(DIN, a.max_outputs_per_factor, a.chunk_rows, FT / 32);
-        filter_mean32_kernel<DIN><<<(unsigned)blocks, FT, smem32, st>>>(cfg, ah);
-    } else {
-        filter_args a1 = a;
-        a1.timing = g_head_timing;
-        filter_mean_kernel<DIN><<<(unsigned)blocks, FT, smem, st>>>(cfg, a1);
+        break;
+    case SLB_MEAN_FP32_SCREENED:
+        filter_mean32_kernel<DIN><<<(unsigned)blocks, FT,
+                                    mean32_smem_bytes(DIN, a.max_outputs_per_factor, a.chunk_rows, FT / 32), st>>>(cfg, a);
+        break;
+    default:
+        filter_mean_kernel<DIN><<<(unsigned)blocks, FT,
+                                  mean_smem_bytes(DIN, a.max_outputs_per_factor, a.chunk_rows), st>>>(cfg, a);
     }
     SLB_LAUNCH_CHECK();
     if (!(g_filter_stages & 1)) return 0;
-    filter_head_kernel<DIN><<<HEAD_CTAS, HT, head_smem, st>>>(cfg, ah);
+    filter_head_kernel<DIN><<<HEAD_CTAS, HT, (size_t)a.plan.doubles * sizeof(double), st>>>(cfg, a);
     SLB_LAUNCH_CHECK();
     return 0;
 }
@@ -1435,21 +1125,13 @@ int slb_debug_filter_stages(int32_t mask) {
 }
 
 int slb_filter_stage1(const slb_sweep* cfg) {
-    if (cfg == nullptr || cfg->gp.num_outputs <= 0) return 0;
-    filter_args a;
-    memset(&a, 0, sizeof(a));
-    size_t smem = 0;
-    head_layout(*cfg, cfg->gp.input_dim, a, smem);
-    return a.screened ? 32 : 64;
+    const int scheme = slb_filter_mean_scheme(cfg);
+    return scheme == SLB_MEAN_NONE ? 0 : scheme == SLB_MEAN_FP64 ? 64 : 32;
 }
 
 int slb_filter_mean_scheme(const slb_sweep* cfg) {
     if (cfg == nullptr || cfg->gp.num_outputs <= 0) return SLB_MEAN_NONE;
-    filter_args a;
-    memset(&a, 0, sizeof(a));
-    size_t smem = 0;
-    head_layout(*cfg, cfg->gp.input_dim, a, smem);
-    return a.grid_means ? SLB_MEAN_GRID_FACTORED : a.screened ? SLB_MEAN_FP32_SCREENED : SLB_MEAN_FP64;
+    return stage1_plan(*cfg).mean_scheme;
 }
 
 int slb_debug_screening_probe(double* mu_dev, double* dm_dev) {
@@ -1482,6 +1164,8 @@ int slb_lyapunov_sweep_filtered(void* stream, const slb_sweep* cfg, int64_t idx_
     if (slb_validate_staged_tables(&cfg->gp, "filtered sweep")) return 1;
     int nomax = 1;
     for (int f = 0; f < cfg->gp.num_factors; ++f) {
+        // (Whead has no device reader since the head stage multiplies the packed Wheadp only; the field stays
+        // part of the descriptor: the parity tests take their reference from it)
         const slb_gp_factor& F = cfg->gp.factors[f];
         SLB_CHECK(F.M == 0 || (F.Whead != nullptr && F.Wheadp != nullptr && F.Xhead != nullptr),
                   "filtered sweep: GP factor %d lacks the filter tables (Whead / Wheadp / Xhead)", f);
@@ -1518,7 +1202,12 @@ int slb_lyapunov_sweep_filtered(void* stream, const slb_sweep* cfg, int64_t idx_
     const int din = cfg->gp.input_dim;
     a.chunk_rows = mean_chunk_rows(din, nomax, 24);
     a.max_outputs_per_factor = nomax;
-    const size_t smem = mean_smem_bytes(din, nomax, a.chunk_rows);
+    a.plan = stage1_plan(*cfg);
+    a.prefetch_factors = (g_filter_stages & 2) ? 1 : 0;
+    a.head_schedule = (g_filter_stages >> 3) & 3;
+    a.probe_mu = g_probe_mu;
+    a.probe_dm = g_probe_dm;
+    a.timing = g_head_timing;
     for (int64_t off = 0; off < n_all; off += CHUNK) {
         const int64_t n = n_all - off < CHUNK ? n_all - off : CHUNK;
         SLB_CUDA(cudaMemsetAsync(a.counts, 0, 64 + SLB_SPLIT_TICKET_BYTES, st));
@@ -1526,7 +1215,7 @@ int slb_lyapunov_sweep_filtered(void* stream, const slb_sweep* cfg, int64_t idx_
         a.negative = negative_dev + off;
         a.values = values_dev ? values_dev + off : nullptr;
         int rc = slb_dispatch_dim<1, 6>(din, "GP input_dim", [&](auto D) {
-            return launch_filter<D>(st, *cfg, a, smem);
+            return launch_filter<D>(st, *cfg, a);
         });
         if (rc) return rc;
         if (!(g_filter_stages & 2)) continue;

@@ -53,6 +53,38 @@ SLB_DEV int first_factor_with_data(const slb_gp_stack& gp, int f) {
     return f;
 }
 
+SLB_DEV double f64_inf() { return __longlong_as_double(0x7ff0000000000000ll); }
+
+// The outputs that live on factor f, their number a compile-time constant for the caller's running sums:
+// fn(std::integral_constant<int, NO>, outs) with 1 <= NO <= MAXNO (a factor without outputs is skipped).
+template <int MAXNO = SLB_MAX_OUT, class Fn>
+SLB_DEV void for_outputs_on_factor(const slb_gp_stack& gp, int f, Fn&& fn) {
+    static_assert(MAXNO <= 6, "one case per count");
+    int outs[SLB_MAX_OUT];
+    int no = 0;
+    for (int o = 0; o < gp.num_outputs; ++o)
+        if (gp.outputs[o].factor == f) outs[no++] = o;
+    switch (no) {
+    case 1: fn(std::integral_constant<int, 1>{}, outs); break;
+    case 2: if constexpr (MAXNO >= 2) fn(std::integral_constant<int, 2>{}, outs); break;
+    case 3: if constexpr (MAXNO >= 3) fn(std::integral_constant<int, 3>{}, outs); break;
+    case 4: if constexpr (MAXNO >= 4) fn(std::integral_constant<int, 4>{}, outs); break;
+    case 5: if constexpr (MAXNO >= 5) fn(std::integral_constant<int, 5>{}, outs); break;
+    case 6: if constexpr (MAXNO >= 6) fn(std::integral_constant<int, 6>{}, outs); break;
+    default: break;
+    }
+}
+
+// scale * (z . prior_mean) of one output, in the operation order of functions.py:439-442
+template <int DIN>
+SLB_DEV double prior_mean_term(const slb_gp_factor& F, const slb_gp_output& G, const double* z) {
+    if (G.prior_mean == nullptr) return 0.0;
+    double mx = f64mul(z[0], G.prior_mean[0]);
+#pragma unroll
+    for (int c = 1; c < DIN; ++c) mx = f64add(mx, f64mul(z[c], G.prior_mean[c]));
+    return f64mul(F.scale, mx);
+}
+
 // thread 0: issue the producer's next slice into buffer `b` and advance
 template <int DIN>
 SLB_DEV void issue_slice(const slb_gp_stack& gp, mean_pipe& P, int b) {
@@ -98,14 +130,7 @@ template <int DIN>
 SLB_DEV void mean_output_finish(const slb_gp_factor& F, const slb_gp_output& G, const double* z,
                                 double dot, double zz, double kbound, bool general, double* mu,
                                 double* mean_err) {
-    double mx = 0.0;
-    if (G.prior_mean != nullptr) {
-        mx = f64mul(z[0], G.prior_mean[0]);
-#pragma unroll
-        for (int c = 1; c < DIN; ++c) mx = f64add(mx, f64mul(z[c], G.prior_mean[c]));
-        mx = f64mul(F.scale, mx);
-    }
-    *mu = f64add(dot, mx) / F.scale;
+    *mu = f64add(dot, prior_mean_term<DIN>(F, G, z)) / F.scale;
     // |mean - exact| <= eps sum_i |k_i| (|L^-1|^T |alpha|)_i <= eps kbound gamma_l1: kernel
     // values to EPS_K (+ the expanded distance's rounding), the M-term sums here, in gamma
     // itself and in the a . alpha form of the full posterior each to (M + 2) 2^-53
@@ -200,14 +225,15 @@ SLB_DEV void mean_factor(const slb_gp_stack& gp, int f, const int* outs, const d
                                 &mu[outs[q]], &mean_err[outs[q]]);
 }
 
-// thread 0 of the block: barriers of the pipeline + the bulk copy of the exp tables (bar[2]); call
-// once per kernel, before the first __syncthreads
+// thread 0 of the block: barriers of the pipeline + the bulk copy of the exp tables (bar[2]; none for a
+// carve-up without tables: tab512 == nullptr); call once per kernel, before the first __syncthreads
 SLB_DEV void mean_pipe_init(mean_pipe& P, double* tab512) {
     slb_bulk::mbar_init(P.bar + 0, 1);
     slb_bulk::mbar_init(P.bar + 1, 1);
-    slb_bulk::mbar_init(P.bar + 2, 1);
+    if (tab512 != nullptr) slb_bulk::mbar_init(P.bar + 2, 1);
     slb_bulk::fence_barrier_init();
     slb_bulk::fence_proxy_async();
+    if (tab512 == nullptr) return;
     slb_bulk::mbar_arrive_expect_tx(P.bar + 2, 576 * sizeof(double));
     slb_bulk::copy_g2s(tab512, g_exp_tables, 576 * sizeof(double), P.bar + 2);
 }
@@ -226,38 +252,32 @@ SLB_DEV void mean_pipe_start(const slb_gp_stack& gp, mean_pipe& P) {
 template <int DIN, bool FAST>
 SLB_DEV void gp_mean_staged(const slb_gp_stack& gp, const double* z, double* mu, double* mean_err,
                             const double* tab512, const double* tab64, mean_pipe& P) {
-    for (int f = 0; f < gp.num_factors; ++f) {
-        int outs[SLB_MAX_OUT];
-        int no = 0;
-        for (int o = 0; o < gp.num_outputs; ++o)
-            if (gp.outputs[o].factor == f) outs[no++] = o;
-        switch (no) {
-        case 1: mean_factor<DIN, 1, FAST>(gp, f, outs, z, mu, mean_err, tab512, tab64, P); break;
-        case 2: mean_factor<DIN, 2, FAST>(gp, f, outs, z, mu, mean_err, tab512, tab64, P); break;
-        case 3: mean_factor<DIN, 3, FAST>(gp, f, outs, z, mu, mean_err, tab512, tab64, P); break;
-        case 4: mean_factor<DIN, 4, FAST>(gp, f, outs, z, mu, mean_err, tab512, tab64, P); break;
-        case 5: mean_factor<DIN, 5, FAST>(gp, f, outs, z, mu, mean_err, tab512, tab64, P); break;
-        case 6: mean_factor<DIN, 6, FAST>(gp, f, outs, z, mu, mean_err, tab512, tab64, P); break;
-        default: break;
-        }
-    }
+    for (int f = 0; f < gp.num_factors; ++f)
+        for_outputs_on_factor(gp, f, [&](auto no, const int* outs) {
+            mean_factor<DIN, decltype(no)::value, FAST>(gp, f, outs, z, mu, mean_err, tab512, tab64, P);
+        });
 }
 
 // shared-memory carve-up of the mean stage: [0, 32) mbarriers (2 slices, 1 exp tables), then the two
-// exp tables (512 + 64 doubles), the slice ring of the inputs and of the gammas
-SLB_DEV void mean_pipe_setup(mean_pipe& P, unsigned char* smem_raw, int din, int chunk_rows, int nomax,
-                             const slb_gp_stack& gp, double** tab512, double** tab64) {
+// exp tables (512 + 64 doubles; left out when tab512 == nullptr: the fp32 screening kernel needs none),
+// the slice ring of the inputs and of the gammas.  Returns the first double behind the ring.
+SLB_DEV double* mean_pipe_setup(mean_pipe& P, unsigned char* smem_raw, int din, int chunk_rows, int nomax,
+                                const slb_gp_stack& gp, double** tab512, double** tab64) {
     P.bar = reinterpret_cast<uint64_t*>(smem_raw);
-    *tab512 = reinterpret_cast<double*>(smem_raw + 32);
-    *tab64 = *tab512 + 512;
+    P.xbuf = reinterpret_cast<double*>(smem_raw + 32);
+    if (tab512 != nullptr) {
+        *tab512 = P.xbuf;
+        *tab64 = *tab512 + 512;
+        P.xbuf = *tab64 + 64;
+    }
     P.C = chunk_rows;
     P.xstride = P.C * (din + 1);
     P.gstride = P.C * nomax;
-    P.xbuf = *tab64 + 64;
     P.gbuf = P.xbuf + 2 * P.xstride;
     P.t = 0;
     P.pf = first_factor_with_data(gp, 0);
     P.pc0 = 0;
+    return P.gbuf + 2 * P.gstride;
 }
 
 // rows per staged slice and dynamic shared memory of a kernel built on the pipeline (host)
@@ -265,8 +285,9 @@ inline int mean_chunk_rows(int din, int nomax, int budget_kb) {
     const int rows = (budget_kb * 1024) / (2 * 8 * (din + 1 + nomax));
     return rows >= 256 ? 256 : (rows & ~7);
 }
-inline size_t mean_smem_bytes(int din, int nomax, int chunk_rows) {
-    return 32 + (512 + 64) * sizeof(double) + (size_t)2 * chunk_rows * (din + 1 + nomax) * sizeof(double);
+inline size_t mean_smem_bytes(int din, int nomax, int chunk_rows, bool exp_tables = true) {
+    return 32 + (exp_tables ? (512 + 64) * sizeof(double) : 0) +
+           (size_t)2 * chunk_rows * (din + 1 + nomax) * sizeof(double);
 }
 
 // ---- fp32 screening mean (filter.cu, filter_mean32_kernel) ---------------------------------------
@@ -455,14 +476,7 @@ SLB_DEV void mean32_factor(const slb_gp_stack& gp, int f, const int* outs, const
         double gsum = 0.0;
         for (int w = 0; w < nw; ++w) gsum += B.red[q * nw + w];
         const slb_gp_output& G = gp.outputs[outs[q]];
-        double mx = 0.0;
-        if (G.prior_mean != nullptr) {
-            mx = f64mul(z[0], G.prior_mean[0]);
-#pragma unroll
-            for (int c = 1; c < DIN; ++c) mx = f64add(mx, f64mul(z[c], G.prior_mean[c]));
-            mx = f64mul(F.scale, mx);
-        }
-        mu[outs[q]] = f64add(E * dot[q], mx) / F.scale;
+        mu[outs[q]] = f64add(E * dot[q], prior_mean_term<DIN>(F, G, z)) / F.scale;
         // + the products that left the fp32 range downwards (each < 2^-126 in the scaled sum)
         dmu[outs[q]] = (1.05 * epsrel * gsum + 1.3e-26 * Mp) / fabs(F.scale) + 1e-300;
     }
@@ -471,27 +485,22 @@ SLB_DEV void mean32_factor(const slb_gp_stack& gp, int f, const int* outs, const
 template <int DIN>
 SLB_DEV void gp_mean32_staged(const slb_gp_stack& gp, const double* z, const double* zcen, double* mu,
                               double* dmu, bool& ok, mean_pipe& P, const mean32_bufs& B) {
-    for (int f = 0; f < gp.num_factors; ++f) {
-        int outs[SLB_MAX_OUT];
-        int no = 0;
-        for (int o = 0; o < gp.num_outputs; ++o)
-            if (gp.outputs[o].factor == f) outs[no++] = o;
-        switch (no) {
-        case 1: mean32_factor<DIN, 1>(gp, f, outs, z, zcen, mu, dmu, ok, P, B); break;
-        case 2: mean32_factor<DIN, 2>(gp, f, outs, z, zcen, mu, dmu, ok, P, B); break;
-        case 3: mean32_factor<DIN, 3>(gp, f, outs, z, zcen, mu, dmu, ok, P, B); break;
-        case 4: mean32_factor<DIN, 4>(gp, f, outs, z, zcen, mu, dmu, ok, P, B); break;
-        case 5: mean32_factor<DIN, 5>(gp, f, outs, z, zcen, mu, dmu, ok, P, B); break;
-        case 6: mean32_factor<DIN, 6>(gp, f, outs, z, zcen, mu, dmu, ok, P, B); break;
-        default: break;
-        }
-    }
+    for (int f = 0; f < gp.num_factors; ++f)
+        for_outputs_on_factor(gp, f, [&](auto no, const int* outs) {
+            mean32_factor<DIN, decltype(no)::value>(gp, f, outs, z, zcen, mu, dmu, ok, P, B);
+        });
 }
 
-// shared memory of the fp32 screening kernel: [0, 32) mbarriers, the fp64 slice ring, the fp32 slice,
-// the block scratch (no exp tables)
+// The fp32 screening kernel's buffers behind the pipeline's carve-up (no exp tables): the block scratch,
+// then the fp32 slice.  Device layout and host size, side by side.
+template <int DIN>
+SLB_DEV void mean32_bufs_setup(mean32_bufs& B, double* behind_pipe, int chunk_rows, int warps) {
+    B.red = behind_pipe;
+    B.xf = reinterpret_cast<float*>(B.red + 8 * warps + 8);
+    B.g = B.xf + chunk_rows * row32<DIN>::W;
+}
 inline size_t mean32_smem_bytes(int din, int nomax, int chunk_rows, int warps) {
     const int w32 = din + 1 <= 2 ? 2 : (din + 1 <= 4 ? 4 : 8);
-    return 32 + (size_t)2 * chunk_rows * (din + 1 + nomax) * sizeof(double) +
-           (size_t)chunk_rows * (w32 + nomax) * sizeof(float) + (size_t)(8 * warps + 8) * sizeof(double);
+    return mean_smem_bytes(din, nomax, chunk_rows, false) + (size_t)(8 * warps + 8) * sizeof(double) +
+           (size_t)chunk_rows * (w32 + nomax) * sizeof(float);
 }

@@ -450,7 +450,7 @@ def test_filter_covariance_expressions(din):
 
 def test_filter_five_factors_head_tables_in_global():
     """d = 5, m = 1, five distinct factors: the head stage stages four factors' tables in shared memory and
-    reads the fifth from global memory (filter_head_kernel<6>, head_group_bound<6, 8, false>)."""
+    reads the fifth from global memory (filter_head_kernel<6>, head_group_bound<6, false>)."""
     wl = _workload(5, 1, 200, [6, 6, 6, 6, 6], seed=77)
     assert wl["lyap"].sweep_descriptor().gp.num_factors == 5
     _filter_check(wl, want_stage1=64)

@@ -15,7 +15,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import bench_workloads as W  # noqa: E402
 from safe_learning_b200 import _native as nat  # noqa: E402
 
-GR, GC = 16, 16                 # tile of filter_grid_mean_kernel (csrc/filter.cu)
+GR, GC = 16, 16                 # tile of filter_grid_mean_kernel (its constants: csrc/gp_mean_grid.cuh)
 DMMA_PEAK = 33.2e12             # fp64 FLOP/s measured on H100 80GB HBM3 (DESIGN.md section 6)
 
 lib = nat.load()
