@@ -405,12 +405,23 @@ int slb_lyapunov_sweep(void* stream, const slb_sweep* cfg, int64_t idx_begin, in
  * SLB_HEAD_RANK training points (factor.Whead / Xhead) -- and decides every point whose
  * comparison `decrease < threshold` has the same outcome for all sigma in [0, bound] (guard band:
  * 1e-6 relative + the mean's error bound); the remaining points are compacted and go through the
- * full fp64 posterior (the kernel of slb_lyapunov_sweep).  Flags are identical to
- * slb_lyapunov_sweep's.
+ * full fp64 posterior (the kernel of slb_lyapunov_sweep).  Every flag equals the exact outcome wherever
+ * the decrease is farther from the threshold than the full kernel's certified error; with the refine
+ * pass's unsplit tiles the flags are identical to slb_lyapunov_sweep's, while tiles whose rows are split
+ * over several CTAs (slb_debug_refine_split) sum in another order and may differ from them within that
+ * error.
  * workspace_dev: >= slb_filter_workspace(n) bytes.  stats_dev: NULL or 4 int64 (device):
  * {decided by mean + prior bound, decided by the head-rank bound, refined by the full posterior,
  * points} accumulated over calls (the caller zeroes it). */
 int64_t slb_filter_workspace(int64_t n);
+/* diagnostics: where a filtered sweep of n <= 2^22 points (one pass) leaves its lists in workspace_dev,
+ * as byte offsets: offsets[0] the counters (uint64 [3]: entries of list A, entries of list B, list A entries
+ * of the factored grid mean without an fp64-class mean), offsets[1] list A (int64 [n]: the points stage 1 left
+ * undecided), offsets[2] list B (int64 [n]: the points the head stage left to the full posterior).  Indices
+ * are relative to idx_begin, in no particular order; only the first counters[0] / counters[1] entries are
+ * written.  The lists describe the LAST pass of the last call only.  Returns non-zero for n < 0,
+ * n > 2^22 or a NULL offsets. */
+int slb_debug_filter_lists(int64_t n, int64_t* offsets);
 /* which first stage slb_lyapunov_sweep_filtered runs for this configuration: 32 = the fp32 screening
  * kernel (plain RBF factors, quadratic V on at most four outputs, constant / abs-linear L_V, tables fit
  * the head stage's shared memory) with an fp64 mean only for the points its error box leaves open;

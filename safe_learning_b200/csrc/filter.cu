@@ -1153,6 +1153,17 @@ int64_t slb_filter_workspace(int64_t n) {
     return WS_HEAD + n * (int64_t)(2 * sizeof(int64_t) + sizeof(filter_side));
 }
 
+int slb_debug_filter_lists(int64_t n, int64_t* offsets) {
+    SLB_CHECK(offsets != nullptr, "slb_debug_filter_lists: null offsets");
+    SLB_CHECK(n >= 0 && n <= CHUNK, "slb_debug_filter_lists: n %lld outside [0, %lld] (one pass)", (long long)n,
+              (long long)CHUNK);
+    // the layout slb_lyapunov_sweep_filtered carves out of its workspace (cap = n for one pass)
+    offsets[0] = 0;
+    offsets[1] = WS_HEAD;
+    offsets[2] = WS_HEAD + n * (int64_t)sizeof(int64_t);
+    return 0;
+}
+
 int slb_lyapunov_sweep_filtered(void* stream, const slb_sweep* cfg, int64_t idx_begin,
                                 int64_t idx_end, uint8_t* negative_dev, double* values_dev,
                                 void* workspace_dev, int64_t* stats_dev) {

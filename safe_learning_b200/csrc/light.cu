@@ -7,6 +7,7 @@
 #include "common.cuh"
 #include "bellman.cuh"
 
+#include <float.h>
 #include <stdarg.h>
 #include <stdio.h>
 #include <string.h>
@@ -777,8 +778,13 @@ pivoted_subset_kernel(const double* __restrict__ K, int M, int r, int64_t* __res
             for (int j = 0; j < t; ++j) col = fma(-li[j], s_prow[j], col);
             col *= inv;
             low[(size_t)i * r + t] = col;
-            const double d = diag[i];
-            diag[i] = (i == piv || d == -INFINITY) ? -INFINITY : d - col * col;
+            // -inf marks the chosen points only: once the kernel's rank is exhausted the remaining diagonal
+            // is rounding noise and col may overflow, so an unchosen point is clamped to the lowest finite
+            // value (a repeated pick would make the "subset" count one observation twice and its variance
+            // bound fall below the full posterior's)
+            const double d = diag[i], nd = d - col * col;
+            diag[i] = (i == piv || d == -INFINITY) ? -INFINITY
+                      : nd >= -DBL_MAX ? nd : -DBL_MAX;
         }
         __syncthreads();
     }
