@@ -384,7 +384,8 @@ SLB_DEV void tri_lookup(const slb_function& f, const double* xin, double* out, i
     grid_index_to_state(g, simp[0] + corner, origin);
     for (int c = 0; c < d; ++c) {
         double xc = xin[c];
-        if (f.flags & SLB_FLAG_PROJECT) xc = fmin(fmax(xc, g.offset[c]), g.upper[c]);
+        // clip as tf.clip_by_value does: a NaN coordinate stays NaN (fmin / fmax would return the limit)
+        if (f.flags & SLB_FLAG_PROJECT) xc = xc < g.offset[c] ? g.offset[c] : (xc > g.upper[c] ? g.upper[c] : xc);
         off[c] = f64sub(xc, origin[c]);
     }
     double w[SLB_MAX_DIM + 1];
@@ -404,7 +405,14 @@ SLB_DEV void tri_lookup(const slb_function& f, const double* xin, double* out, i
     }
     if (f.flags & SLB_FLAG_GRADIENT) {
         // Triangulation.gradient (:1260-1326): weights[k][0] = -sum_c H[k][c], weights[k][1 + c] =
-        // H[k][c]; d/dx_k = sum_v weights[k][v] * value[vertex v]   (one output column)
+        // H[k][c]; d/dx_k = sum_v weights[k][v] * value[vertex v]   (one output column).  A point with
+        // a NaN coordinate has no simplex, so its gradient is NaN (DESIGN.md §3.2).
+        bool nan = false;
+        for (int c = 0; c < d; ++c) nan = nan || xin[c] != xin[c];
+        if (nan) {
+            for (int k = 0; k < d; ++k) out[k] = __longlong_as_double(0x7ff8000000000000ll);
+            return;
+        }
         for (int k = 0; k < d; ++k) {
             double hs = H[k * d];
             for (int c = 1; c < d; ++c) hs = f64add(hs, H[k * d + c]);

@@ -59,6 +59,14 @@ def _triangulation_of(value_function):
     return base
 
 
+def min_weight_of_stats(slot):
+    """The smallest operator weight from slot 0 of the value statistics (slb200.h ``SLB_VALUE_STATS``): the
+    complement of the weight's order-preserving key (``value_key``, value_opt.cu)."""
+    key = ~np.uint64(slot)
+    bits = (key & np.uint64(0x7fffffffffffffff)) if key >> np.uint64(63) else ~key
+    return float(np.array([bits], dtype=np.uint64).view(np.float64)[0])
+
+
 class PolicyIteration(object):
     """See ``reinforcement_learning.py:26-63`` for the parameters."""
 
@@ -353,12 +361,10 @@ class PolicyIteration(object):
                   "slb_value_solve")
         host = torch.cat((values, stats.view(torch.float64))).cpu().numpy()  # the one sync
         raw = host[n:].view(np.uint64)
-        key = ~raw[0]                                      # order-preserving key of the min weight
-        min_weight = (key & np.uint64(0x7fffffffffffffff)) if key >> np.uint64(63) else ~key
         info = {"status": int(raw[7]), "iterations": int(raw[4]),
                 "delta": float(host[n + 5]), "bound": float(host[n + 6]),
                 "rho": float(host[n + 1]), "repaired_rows": int(raw[2]), "tier": int(raw[8]),
-                "min_weight": float(np.array([min_weight], dtype=np.uint64).view(np.float64)[0])}
+                "min_weight": min_weight_of_stats(raw[0])}
         self.last_solve = info
         out = host[:n].reshape(n, 1).copy()
         if info["status"] == nat.VALUE_CONVERGED:

@@ -50,6 +50,13 @@ KINDS = ["oracle", pytest.param("product", marks=pytest.mark.gpu)]
 
 
 # ------------------------------------------------------------------ grid + triangulation
+HIGH_DIM = ("h4", "h5", "h6")          # triangulation_high_dim.npz (make_golden_triangulation_high_dim.py)
+
+
+def _one_at_a_time(tri, pts):
+    return np.vstack([tri(p[None, :]) for p in pts])
+
+
 @pytest.mark.parametrize("kind", KINDS)
 def test_grid_and_triangulation_fixture(kind):
     ns, _, _ = backend(kind)
@@ -79,6 +86,30 @@ def test_grid_and_triangulation_fixture(kind):
                 assert_allclose(got, want, rtol=1e-12, atol=1e-12)
             elif project or d <= 2:
                 assert_allclose(tri(outside), want, rtol=1e-12, atol=1e-12)
+    # d = 4..6: the same comparisons; every vertex and a point beyond each of the 2^d corner patterns
+    # (the corner_simplex table) were queried alone, and vertex queries are order dependent upstream
+    # (DESIGN.md §3.2 Q6), so the product is held to them only through the exact reference
+    # (tests/test_triangulation_reference_host.py, tests/test_gpu_triangulation_shapes.py)
+    fix = load("triangulation_high_dim.npz")
+    for tag in HIGH_DIM:
+        grid = ns.GridWorld(fix[tag + "_limits"], fix[tag + "_num"])
+        assert_array_equal(grid.all_points, fix[tag + "_vertices"])
+        for project in (False, True):
+            tri = ns.Triangulation(grid, fix[tag + "_vals"], project=project)
+            key = tag + ("_proj" if project else "_noproj")
+            tables = tri if kind == "oracle" else tri.tri
+            assert_array_equal(tables.unit_simplices, fix[tag + "_unit_simplices"])
+            assert_array_equal(tables.hyperplanes, fix[tag + "_hyperplanes"])
+            for group in ("inside", "faces", "corners", "outside", "vertices"):
+                pts, want = fix[tag + "_" + group], fix[key + "_" + group + "_value"]
+                if kind == "oracle":
+                    assert_allclose(_one_at_a_time(tri, pts), want, rtol=1e-12, atol=1e-12)
+                elif group == "outside" and not project:
+                    clipped = (pts < grid.limits[:, 0]) | (pts > grid.limits[:, 1])
+                    every = clipped.all(axis=1)
+                    assert_allclose(tri(pts[every]), want[every], rtol=1e-12, atol=1e-12)
+                elif group != "vertices":
+                    assert_allclose(tri(pts), want, rtol=1e-12, atol=1e-12)
 
 
 # ------------------------------------------------------------------ GP posterior
@@ -207,6 +238,15 @@ def test_triangulation_gradient_fixture(kind):
         tri = ns.Triangulation(grid, fix[tag + "_vals"])
         assert_allclose(tri.gradient(fix[tag + "_inside"]), fix[tag + "_gradient"], rtol=1e-12,
                         atol=1e-13)
+    hfix = load("triangulation_high_dim.npz")
+    for tag in HIGH_DIM:
+        grid = ns.GridWorld(hfix[tag + "_limits"], hfix[tag + "_num"])
+        tri = ns.Triangulation(grid, hfix[tag + "_gvals"])
+        for group in ("inside", "faces", "corners"):      # the oracle's scipy walk: one query at a time
+            pts = hfix[tag + "_" + group]
+            got = (np.vstack([tri.gradient(p[None, :]) for p in pts]) if kind == "oracle"
+                   else tri.gradient(pts))
+            assert_allclose(got, hfix[tag + "_" + group + "_gradient"], rtol=1e-12, atol=1e-13)
     qgrid = ns.GridWorld([[-1, 1], [-1, 1]], [25, 21])
     qtri = ns.Triangulation(qgrid, fix["quirk_vals"])
     missed = np.abs(fix["quirk_at_vertices"] - fix["quirk_vals"]).ravel() > 1e-9

@@ -140,12 +140,16 @@ def test_small_functions_bit_exact(sl):
                        O.LinearSystem(A)(x))
 
 
-@pytest.mark.parametrize("dims,project", [(1, False), (2, False), (2, True), (3, True)])
+TRI_LIMITS = [[-1.0, 1.5], [0.0, 2.0], [-0.5, 0.5], [-1.2, 0.8], [0.3, 1.1], [-2.0, -0.5]]
+
+
+@pytest.mark.parametrize("dims,project", [(1, False), (2, False), (2, True), (3, True), (4, True), (5, True),
+                                          (6, True)])
 def test_triangulation_vs_oracle(sl, dims, project):
     """functions.py:1103-1158, 1473-1499; reference tests test_functions.py:457-701."""
     rng = np.random.default_rng(dims)
-    limits = [[-1.0, 1.5], [0.0, 2.0], [-0.5, 0.5]][:dims]
-    num = [5, 4, 3][:dims]
+    limits = TRI_LIMITS[:dims]
+    num = [5, 4, 3, 3, 3, 2][:dims]
     g_gpu, g_cpu = sl.GridWorld(limits, num), O.GridWorld(limits, num)
     vals = rng.normal(size=(g_cpu.nindex, 2))
     t_gpu = sl.Triangulation(g_gpu, vals, project=project)
@@ -153,7 +157,11 @@ def test_triangulation_vs_oracle(sl, dims, project):
     lo, hi = np.array(limits)[:, 0], np.array(limits)[:, 1]
     span = 0.3 * (hi - lo)
     pts = rng.uniform(lo - span, hi + span, size=(2000, dims))
-    pts = np.vstack((pts, g_cpu.all_points))                 # vertices: shared-face lookups
+    # vertices: shared-face lookups.  From d = 5 on, exact-vertex queries hit the Q6 rounding (DESIGN.md
+    # §3.2) where the oracle's batch walk and the library's first fit pick different extrapolating
+    # simplices; tests/test_gpu_triangulation_shapes.py holds them to the exact reference instead
+    if dims <= 4:
+        pts = np.vstack((pts, g_cpu.all_points))
     got = t_gpu(pts)
     # A non-projected query outside the grid in EVERY coordinate is clipped onto a unit-cell
     # corner where several simplices meet; scipy's find_simplex walks from the previous query's
@@ -167,13 +175,13 @@ def test_triangulation_vs_oracle(sl, dims, project):
     assert_allclose(t_gpu(inside), t_cpu(inside), rtol=1e-13, atol=1e-13)
 
 
-@pytest.mark.parametrize("dims", [1, 2, 3])
+@pytest.mark.parametrize("dims", [1, 2, 3, 4, 5, 6])
 def test_triangulation_gradient_vs_oracle(sl, dims):
     """Triangulation.gradient (functions.py:1260-1326) and max |.| over it -- the Lipschitz lambda
     of examples/inverted_pendulum.ipynb cell 14 -- incl. queries on vertices and outside."""
     rng = np.random.default_rng(dims)
-    limits = [[-1.0, 1.5], [0.0, 2.0], [-0.5, 0.5]][:dims]
-    num = [7, 5, 4][:dims]
+    limits = TRI_LIMITS[:dims]
+    num = [7, 5, 4, 3, 3, 2][:dims]
     g_gpu, g_cpu = sl.GridWorld(limits, num), O.GridWorld(limits, num)
     vals = rng.normal(size=(g_cpu.nindex, 1))
     lo, hi = g_cpu.limits[:, 0], g_cpu.limits[:, 1]

@@ -20,6 +20,8 @@ pytestmark = pytest.mark.gpu
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden",
                       "triangulation_param_derivative.npz")
+GOLDEN_HIGH_DIM = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden",
+                               "triangulation_high_dim.npz")
 T64 = torch.float64
 CUDA = "cuda"
 
@@ -97,17 +99,26 @@ def test_all_points_on_one_vertex():
 
 
 # ---------------------------------------------------------------- 2. parameter_derivative vs the reference
-def test_parameter_derivative_matches_reference_fixture():
+def _fixture_cases():
+    """(fixture, key, points) of triangulation_param_derivative.npz (d = 1..3) and of
+    triangulation_high_dim.npz (d = 4..6, whose points are stored once per grid and group)."""
     fix = np.load(GOLDEN)
-    keys = sorted(k[:-len("_points")] for k in fix.files if k.endswith("_points"))
+    for key in sorted(k[:-len("_points")] for k in fix.files if k.endswith("_points")):
+        yield fix, key, fix[key + "_points"]
+    high = np.load(GOLDEN_HIGH_DIM)
+    for key in sorted(k[:-len("_cols")] for k in high.files if k.endswith("_cols")):
+        tag, _, group = key.split("_", 2)
+        yield high, key, high[tag + "_" + group]
+
+
+def test_parameter_derivative_matches_reference_fixture():
     report = {}
-    for key in keys:
+    for fix, key, pts in _fixture_cases():
         tag, proj, group = key.split("_", 2)
         grid = sl.GridWorld(fix[tag + "_limits"], fix[tag + "_num"])
         rng = np.random.default_rng(1)
         v = rng.normal(size=(grid.nindex, 1))
         tri = sl.Triangulation(grid, v, project=proj == "proj")
-        pts = fix[key + "_points"]
         pd = tri.tri.parameter_derivative(pts)
         n, nsimp = fix[key + "_cols"].shape
         assert pd.shape == (n, grid.nindex)

@@ -71,8 +71,10 @@ def library_simplices(tri, x):
         take = ~done & (wmin > best_min)
         best[take], best_min[take] = s, wmin[take]
         done |= wmin >= -W_TOL
-    if d > 1 and all_clipped.any():
-        best[all_clipped] = tri.find_simplex(x[all_clipped]) % tri.nsimplex_unit
+    # Qhull's simplex of an isolated query (the library's corner_simplex table): within one call scipy's
+    # walk starts from the previous query's simplex, so the points are asked one at a time
+    for i in np.flatnonzero(all_clipped) if d > 1 else ():
+        best[i] = tri.find_simplex(x[i:i + 1])[0] % tri.nsimplex_unit
     return best
 
 
