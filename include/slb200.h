@@ -320,6 +320,12 @@ int         slb_debug_phase_timing(void* buffer_dev);
  * fp64 means of the round, final decision, exit}, and [132][0] to the time the last warp of the first
  * stage left (tools/head_stage_timeline.py); pass NULL to switch it off (default) */
 int         slb_debug_head_timing(void* buffer_dev);
+/* diagnostics: when buffer_dev != NULL (uint64 [tiles][8], zeroed by the caller; tiles = the launch's
+ * 16 x 16 tiles), every later filtered sweep whose stage 1 runs the factored grid mean raises entry [t][m]
+ * to the %globaltimer (ns) at which the last warp of tile t's CTA passed mark m = {entry, prologue done,
+ * work items 0, 1, 2 and 3 (and later) done, means done, exit} (tools/stage1_timeline.py); pass NULL to
+ * switch it off (default) */
+int         slb_debug_stage1_timing(void* buffer_dev);
 /* Records an event (owned by the library, one per device) on `stream` that every later launch reading
  * the packed factors (slb_gp_factor.Wpack: the full posterior of slb_gp_predict / slb_lyapunov_sweep /
  * slb_lyapunov_points and the refine pass of slb_lyapunov_sweep_filtered) waits for on ITS stream.  A

@@ -107,6 +107,7 @@ struct filter_args {
     double* probe_mu;                  // slb_debug_screening_probe: nullptr or [n, D] screened means ...
     double* probe_dm;                  // ... and their certified error bounds (inf: point left to fp64)
     unsigned long long* timing;        // slb_debug_head_timing: nullptr or [HEAD_CTAS + 1][8] %globaltimer
+    unsigned long long* timing1;       // slb_debug_stage1_timing: nullptr or [tiles][8] %globaltimer
     int head_schedule;                 // head stage: 0 chosen from the list length, 1 split, 2 round loop
 };
 
@@ -120,6 +121,15 @@ SLB_DEV void timing_mark(const filter_args& a, int slot) {
     atomicMax(a.timing + slot, t);
 }
 SLB_DEV void head_mark(const filter_args& a, int mark) { timing_mark(a, blockIdx.x * 8 + mark); }
+// slb_debug_stage1_timing: the same, per tile of the factored grid mean (row blockIdx.x); work item k
+// (one factor and regime) marks S1_ITEM + min(k, 3)
+enum { S1_ENTRY, S1_PROLOGUE, S1_ITEM, S1_MEANS = S1_ITEM + 4, S1_EXIT };
+SLB_DEV void stage1_mark(const filter_args& a, int mark) {
+    if (a.timing1 == nullptr || (threadIdx.x & 31) != 0) return;
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    atomicMax(a.timing1 + blockIdx.x * 8 + mark, t);
+}
 
 // outcome for err_j = beta_j sigma_j with sigma_j in [0, shi_j]:  +1 decided negative (True),
 // 0 decided not negative (False), -1 undecided.  term_j = L_V(mu)_j beta_j sigma_j lies between 0 and
@@ -400,13 +410,22 @@ filter_mean32_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a)
 }
 
 // ---- stage 1, factored grid mean (gp_mean_grid.cuh): one CTA per GR x GC tile of a 2-D grid -------------
+// Thread t owns point t of the tile (row-major: the flag and V(x) stores are contiguous along the grid's
+// axis 1) in the prologue and the decision; in between, the tile's work items (factor, regime) alternate
+// between the two warp groups, which meet the points' z / regime and leave their mu / dm in shared memory.
 template <int DIN>
 __global__ void __launch_bounds__(GT, 2)
 filter_grid_mean_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
     static_assert(DIN == 3, "the factored grid mean is written for z = [x0, x1, u]");
+    stage1_mark(a, S1_ENTRY);
     extern __shared__ __align__(16) unsigned char smem_raw[];
     double* smem = reinterpret_cast<double*>(smem_raw);
-    double* tab = smem + GSMEM_PRE_TAB;                                  // [512] of exp_neg_fast
+    double* tab = smem + GSMEM_TAB;                                      // [512] of exp_neg_fast
+    double* zs = smem + GSMEM_Z;
+    double* mus = smem + GSMEM_MU;
+    double* dms = smem + GSMEM_DM;
+    int* present = reinterpret_cast<int*>(smem + GSMEM_REG);
+    int8_t* regs = reinterpret_cast<int8_t*>(present + GT / 32);
     for (int i = threadIdx.x; i < 512; i += GT) tab[i] = g_exp_tables[i];   // visible after the first barrier
     prefetch_descriptor_operands(cfg);
     // the training rows and weights every tile reads chunk by chunk: into L2 while the prologue runs
@@ -420,64 +439,86 @@ filter_grid_mean_kernel(const __grid_constant__ slb_sweep cfg, const filter_args
         for (size_t off = (size_t)threadIdx.x * 128; off < bytes; off += (size_t)GT * 128)
             asm volatile("prefetch.global.L2 [%0];" ::"l"(reinterpret_cast<const char*>(cfg.gp.outputs[o].gamma_f) + off));
     }
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int64_t n0 = cfg.grid.num_points[0], n1 = cfg.grid.num_points[1];
     const int64_t ntc = (n1 + GC - 1) / GC;
     const int64_t row0 = a.idx_begin / n1 + (int64_t)(blockIdx.x / ntc) * GR;
     const int64_t col0 = (int64_t)(blockIdx.x % ntc) * GC;
     const slb_function& pol = cfg.policy;
 
-    // ---- the thread's two points (its lanes' C-fragment positions): x, V(x), threshold(x), u = policy(x)
-    const int64_t gi = row0 + (warp / GCB) * 8 + (lane >> 2);
-    double z[2][3], vx[2], thr[2];
-    bool valid[2], sane[2];
-    int64_t rel[2];
-    int reg[2];
-    const double ulo = (pol.flags & SLB_FLAG_SCALE) ? f64mul(pol.lower, pol.out_scale) : pol.lower;
-    const double uhi = (pol.flags & SLB_FLAG_SCALE) ? f64mul(pol.upper, pol.out_scale) : pol.upper;
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-        const int64_t gk = col0 + (warp % GCB) * 8 + 2 * (lane & 3) + h;
-        const int64_t flat = gi * n1 + gk;
-        valid[h] = gi < n0 && gk < n1 && flat >= a.idx_begin && flat < a.idx_begin + a.n;
-        rel[h] = valid[h] ? flat - a.idx_begin : 0;   // every thread stays for the block barriers
+    // ---- the thread's point: x, V(x), threshold(x), u = policy(x); z and the regime go to shared memory
+    const int pt = threadIdx.x;
+    const int64_t gi = row0 + pt / GC, gk = col0 + pt % GC;
+    const int64_t flat = gi * n1 + gk;
+    const bool valid = gi < n0 && gk < n1 && flat >= a.idx_begin && flat < a.idx_begin + a.n;
+    const int64_t rel = valid ? flat - a.idx_begin : 0;   // every thread stays for the block barriers
+    double vx, thr;
+    int reg;
+    bool sane;
+    {
         double x[SLB_MAX_IN];
-        sane[h] = stage1_point<DIN>(cfg, a.idx_begin + rel[h], x, &vx[h], &thr[h]);
+        sane = stage1_point<DIN>(cfg, a.idx_begin + rel, x, &vx, &thr);
 #pragma unroll
-        for (int c = 0; c < 3; ++c) z[h][c] = x[c];
+        for (int c = 0; c < 3; ++c) zs[pt * 3 + c] = x[c];
         // the regime is the clip the policy computed: saturated points carry the constant itself
-        reg[h] = !(valid[h] && sane[h]) ? -1
-                 : (pol.flags & SLB_FLAG_SATURATE) && z[h][2] == ulo ? 0
-                 : (pol.flags & SLB_FLAG_SATURATE) && z[h][2] == uhi ? 1 : 2;
+        const double ulo = (pol.flags & SLB_FLAG_SCALE) ? f64mul(pol.lower, pol.out_scale) : pol.lower;
+        const double uhi = (pol.flags & SLB_FLAG_SCALE) ? f64mul(pol.upper, pol.out_scale) : pol.upper;
+        reg = !(valid && sane) ? -1
+              : (pol.flags & SLB_FLAG_SATURATE) && x[2] == ulo ? 0
+              : (pol.flags & SLB_FLAG_SATURATE) && x[2] == uhi ? 1 : 2;
     }
+    regs[pt] = (int8_t)reg;
+#pragma unroll
+    for (int o = 0; o < GNO; ++o) { mus[pt * GNO + o] = 0.0; dms[pt * GNO + o] = f64_inf(); }
+    const unsigned rbits = __reduce_or_sync(0xffffffffu, reg >= 0 ? 1u << reg : 0u);
+    if ((threadIdx.x & 31) == 0) present[threadIdx.x >> 5] = (int)rbits;
+    __syncthreads();                              // z, regimes and the exp table visible
+    stage1_mark(a, S1_PROLOGUE);
 
-    // ---- posterior means, factor by factor
-    double mu[2][GNO], dm[2][GNO];
+    // ---- posterior means: the work items (factor ascending, then regime), item k on group k % GG
+    int regimes = 0;
 #pragma unroll
-    for (int h = 0; h < 2; ++h)
-#pragma unroll
-        for (int o = 0; o < GNO; ++o) { mu[h][o] = 0.0; dm[h][o] = f64_inf(); }
-    for (int f = 0; f < cfg.gp.num_factors; ++f)
-        for_outputs_on_factor<GNO>(cfg.gp, f, [&](auto no, const int* outs) {
-            grid_mean_factor<decltype(no)::value>(cfg, f, outs, smem, tab, row0, col0, z, reg, mu, dm);
-        });
-
-    // ---- per point: the comparison over mu +- dm and sigma_j in [0, prior sigma_j] (as filter_mean32_kernel)
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-        double m[SLB_MAX_OUT], d[SLB_MAX_OUT];
-#pragma unroll
-        for (int j = 0; j < SLB_MAX_OUT; ++j) {
-            m[j] = j < GNO ? mu[h][j] : 0.0;
-            d[j] = j < GNO ? dm[h][j] : 0.0;
+    for (int w = 0; w < GT / 32; ++w) regimes |= present[w];
+    const int grp = threadIdx.x / GGT;
+    int item = 0;
+    for (int f = 0; f < cfg.gp.num_factors; ++f) {
+        int outs[SLB_MAX_OUT], no = 0;                // the outputs on factor f (none: no item)
+        for (int o = 0; o < cfg.gp.num_outputs; ++o)
+            if (cfg.gp.outputs[o].factor == f) outs[no++] = o;
+        if (no == 0 || no > GNO) continue;
+        for (int r = 0; r < 3; ++r) {
+            if (!((regimes >> r) & 1)) continue;
+            if (item % GG == grp) {
+                // four outputs in two passes of two: four accumulator sets do not fit 128 registers.  Every
+                // output's sum is its own, so its mean is the same in either pass.
+                const int np = no == 4 ? 2 : no;
+                for (int q0 = 0; q0 < no; q0 += np) {
+                    double* gsm = smem + grp * GGRP;
+                    if (np == 1) grid_mean_item<1>(cfg, f, r, outs + q0, gsm, tab, row0, col0, zs, regs, mus, dms);
+                    else if (np == 2) grid_mean_item<2>(cfg, f, r, outs + q0, gsm, tab, row0, col0, zs, regs, mus, dms);
+                    else grid_mean_item<3>(cfg, f, r, outs + q0, gsm, tab, row0, col0, zs, regs, mus, dms);
+                }
+                stage1_mark(a, S1_ITEM + min(item, 3));
+            }
+            ++item;
         }
-        filter_side t;
-        t.thr = thr[h];
-#pragma unroll
-        for (int c = 0; c < DIN; ++c) t.z[c] = z[h][c];
-        stage1_screened_finish<DIN>(cfg, a, valid[h], sane[h], rel[h], t, vx[h], m, d);
     }
+    __syncthreads();                              // every item's mu / dm visible
+    stage1_mark(a, S1_MEANS);
+
+    // ---- the comparison over mu +- dm and sigma_j in [0, prior sigma_j] (as filter_mean32_kernel)
+    double m[SLB_MAX_OUT], d[SLB_MAX_OUT];
+#pragma unroll
+    for (int j = 0; j < SLB_MAX_OUT; ++j) {
+        m[j] = j < GNO ? mus[pt * GNO + j] : 0.0;
+        d[j] = j < GNO ? dms[pt * GNO + j] : 0.0;
+    }
+    filter_side t;
+    t.thr = thr;
+#pragma unroll
+    for (int c = 0; c < DIN; ++c) t.z[c] = zs[pt * 3 + c];
+    stage1_screened_finish<DIN>(cfg, a, valid, sane, rel, t, vx, m, d);
     timing_mark(a, HEAD_CTAS * 8);
+    stage1_mark(a, S1_EXIT);
 }
 
 // ---- stage 2: variance given the head subset, one warp per HP undecided points ---------------------
@@ -992,6 +1033,7 @@ filter_head_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
 double* g_probe_mu = nullptr;          // slb_debug_screening_probe
 double* g_probe_dm = nullptr;
 unsigned long long* g_head_timing = nullptr;   // slb_debug_head_timing
+unsigned long long* g_stage1_timing = nullptr; // slb_debug_stage1_timing
 int g_filter_stages = 3;               // slb_debug_filter_stages: bit 0 head stage, bit 1 refine pass,
                                        // bit 2 forces the fp64 mean stage (no fp32 screening), bit 3 /
                                        // bit 4 force the head stage's split schedule / round loop,
@@ -1078,10 +1120,15 @@ int launch_filter(cudaStream_t st, const slb_sweep& cfg, const filter_args& a) {
                                       cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
         SLB_CUDA(cudaFuncSetAttribute(filter_head_kernel<DIN>,
                                       cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        if constexpr (DIN == 3)
+        if constexpr (DIN == 3) {
             SLB_CUDA(cudaFuncSetAttribute(filter_grid_mean_kernel<DIN>,
                                           cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           (int)grid_mean_smem_bytes()));
+            // all of the unified L1 / shared memory as shared: two 111 KB CTAs per SM
+            SLB_CUDA(cudaFuncSetAttribute(filter_grid_mean_kernel<DIN>,
+                                          cudaFuncAttributePreferredSharedMemoryCarveout,
+                                          (int)cudaSharedmemCarveoutMaxShared));
+        }
         if (device >= 0 && device < 64) configured[device].store(true, std::memory_order_release);
     }
     const int64_t blocks = (a.n + FT - 1) / FT;
@@ -1142,6 +1189,11 @@ int slb_debug_screening_probe(double* mu_dev, double* dm_dev) {
 
 int slb_debug_head_timing(void* buffer_dev) {
     g_head_timing = static_cast<unsigned long long*>(buffer_dev);
+    return 0;
+}
+
+int slb_debug_stage1_timing(void* buffer_dev) {
+    g_stage1_timing = static_cast<unsigned long long*>(buffer_dev);
     return 0;
 }
 
@@ -1219,6 +1271,7 @@ int slb_lyapunov_sweep_filtered(void* stream, const slb_sweep* cfg, int64_t idx_
     a.probe_mu = g_probe_mu;
     a.probe_dm = g_probe_dm;
     a.timing = g_head_timing;
+    a.timing1 = g_stage1_timing;
     for (int64_t off = 0; off < n_all; off += CHUNK) {
         const int64_t n = n_all - off < CHUNK ? n_all - off : CHUNK;
         SLB_CUDA(cudaMemsetAsync(a.counts, 0, 64 + SLB_SPLIT_TICKET_BYTES, st));

@@ -21,9 +21,12 @@
 // The tables run on the uniform offsets xi_i = (i - 8) h0, h0 = unit0 / l0 (eta likewise): a column of
 // E0 is g^(i - 8), g = exp(-h0 p_j), from two exponentials and 15 products -- 5 M exponentials per tile
 // and regime (two per table column, one weight) instead of GR GC M -- and GR GC M fp64 FMAs in DMMA
-// m8n8k4 (warp w: the 8 x 8 block (w / GCB, w % GCB) of the tile; its C fragment is its lanes' points).
-// A tile computes every regime its points are in (saturated low / high, affine), each point keeps its
-// own.  The summation order is fixed: two runs are bit-identical.
+// m8n8k4 (warp w of a group: the 8 x 8 block (w / GCB, w % GCB) of the tile; its C fragment is two points
+// of each lane).  A tile computes every regime its points are in (saturated low / high, affine), each
+// point keeps its own.  Its work items are its (factor, regime) pairs -- factors ascending, regimes 0, 1, 2
+// as its points need them -- dealt in turn to the CTA's two warp groups, each with its own tables and
+// named barrier: an item's arithmetic does not depend on the group that runs it, and the summation order
+// within an item is fixed, so two runs are bit-identical.
 // Certified bound (u = 2^-53, rho = max|xi| sqrt(1 + alpha^2) + max|eta| sqrt(1 + beta^2) >= |w - cw|,
 // s_j = |D_j|, Sg = gamma_l1 >= sum_j |gamma_oj|):
 //   each term: the weight and Q from one exp_neg_fast each (EPS_K relative; its reduction x = n ln2 / 512
@@ -47,8 +50,10 @@
 // constant leaves its points to the fp64 route (dm = inf), like points the prologue finds insane.
 constexpr int GR = 16, GC = 16;        // grid rows (axis 0) x columns (axis 1, contiguous) per CTA tile
 constexpr int GCB = GC / 8;            // column blocks
-constexpr int GT = GR * GC / 2;        // threads: one warp per 8 x 8 block, two points per thread (two CTAs
-                                       // per SM: one's barriers and round trips hide behind the other)
+constexpr int GG = 2;                  // warp groups per CTA: the tile's work items alternate between them
+constexpr int GGT = GR * GC / 2;       // threads per group: one warp per 8 x 8 block, two points per thread
+constexpr int GT = GG * GGT;           // threads per CTA: one per point in the prologue and the decision (two
+                                       // CTAs per SM: one's barriers and round trips hide behind the other)
 constexpr int GJ = 128;                // training rows per chunk of the tables
 constexpr int GNO = 4;                 // outputs per factor (screening_applicable: at most 4 outputs)
 constexpr double GRID_RHO_MAX = 12.0;
@@ -56,26 +61,43 @@ constexpr double GRID_K_DROP = 600.0;
 constexpr int GFS = 36;                // doubles per fragment (32 used): the recurrence's column stores hit
                                        // every bank pair once, the contraction's loads stay contiguous
 constexpr int GTAB = (GR / 8) * (GJ / 4) * GFS;   // one table of a chunk, in fragments
-constexpr int GSMEM_PRE_TAB = 2 * GTAB + GNO * GJ + 2 * GJ + 2 * (GR + GC);   // doubles before the exp table
+constexpr int GGRP = 2 * GTAB + GNO * GJ + 2 * GJ + 2 * (GR + GC);   // doubles of one group's item state
+// the CTA's dynamic shared memory, in doubles: [GG][GGRP] the groups' item state, [512] the exp table,
+// [GR GC][3] z of the tile's points, [GR GC][GNO] their means mu and bounds dm, then [GT / 32] ints: the
+// regimes present in each warp's points, and [GR GC] bytes: the points' regimes.  111.3 KB: two CTAs per SM
+// with their 1 KB of static shared memory and 1 KB reserved each (228 KB).
+constexpr int GSMEM_TAB = GG * GGRP;
+constexpr int GSMEM_Z = GSMEM_TAB + 512;
+constexpr int GSMEM_MU = GSMEM_Z + GR * GC * 3;
+constexpr int GSMEM_DM = GSMEM_MU + GR * GC * GNO;
+constexpr int GSMEM_REG = GSMEM_DM + GR * GC * GNO;
 static_assert(GR == 16 && GC == 16, "the recurrence runs 8 steps each way from the tile's centre");
+static_assert(GT == GR * GC, "one point per thread in the prologue and the decision");
+static_assert(GGT == GJ, "one training row per group thread and chunk");
 
 inline size_t grid_mean_smem_bytes() {
-    return (size_t)(GSMEM_PRE_TAB + 512) * sizeof(double);
+    return (size_t)GSMEM_REG * sizeof(double) + (GT / 32) * sizeof(int) + GR * GC;
 }
 
-// one factor with NO outputs (compile-time: accumulators in registers) for the tile; writes mu / dm of
-// the thread's two points for the factor's outputs
+// the barrier of warp group grp alone (barrier 0 is __syncthreads'; constant ids: three barriers in all)
+SLB_DEV void grid_group_sync(int grp) {
+    if (grp == 0) asm volatile("bar.sync 1, %0;" ::"n"(GGT) : "memory");
+    else asm volatile("bar.sync 2, %0;" ::"n"(GGT) : "memory");
+}
+
+// one work item of the tile -- factor f with NO outputs (compile-time: accumulators in registers), regime r
+// -- on the calling thread's warp group (its item state at gsm); writes mu / dm [point][output] of the
+// tile's points in regime r for the factor's outputs.  z / reg: [point] as the prologue left them.
 template <int NO>
-SLB_DEV void grid_mean_factor(const slb_sweep& cfg, int f, const int* outs, double* smem, const double* tab,
-                              int64_t row0,
-                              int64_t col0, const double (*z)[3], const int* reg, double (*mu)[GNO],
-                              double (*dm)[GNO]) {
+SLB_DEV void grid_mean_item(const slb_sweep& cfg, int f, int r, const int* outs, double* gsm, const double* tab,
+                            int64_t row0, int64_t col0, const double* z, const int8_t* reg, double* mu, double* dm) {
     const slb_gp_factor& F = cfg.gp.factors[f];
     const slb_grid& g = cfg.grid;
     const slb_function& pol = cfg.policy;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int grp = threadIdx.x / GGT, gt = threadIdx.x % GGT;
+    const int lane = gt & 31, warp = gt >> 5;
     const int rb = warp / GCB, cb = warp % GCB;
-    double* e0f = smem;                        // [GR / 8][J / 4][GFS]: DMMA A fragments
+    double* e0f = gsm;                         // [GR / 8][J / 4][GFS]: DMMA A fragments
     double* e1f = e0f + GTAB;                  // [GC / 8][J / 4][GFS]: DMMA B fragments
     double* wg = e1f + GTAB;                   // [NO][GJ] gamma_oj exp(-|D_j|^2 / 2)
     double* pq = wg + GNO * GJ;                // [2][GJ]
@@ -86,20 +108,20 @@ SLB_DEV void grid_mean_factor(const slb_sweep& cfg, int f, const int* outs, doub
     // the centre: grid point (GR / 2, GC / 2) of the tile, in the factor's units
     const double cw0 = f64add(f64mul((double)(row0 + GR / 2), g.unit_maxes[0]), g.offset[0]) / l0;
     const double cw1 = f64add(f64mul((double)(col0 + GC / 2), g.unit_maxes[1]), g.offset[1]) / l1;
-    __syncthreads();                           // the previous factor is done with the tables
+    grid_group_sync(grp);                      // the group's previous item is done with the tables
     // the tables run on the uniform offsets xi_i = (i - GR / 2) h0, h0 = unit / l0 (a recurrence along the
     // axis); the grid's own points are within dev of them (a perturbation of the point, in the bound)
     const double h0 = g.unit_maxes[0] / l0, h1 = g.unit_maxes[1] / l1;
-    if (threadIdx.x < GR + GC) {
-        const int c = threadIdx.x < GR ? 0 : 1;
-        const int i = c == 0 ? threadIdx.x : threadIdx.x - GR;
+    if (gt < GR + GC) {
+        const int c = gt < GR ? 0 : 1;
+        const int i = c == 0 ? gt : gt - GR;
         const int64_t gi = (c == 0 ? row0 : col0) + i;
         const double x = f64add(f64mul((double)gi, g.unit_maxes[c]), g.offset[c]);   // grid_index_to_state
         const double ideal = (double)(i - GR / 2) * (c == 0 ? h0 : h1);
-        xi[threadIdx.x] = ideal;
-        dev[threadIdx.x] = fabs((x / (c == 0 ? l0 : l1) - (c == 0 ? cw0 : cw1)) - ideal);
+        xi[gt] = ideal;
+        dev[gt] = fabs((x / (c == 0 ? l0 : l1) - (c == 0 ? cw0 : cw1)) - ideal);
     }
-    __syncthreads();
+    grid_group_sync(grp);
     double mxi = 0.0, meta = 0.0, pert = 0.0;
 #pragma unroll
     for (int r = 0; r < GR; ++r) mxi = fmax(mxi, fabs(xi[r]));
@@ -112,8 +134,7 @@ SLB_DEV void grid_mean_factor(const slb_sweep& cfg, int f, const int* outs, doub
     const int Mp = padded_rows(F.M);
     const double u53 = 1.1102230246251565e-16;
     const double sc = (pol.flags & SLB_FLAG_SCALE) ? pol.out_scale : 1.0;
-    for (int r = 0; r < 3; ++r) {
-        if (!__syncthreads_or(reg[0] == r || reg[1] == r)) continue;
+    {
         double alpha = 0.0, beta = 0.0, cw2;
         if (r == 2) {
             alpha = f64mul(f64mul(__ldg(pol.matrix + 0), sc), l0) / l2;
@@ -129,43 +150,42 @@ SLB_DEV void grid_mean_factor(const slb_sweep& cfg, int f, const int* outs, doub
         double acc[NO][2][2];
 #pragma unroll
         for (int q = 0; q < NO; ++q) { acc[q][0][0] = acc[q][0][1] = acc[q][1][0] = acc[q][1][1] = 0.0; }
-        // the thread's training row of a chunk (GT == GJ), loaded one chunk ahead: its L2 round trip runs
+        // the thread's training row of a chunk (GGT == GJ), loaded one chunk ahead: its L2 round trip runs
         // behind the previous chunk's tables and contraction
-        static_assert(GT == GJ, "one training row per thread and chunk");
         double nx[3] = {0.0, 0.0, 0.0}, ng[NO];
 #pragma unroll
         for (int q = 0; q < NO; ++q) ng[q] = 0.0;
-        if (ok && (int)threadIdx.x < Mp) {
-            const double2 x01 = *reinterpret_cast<const double2*>(F.Xf + (size_t)threadIdx.x * 4);
-            nx[0] = x01.x; nx[1] = x01.y; nx[2] = F.Xf[(size_t)threadIdx.x * 4 + 2];
+        if (ok && gt < Mp) {
+            const double2 x01 = *reinterpret_cast<const double2*>(F.Xf + (size_t)gt * 4);
+            nx[0] = x01.x; nx[1] = x01.y; nx[2] = F.Xf[(size_t)gt * 4 + 2];
 #pragma unroll
-            for (int q = 0; q < NO; ++q) ng[q] = cfg.gp.outputs[outs[q]].gamma_f[threadIdx.x];
+            for (int q = 0; q < NO; ++q) ng[q] = cfg.gp.outputs[outs[q]].gamma_f[gt];
         }
         for (int j0 = 0; ok && j0 < Mp; j0 += GJ) {
             const int J = min(GJ, Mp - j0), J4 = J >> 2;
-            __syncthreads();                   // the previous chunk's tables are consumed
-            if ((int)threadIdx.x < J) {
+            grid_group_sync(grp);              // the previous chunk's tables are consumed
+            if (gt < J) {
                 const double d0 = cw0 - nx[0], d1 = cw1 - nx[1], d2 = cw2 - nx[2];
                 const double K = fma(d0, d0, fma(d1, d1, d2 * d2));
                 const bool keep = K <= GRID_K_DROP;          // dropped rows: weight 0, tables of ones
                 bool far;
                 const double w = keep ? exp_neg_fast(-0.5 * K, tab, far) : 0.0;
-                pq[threadIdx.x] = keep ? fma(alpha, d2, d0) : 0.0;
-                pq[GJ + threadIdx.x] = keep ? fma(beta, d2, d1) : 0.0;
+                pq[gt] = keep ? fma(alpha, d2, d0) : 0.0;
+                pq[GJ + gt] = keep ? fma(beta, d2, d1) : 0.0;
 #pragma unroll
-                for (int q = 0; q < NO; ++q) wg[q * GJ + threadIdx.x] = ng[q] * w;
+                for (int q = 0; q < NO; ++q) wg[q * GJ + gt] = ng[q] * w;
             }
-            const int jn = j0 + GJ + (int)threadIdx.x;
+            const int jn = j0 + GJ + gt;
             if (jn < Mp) {
                 const double2 x01 = *reinterpret_cast<const double2*>(F.Xf + (size_t)jn * 4);
                 nx[0] = x01.x; nx[1] = x01.y; nx[2] = F.Xf[(size_t)jn * 4 + 2];
 #pragma unroll
                 for (int q = 0; q < NO; ++q) ng[q] = cfg.gp.outputs[outs[q]].gamma_f[jn];
             }
-            __syncthreads();
+            grid_group_sync(grp);
             // one table column (training row jj, axis c) per task: exp(-o h p) = g^o for the offsets
             // o = -8 .. 7 from two exps g = exp(-h p), 1 / g = exp(h p) and products outwards from o = 0
-            for (int task = threadIdx.x; task < 2 * J; task += GT) {
+            for (int task = gt; task < 2 * J; task += GGT) {
                 const int c = task >= J ? 1 : 0, jj = task - c * J;
                 const double t = (c ? h1 : h0) * pq[c * GJ + jj];
                 bool far;
@@ -179,7 +199,7 @@ SLB_DEV void grid_mean_factor(const slb_sweep& cfg, int f, const int* outs, doub
 #pragma unroll
                 for (int o = 1; o <= 8; ++o) { v *= gu; col[(8 - o) * 4] = v; }          // m = 8 - o
             }
-            __syncthreads();
+            grid_group_sync(grp);
             const double* pa = e0f + rb * J4 * GFS + lane;
             const double* pb = e1f + cb * J4 * GFS + lane;
 #pragma unroll 2
@@ -212,7 +232,8 @@ SLB_DEV void grid_mean_factor(const slb_sweep& cfg, int f, const int* outs, doub
                                    exp(-0.5 * kd * kd));
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-            if (reg[h] != r) continue;
+            const int p = ti * GC + tk0 + h;
+            if (reg[p] != r) continue;
             const double x0 = xi[ti], e1 = eta[tk0 + h];
             const double v = fma(alpha, x0, beta * e1);
             bool far;
@@ -221,13 +242,12 @@ SLB_DEV void grid_mean_factor(const slb_sweep& cfg, int f, const int* outs, doub
             for (int q = 0; q < NO; ++q) {
                 const slb_gp_output& G = cfg.gp.outputs[outs[q]];
                 const double m =
-                    f64add(f64mul(acc[q][0][h] + acc[q][1][h], Q), prior_mean_term<3>(F, G, z[h])) / F.scale;
+                    f64add(f64mul(acc[q][0][h] + acc[q][1][h], Q), prior_mean_term<3>(F, G, z + 3 * p)) / F.scale;
                 const double bound = ok && eps < 1e-3
                                          ? (eps * G.gamma_l1 + 1e-150 * (Mp + 1)) / fabs(F.scale) + 1e-300
                                          : f64_inf();
-#pragma unroll
-                for (int o = 0; o < GNO; ++o)
-                    if (o == outs[q]) { mu[h][o] = m; dm[h][o] = bound; }
+                mu[p * GNO + outs[q]] = m;         // outs[q] < GNO (grid_mean_applicable: at most 4 outputs)
+                dm[p * GNO + outs[q]] = bound;
             }
         }
     }
