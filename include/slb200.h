@@ -396,6 +396,24 @@ int slb_gp_vjp(void* stream, const slb_gp_stack* gp, const double* points_dev, i
                const double* grad_mean_dev, const double* grad_err_dev, double* grad_points_dev,
                void* workspace_dev);
 
+/* ---- gradient of the GP log marginal likelihood with respect to the hyper-parameters (gpflow 0.4.0
+ *      GPR.build_likelihood): with K = kern.K(X) + noise I, alpha = K^-1 (Y - m(X)), W = alpha alpha^T - K^-1,
+ *        d LML / d theta = 1/2 sum_ij W_ij d K_ij / d theta,     d LML / d noise = 1/2 tr W,
+ *      for every slot of the covariance expression kern (num_prims >= 1; GPRCached.scale does not enter).
+ *      X_dev [M, d_in] raw inputs, Kinv_dev [M, M] = K^-1 (row-major, both triangles), alpha_dev [M];
+ *      grad_dev [SLB_GP_HYPER_SLOTS] (device) receives, for primitive p, d / d prims[p].variance at
+ *      [p * (1 + SLB_MAX_IN)] and d / d prims[p].w[c] at [p * (1 + SLB_MAX_IN) + 1 + c] (w = 1 / lengthscale
+ *      for the stationary kinds, the per-column variance for LINEAR; slots of absent primitives and columns
+ *      are 0), and d / d noise last.  WHITE is K(X)'s form: its variance counts on the diagonal i == j only.
+ *      One pass over the lower triangle in tiles of SLB_GP_HYPER_TILE x SLB_GP_HYPER_TILE pairs; per-tile
+ *      sums go to workspace_dev (>= slb_gp_lml_grad_workspace(M) bytes) and are added in tile order: two
+ *      calls give bit-identical results.  M == 0 returns before any CUDA call (grad_dev is not written). */
+#define SLB_GP_HYPER_TILE 64
+#define SLB_GP_HYPER_SLOTS (SLB_MAX_KPRIM * (1 + SLB_MAX_IN) + 1)
+int64_t slb_gp_lml_grad_workspace(int32_t M);
+int slb_gp_lml_grad(void* stream, const double* X_dev, int32_t M, int32_t d_in, const slb_kernel* kern,
+                    const double* Kinv_dev, const double* alpha_dev, double* grad_dev, void* workspace_dev);
+
 /* ---- the fused Lyapunov sweep over flat grid indices [idx_begin, idx_end):
  *      index -> x (functions.py:714-731) -> u = policy(x) -> [x,u] -> GP mean / beta*sigma
  *      (or deterministic dynamics) -> V(x), V(mu), L_V(mu) . e -> decrease < threshold

@@ -25,6 +25,9 @@ FLAG_SATURATE, FLAG_ABS, FLAG_NORM1, FLAG_PROJECT, FLAG_SCALE, FLAG_GRADIENT, FL
     1, 2, 4, 8, 16, 32, 64
 K_RBF, K_MATERN12, K_MATERN32, K_MATERN52, K_LINEAR, K_CONSTANT, K_WHITE = range(7)
 SLB_MAX_KPRIM = 6
+# slb_gp_lml_grad: tile edge and gradient slots [prim][variance, w[0..SLB_MAX_IN)] + noise (include/slb200.h)
+SLB_GP_HYPER_TILE = 64
+SLB_GP_HYPER_SLOTS = SLB_MAX_KPRIM * (1 + SLB_MAX_IN) + 1
 ABI_VERSION = 6
 # slb_value_solve: stats slots and status codes (include/slb200.h)
 VALUE_STATS = 16
@@ -187,6 +190,8 @@ SIGNATURES = {
     "slb_triangulation_rows": (C.c_int, [_vp, C.POINTER(SlbFunction), _dp, _i64, _vp, _dp]),
     "slb_gp_vjp_workspace": (C.c_int64, [C.POINTER(SlbGpStack), _i64]),
     "slb_gp_vjp": (C.c_int, [_vp, C.POINTER(SlbGpStack), _dp, _i64, _dp, _dp, _dp, _vp]),
+    "slb_gp_lml_grad_workspace": (C.c_int64, [_i32]),
+    "slb_gp_lml_grad": (C.c_int, [_vp, _dp, _i32, _i32, C.POINTER(SlbKernel), _dp, _dp, _dp, _vp]),
 }
 
 _lib = None

@@ -50,6 +50,9 @@ void slb_count_launch();
 int slb_validate_function(const slb_function* f, const char* what, int expect_in /* <=0: any */);
 int slb_fn_columns(const slb_function& f);
 int slb_validate_dynamics(const slb_function* f, const char* who, int d, int m);
+// the covariance expression's own checks (primitive count, kinds, term order, weights of the first
+// d_in columns non-negative); messages start with `who`
+int slb_validate_kernel(const slb_kernel& K, int d_in, const char* who);
 int slb_validate_gp(const slb_gp_stack* gp);
 int slb_validate_staged_tables(const slb_gp_stack* gp, const char* who);
 int slb_validate_grid(const slb_grid* g, bool need_points);

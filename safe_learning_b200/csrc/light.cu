@@ -166,6 +166,23 @@ int slb_validate_dynamics(const slb_function* f, const char* who, int d, int m) 
     return 0;
 }
 
+int slb_validate_kernel(const slb_kernel& K, int d_in, const char* who) {
+    SLB_CHECK(K.num_prims >= 0 && K.num_prims <= SLB_MAX_KPRIM,
+              "%s: %d kernel primitives outside 0..%d", who, K.num_prims, SLB_MAX_KPRIM);
+    for (int i = 0; i < K.num_prims; ++i) {
+        const slb_kernel_prim& P = K.prims[i];
+        SLB_CHECK(P.kind >= SLB_K_RBF && P.kind <= SLB_K_WHITE,
+                  "%s: kernel primitive %d has unknown kind %d", who, i, P.kind);
+        const int prev = i == 0 ? 0 : K.prims[i - 1].term;
+        SLB_CHECK(P.term == prev || P.term == prev + 1,
+                  "%s: kernel primitives must be listed in term order", who);
+        SLB_CHECK(i > 0 || P.term == 0, "%s: kernel terms start at 0", who);
+        for (int c = 0; c < d_in; ++c)
+            SLB_CHECK(P.w[c] >= 0.0, "%s: kernel primitive %d has a negative weight", who, i);
+    }
+    return 0;
+}
+
 int slb_validate_gp(const slb_gp_stack* gp) {
     if (gp->num_outputs == 0) return 0;
     SLB_CHECK(gp->num_outputs >= 1 && gp->num_outputs <= SLB_MAX_OUT, "GP outputs %d outside 1..%d",
@@ -180,25 +197,13 @@ int slb_validate_gp(const slb_gp_stack* gp) {
                   F.nrb);
         SLB_CHECK(F.M == 0 || (F.Xs != nullptr && F.Wpack != nullptr), "GP factor %d: null table", f);
         SLB_CHECK(F.scale > 0.0, "GP factor %d: scale must be positive", f);
-        const slb_kernel& K = F.kernel;
-        SLB_CHECK(K.num_prims >= 0 && K.num_prims <= SLB_MAX_KPRIM,
-                  "GP factor %d: %d kernel primitives outside 0..%d", f, K.num_prims, SLB_MAX_KPRIM);
-        if (K.num_prims == 0) {
+        char who[32];
+        snprintf(who, sizeof(who), "GP factor %d", f);
+        if (slb_validate_kernel(F.kernel, gp->input_dim, who)) return 1;
+        if (F.kernel.num_prims == 0) {
             for (int c = 0; c < gp->input_dim; ++c)
                 SLB_CHECK(F.lengthscales[c] > 0.0, "GP factor %d: lengthscale[%d] must be positive",
                           f, c);
-        }
-        for (int i = 0; i < K.num_prims; ++i) {
-            const slb_kernel_prim& P = K.prims[i];
-            SLB_CHECK(P.kind >= SLB_K_RBF && P.kind <= SLB_K_WHITE,
-                      "GP factor %d: kernel primitive %d has unknown kind %d", f, i, P.kind);
-            const int prev = i == 0 ? 0 : K.prims[i - 1].term;
-            SLB_CHECK(P.term == prev || P.term == prev + 1,
-                      "GP factor %d: kernel primitives must be listed in term order", f);
-            SLB_CHECK(i > 0 || P.term == 0, "GP factor %d: kernel terms start at 0", f);
-            for (int c = 0; c < gp->input_dim; ++c)
-                SLB_CHECK(P.w[c] >= 0.0, "GP factor %d: kernel primitive %d has a negative weight",
-                          f, i);
         }
     }
     for (int o = 0; o < gp->num_outputs; ++o) {

@@ -13,6 +13,7 @@ Constant, White, sums and products, ``active_dims``; arithmetic of ``gpflow==0.4
 
 from __future__ import annotations
 
+import collections
 import hashlib
 import itertools
 import weakref
@@ -1468,6 +1469,17 @@ class Kernel(object):
     def is_plain_rbf(self, din):
         return False
 
+    def primitives(self, path="kern"):
+        """``(path, primitive)`` of every primitive object of the expression tree in tree order, each
+        object once (at its first path): a primitive that product expansion puts in several terms is
+        one set of parameters."""
+        out, seen = [], set()
+        for p, prim in self._walk(path):
+            if id(prim) not in seen:
+                seen.add(id(prim))
+                out.append((p, prim))
+        return out
+
     def K_device(self, X, X2=None):
         """K(X, X2) on raw inputs (device tensors), gpflow arithmetic."""
         total = None
@@ -1520,6 +1532,10 @@ class Sum(Kernel):
     def terms(self):
         return [term for k in self.kern_list for term in k.terms()]
 
+    def _walk(self, path):
+        for i, k in enumerate(self.kern_list):
+            yield from k._walk("%s.kern_list[%d]" % (path, i))
+
 
 Add = Sum
 
@@ -1533,6 +1549,8 @@ class Product(Kernel):
         for k in self.kern_list:
             out = [a + b for a in out for b in k.terms()]
         return out
+
+    _walk = Sum._walk
 
 
 Prod = Product
@@ -1552,8 +1570,18 @@ class _Primitive(Kernel):
             raise DimensionError("active_dims %r does not select input_dim = %d columns"
                                  % (self.active_dims, self.input_dim))
 
+    PARAMS = ("variance",)        # hyper-parameter attributes, in GPRCached.hyperparameters() order
+
     def terms(self):
         return [[self]]
+
+    def _walk(self, path):
+        yield path, self
+
+    def _slot_gradient(self, g_variance, g_w):
+        """Gradients of this primitive's parameters from one descriptor occurrence's slot gradients
+        (``slb_gp_lml_grad``: ``g_variance``, ``g_w[c]`` per input column), one value per component."""
+        return {"variance": g_variance}
 
     def _slice(self, X):
         return X[:, self.active_dims]
@@ -1570,6 +1598,8 @@ class _Primitive(Kernel):
 
 
 class _Stationary(_Primitive):
+    PARAMS = ("variance", "lengthscales")
+
     def __init__(self, input_dim, variance=1.0, lengthscales=None, active_dims=None, ARD=False):
         _Primitive.__init__(self, input_dim, active_dims)
         self.variance = float(variance)
@@ -1580,6 +1610,11 @@ class _Stationary(_Primitive):
 
     def _weights(self):
         return 1.0 / self.lengthscales
+
+    def _slot_gradient(self, g_variance, g_w):
+        # w = 1 / l:  d / d l = -(d / d w) / l^2
+        return {"variance": g_variance,
+                "lengthscales": -np.asarray(g_w)[self.active_dims] / self.lengthscales ** 2}
 
     def hyper_key(self):
         return (self.KIND, tuple(self.active_dims), self.variance,
@@ -1665,6 +1700,9 @@ class Linear(_Primitive):
     def _weights(self):
         return self.variance
 
+    def _slot_gradient(self, g_variance, g_w):
+        return {"variance": np.asarray(g_w)[self.active_dims]}     # w_c is the column's variance
+
     def _K(self, X, X2=None):
         var = torch.as_tensor(self.variance, dtype=torch.float64, device=X.device)
         X = self._slice(X)
@@ -1727,6 +1765,31 @@ class Likelihood(object):
 
     def __init__(self, variance=1.0):
         self.variance = float(variance)
+
+
+# gpflow 0.4.0's positive transform (transforms.Log1pe): value = softplus(free) + 1e-6
+_POSITIVE_LOWER = 1e-6
+
+
+def _param_value(owner, name):
+    """Copy of hyper-parameter ``owner.name``: a float, or one value per column when ``owner.ARD``."""
+    value = np.asarray(getattr(owner, name), dtype=np.float64)
+    if value.ndim == 0:
+        return float(value)
+    if getattr(owner, "ARD", False):
+        return value.copy()
+    if np.any(value != value[0]):
+        raise ValueError("%s.%s holds %s although ARD is False: a non-ARD parameter is one value"
+                         % (type(owner).__name__, name, value.tolist()))
+    return float(value[0])
+
+
+def _set_param_value(owner, name, value):
+    old = getattr(owner, name)
+    if np.ndim(old) == 0:
+        setattr(owner, name, float(value))
+    else:
+        setattr(owner, name, np.broadcast_to(np.asarray(value, dtype=np.float64), np.shape(old)).copy())
 
 
 class _Factor(object):
@@ -2107,6 +2170,133 @@ class GPRCached(object):
         o.prior_mean = None if self._prior_dev is None else self._prior_dev.data_ptr()
         o.gamma_f, o.gamma_l1 = self._gamma_f_dev.data_ptr(), self._gamma_l1
 
+    # hyper-parameters and the log marginal likelihood (gpflow 0.4.0 GPR.build_likelihood) ------------
+    def _hyper_params(self):
+        """``(path, owner, attribute)`` of every hyper-parameter, in ``hyperparameters()`` order."""
+        out = [("%s.%s" % (path, name), prim, name)
+               for path, prim in self.kern.primitives() for name in prim.PARAMS]
+        out.append(("likelihood.variance", self.likelihood, "variance"))
+        return out
+
+    def hyperparameters(self):
+        """Ordered dict from a path relative to the model (``kern.variance``,
+        ``kern.kern_list[1].kern_list[0].lengthscales``, ``likelihood.variance``) to a copy of the
+        value: a float, or one value per active column for an ARD primitive.  A primitive that
+        appears in several product terms is listed once."""
+        return collections.OrderedDict((path, _param_value(owner, name))
+                                       for path, owner, name in self._hyper_params())
+
+    def _set_hyperparameters(self, values):
+        where = {path: (owner, name) for path, owner, name in self._hyper_params()}
+        for path, value in values.items():
+            _set_param_value(*where[path], value)
+
+    def _log_likelihood(self, want_grad):
+        """LML and, if ``want_grad``, its gradient in ``slb_gp_lml_grad``'s descriptor slots.  Its own
+        factorisation of ``K + noise I`` (torch / cuSOLVER): the cached posterior factor and the filter
+        tables are not touched.  A matrix that is not positive definite raises
+        ``torch.linalg.LinAlgError``."""
+        lib = nat.load()
+        M, din = self._X.shape
+        kstruct = nat.SlbKernel()
+        self.kern.fill(kstruct, din)
+        slots = np.zeros(nat.SLB_GP_HYPER_SLOTS)
+        if M == 0:
+            if want_grad:           # the descriptor checks still run; nothing is launched
+                nat.check(lib.slb_gp_lml_grad(None, None, 0, din, kstruct, None, None, None, None),
+                          "slb_gp_lml_grad")
+            return 0.0, slots
+        X = dev.to_device(self._X)
+        K = self.kern.K_device(X) + torch.eye(M, dtype=torch.float64, device=X.device) * self.likelihood.variance
+        L = torch.linalg.cholesky(K)
+        d = dev.to_device(self._Y)
+        if self.mean_function is not None:
+            d = d - self.mean_function.evaluate_device(self._X)
+        a = torch.linalg.solve_triangular(L, d, upper=False)
+        lml = -0.5 * M * np.log(2 * np.pi) - torch.log(torch.diagonal(L)).sum() - 0.5 * (a * a).sum()
+        if want_grad:
+            alpha = torch.cholesky_solve(d, L)[:, 0].contiguous()
+            kinv = torch.cholesky_inverse(L).contiguous()
+            work = dev.empty((int(lib.slb_gp_lml_grad_workspace(M)) // 8,))
+            grad = dev.empty((nat.SLB_GP_HYPER_SLOTS,))
+            nat.check(lib.slb_gp_lml_grad(dev.stream(), X.data_ptr(), M, din, kstruct, kinv.data_ptr(),
+                                          alpha.data_ptr(), grad.data_ptr(), work.data_ptr()),
+                      "slb_gp_lml_grad")
+            slots = grad.cpu().numpy()
+        return float(lml.item()), slots
+
+    def compute_log_likelihood(self):
+        """Log marginal likelihood ``log N(Y | m(X), K(X) + noise I)`` (gpflow's name); 0 for an
+        empty data set.  ``scale`` does not enter (the reference scales only the prediction cache)."""
+        return self._log_likelihood(False)[0]
+
+    def log_likelihood_and_gradient(self):
+        """``(LML, {path: d LML / d parameter})``, each gradient shaped like its parameter in
+        ``hyperparameters()``: the fused kernel's slot gradients chained to the parameters (``d / d l =
+        -(d / d w) / l^2``, a non-ARD value sums its columns, a shared primitive sums its terms)."""
+        lml, slots = self._log_likelihood(True)
+        stride = 1 + nat.SLB_MAX_IN
+        per_prim = {}
+        flat = [p for term in self.kern.terms() for p in term]
+        for i, prim in enumerate(flat):
+            acc = per_prim.setdefault(id(prim), {})
+            for name, g in prim._slot_gradient(slots[i * stride], slots[i * stride + 1:(i + 1) * stride]).items():
+                acc[name] = acc.get(name, 0.0) + np.asarray(g, dtype=np.float64)
+        grads = collections.OrderedDict()
+        for path, owner, name in self._hyper_params():
+            g = slots[-1] if owner is self.likelihood else per_prim[id(owner)][name]
+            grads[path] = float(np.sum(g)) if np.ndim(_param_value(owner, name)) == 0 else g.copy()
+        return lml, grads
+
+    def optimize(self, method="L-BFGS-B", tol=None, callback=None, maxiter=1000, fixed=()):
+        """Fit the kernel and noise hyper-parameters by maximising the log marginal likelihood
+        (gpflow 0.4.0 ``Model.optimize``): ``scipy.optimize.minimize(jac=True)`` of ``-LML`` in the
+        free space of gpflow's positive transform (``softplus(x) + 1e-6``); ``callback`` receives that
+        free vector.  ``fixed``: paths of ``hyperparameters()`` held at their values (gpflow's
+        ``param.fixed = True``, e.g. ``"likelihood.variance"`` for a known measurement noise).  The
+        fitted values are written back into the kernel objects and ``likelihood``; the next sweep
+        refits the posterior.  Returns scipy's ``OptimizeResult``.  A free parameter at or below 1e-6
+        raises ``ValueError``; if the search fails (e.g. a Cholesky failure) the original values are
+        restored and the error propagates."""
+        import scipy.optimize
+        import scipy.special
+        start = self.hyperparameters()
+        unknown = [p for p in fixed if p not in start]
+        if unknown:
+            raise ValueError("fixed: unknown hyper-parameter path(s) %s; known: %s" % (unknown, list(start)))
+        free = [p for p in start if p not in fixed]
+        low = [p for p in free if np.any(np.asarray(start[p]) <= _POSITIVE_LOWER)]
+        if low:
+            raise ValueError("hyper-parameter(s) %s start at or below the positive transform's floor %g"
+                             % (low, _POSITIVE_LOWER))
+        shapes = [np.shape(start[p]) for p in free]
+        y0 = np.concatenate([np.ravel(start[p]) for p in free])
+        ys = y0 - _POSITIVE_LOWER
+        x0 = ys + np.log(-np.expm1(-ys))              # softplus^-1
+
+        def unpack(x):
+            y = np.logaddexp(0.0, x) + _POSITIVE_LOWER
+            out, k = {}, 0
+            for p, shape in zip(free, shapes):
+                n = int(np.prod(shape))
+                out[p] = float(y[k]) if shape == () else y[k:k + n].reshape(shape)
+                k += n
+            return out
+
+        def objective(x):
+            self._set_hyperparameters(unpack(x))
+            lml, grads = self.log_likelihood_and_gradient()
+            g = np.concatenate([np.ravel(grads[p]) for p in free])
+            return -lml, -g * scipy.special.expit(x)
+
+        try:
+            result = scipy.optimize.minimize(objective, x0, method=method, jac=True, tol=tol, callback=callback,
+                                             options=dict(maxiter=maxiter))
+        except BaseException:
+            self._set_hyperparameters(start)
+            raise
+        self._set_hyperparameters(unpack(result.x))
+        return result
 
     def variance_floor(self):
         """Certified lower bound of posterior variance / prior variance (see ``_head``)."""

@@ -28,8 +28,11 @@
             (batch 1000, notebook-kernel FunctionStack at M = 0, 50, 200) through the GP node against
             torch_predict as a plain dynamics callable, and the VJP alone on C2's GPs (plain RBF, M = 500,
             two factors) for 10^3, 10^4 and 65536 points against the forward and torch autograd
+  gp_fit    GPRCached hyper-parameter fit at M = 500, 2000, 5000 (notebook kernel and ARD RBF, d_in = 3): the
+            fused gradient kernel alone, one value + gradient, torch autograd of the same, optimize(maxiter=50)
 
     python tools/bench_extra.py [bellman] [det] [c5] [shared] [roa] [reward_rollout] [value_opt] [train] [nn_lv] [gp_vjp]
+                                [gp_fit]
 """
 import json
 import os
@@ -728,6 +731,97 @@ def gp_vjp():
                           "ms_vjp_mean_only": ms_mean, "ms_forward": ms_fwd, "ms_torch_autograd": ms_torch,
                           "gflop_err_term": flops / 1e9, "tflops": flops / ms_both / 1e9,
                           "share_of_dmma_peak": flops / ms_both / 1e9 / PEAK_TF, **info}))
+
+
+def _gp_fit_kernel(kind, din, K):
+    """(product kernel, hyper-parameter tensors, torch expression of K(X) in them) of a gp_fit workload."""
+    if kind == "notebook":
+        kern = K.Linear(din, variance=np.linspace(0.2, 0.5, din), ARD=True) + \
+            K.Matern32(1, variance=0.8, lengthscales=0.7, active_dims=[0]) * K.Linear(1, variance=0.6)
+
+        def expr(X, t):
+            x0 = X[:, :1] / t["kern.kern_list[1].kern_list[0].lengthscales"]
+            sq = (x0 * x0).sum(1)
+            r = torch.sqrt(-2 * x0 @ x0.T + sq[:, None] + sq[None, :] + 1e-12)
+            m32 = t["kern.kern_list[1].kern_list[0].variance"] * (1 + np.sqrt(3) * r) * torch.exp(-np.sqrt(3) * r)
+            return (X * t["kern.kern_list[0].variance"]) @ X.T + \
+                m32 * ((X[:, :1] * t["kern.kern_list[1].kern_list[1].variance"]) @ X[:, :1].T)
+    else:
+        kern = K.RBF(din, variance=1.3, lengthscales=np.linspace(0.7, 1.2, din), ARD=True)
+
+        def expr(X, t):
+            xs = X / t["kern.lengthscales"]
+            sq = (xs * xs).sum(1)
+            return t["kern.variance"] * torch.exp(-0.5 * (-2 * xs @ xs.T + sq[:, None] + sq[None, :]))
+    return kern, expr
+
+
+def gp_fit():
+    """GPRCached hyper-parameter fit (d_in = 3, noise 0.01): the notebook kernel Linear(3, ARD) + Matern32(1,
+    active_dims=[0]) * Linear(1) and an ARD RBF at M = 500, 2000, 5000.  Reported: the fused gradient kernel
+    alone (slb_gp_lml_grad on a given K^-1 and alpha; it reads the lower triangle of K^-1 once, M (M + 1) / 2
+    doubles); one log_likelihood_and_gradient (K, Cholesky, K^-1, alpha, kernel, host copy); the same LML and
+    gradient by torch autograd through the tensor expression of K; optimize(maxiter=50) wall time."""
+    import time
+    from safe_learning_b200 import _native as nat
+    lib = nat.load()
+    info = None
+    din = 3
+    for kind in ("notebook", "rbf_ard"):
+        for M in (500, 2000, 5000):
+            rng = np.random.default_rng(M)
+            X = rng.uniform(-1, 1, (M, din))
+            Y = np.sin(2 * X).sum(axis=1, keepdims=True) + 0.1 * rng.standard_normal((M, 1))
+            kern, expr = _gp_fit_kernel(kind, din, sl.kernels)
+            gp = sl.GPR(X, Y, kern, noise_variance=0.01)
+            Xd = torch.tensor(X, device="cuda")
+            Yd = torch.tensor(Y, device="cuda")
+            Kn = kern.K_device(Xd) + 0.01 * torch.eye(M, dtype=torch.float64, device="cuda")
+            L = torch.linalg.cholesky(Kn)
+            kinv = torch.cholesky_inverse(L).contiguous()
+            alpha = torch.cholesky_solve(Yd, L)[:, 0].contiguous()
+            ks = nat.SlbKernel()
+            kern.fill(ks, din)
+            work = torch.empty(int(lib.slb_gp_lml_grad_workspace(M)) // 8, dtype=torch.float64, device="cuda")
+            grad = torch.empty(nat.SLB_GP_HYPER_SLOTS, dtype=torch.float64, device="cuda")
+            stream = torch.cuda.current_stream().cuda_stream
+
+            def fused():
+                nat.check(lib.slb_gp_lml_grad(stream, Xd.data_ptr(), M, din, ks, kinv.data_ptr(), alpha.data_ptr(),
+                                              grad.data_ptr(), work.data_ptr()), "slb_gp_lml_grad")
+
+            if info is None:
+                info = _gpu_info(lambda: [fused() for _ in range(200)])
+            ms_kernel = timed(fused, steps=50, warmup=5)
+            ms_value_grad = timed(gp.log_likelihood_and_gradient, steps=10)
+
+            def autograd():
+                t = {p: torch.tensor(np.asarray(v, dtype=np.float64), device="cuda", requires_grad=True)
+                     for p, v in gp.hyperparameters().items()}
+                Lt = torch.linalg.cholesky(expr(Xd, t) + t["likelihood.variance"]
+                                           * torch.eye(M, dtype=torch.float64, device="cuda"))
+                a = torch.linalg.solve_triangular(Lt, Yd, upper=False)
+                lml = -0.5 * M * np.log(2 * np.pi) - torch.log(torch.diagonal(Lt)).sum() - 0.5 * (a * a).sum()
+                torch.autograd.grad(lml, list(t.values()))
+
+            ms_autograd = timed(autograd, steps=10)
+            start = gp.hyperparameters()
+            fits = []
+            for _ in range(3):
+                gp._set_hyperparameters(start)
+                torch.cuda.synchronize()
+                t0 = time.perf_counter()
+                res = gp.optimize(maxiter=50, fixed=("likelihood.variance",))
+                torch.cuda.synchronize()
+                fits.append(time.perf_counter() - t0)
+            nbytes = M * (M + 1) / 2 * 8
+            print(json.dumps({"bench": "gp_fit", "kernel": kind, "d_in": din, "M": M, "ms_fused_kernel": ms_kernel,
+                              "kinv_gbs": nbytes / ms_kernel / 1e6, "ms_value_and_gradient": ms_value_grad,
+                              "ms_torch_autograd": ms_autograd, "autograd_over_value_and_gradient":
+                              ms_autograd / ms_value_grad, "s_optimize_maxiter50": float(np.median(fits)),
+                              "optimize_nfev": int(res.nfev), "optimize_nit": int(res.nit),
+                              "note": "median of CUDA events (kernel: 50, calls: 10); optimize: median of 3 "
+                                      "wall-clock fits from the same start", **info}))
 
 
 def _stage1(lyap):
