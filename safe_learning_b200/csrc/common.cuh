@@ -762,6 +762,69 @@ SLB_DEV int eval_fn_small(const slb_function& f, const double* in, double* out) 
     return eval_fn(f, in, out);
 }
 
+// Register-only evaluators of the closed form the filter's factored grid path runs on (filter.cu,
+// grid_mean_applicable): the saturated linear policy, V = x^T P x and a LINEAR L_V / L_f.  Shapes are
+// compile-time, operands and results stay in registers and there is no fallback call: the host has proved
+// the kind and flags.  Each is eval_fn_small's arithmetic operation for operation, and so bit-identical to
+// eval_fn (for out_dim 3 and 4, which eval_fn_small leaves to eval_fn, eval_fn's own order).
+template <int N> struct slb_vec { double v[N]; };
+constexpr int SLB_MAX_LIN_OUT = 4;     // out_dim of a closed-form L_V / L_f (grid_mean_applicable)
+
+// LINEAR, in_dim N, out_dim <= MO (run time), flags among SATURATE | ABS | NORM1 | SCALE.  Returns the
+// columns; `cols` = their number (1 after NORM1).
+template <int N, int MO>
+SLB_DEV slb_vec<MO> eval_linear_reg(const slb_function& f, const double (&x)[N], int& cols) {
+    const int od = f.out_dim;
+    slb_vec<MO> y;
+#pragma unroll
+    for (int o = 0; o < MO; ++o) {
+        y.v[o] = 0.0;
+        if (o < od) {
+            const double* row = f.matrix + o * N;
+            double acc = f64mul(x[0], __ldg(row));
+#pragma unroll
+            for (int k = 1; k < N; ++k) acc = f64add(acc, f64mul(x[k], __ldg(row + k)));
+            y.v[o] = acc;
+        }
+    }
+    if (f.flags & SLB_FLAG_SATURATE) {
+#pragma unroll
+        for (int o = 0; o < MO; ++o) y.v[o] = fmin(fmax(y.v[o], f.lower), f.upper);
+    }
+    if (f.flags & (SLB_FLAG_ABS | SLB_FLAG_NORM1)) {
+#pragma unroll
+        for (int o = 0; o < MO; ++o) y.v[o] = fabs(y.v[o]);
+    }
+    cols = od;
+    if (f.flags & SLB_FLAG_NORM1) {
+#pragma unroll
+        for (int o = 1; o < MO; ++o)
+            if (o < od) y.v[0] = f64add(y.v[0], y.v[o]);
+        cols = 1;
+    }
+    if (f.flags & SLB_FLAG_SCALE) {
+#pragma unroll
+        for (int o = 0; o < MO; ++o) y.v[o] = f64mul(y.v[o], f.out_scale);
+    }
+    return y;
+}
+
+// QUADRATIC, in_dim N, flags among SCALE:  sum_c (sum_r x_r P[r,c]) x_c
+template <int N>
+SLB_DEV double eval_quadratic_reg(const slb_function& f, const double (&x)[N]) {
+    double total = 0.0;
+#pragma unroll
+    for (int c = 0; c < N; ++c) {
+        double lin = f64mul(x[0], __ldg(f.matrix + c));
+#pragma unroll
+        for (int r = 1; r < N; ++r) lin = f64add(lin, f64mul(x[r], __ldg(f.matrix + r * N + c)));
+        const double prod = f64mul(lin, x[c]);
+        total = (c == 0) ? prod : f64add(total, prod);
+    }
+    if (f.flags & SLB_FLAG_SCALE) total = f64mul(total, f.out_scale);
+    return total;
+}
+
 // The per-point prologue / epilogue of a sweep kernel reads a handful of small operands through
 // pointers of the descriptor (policy / V / L_V / L_f matrices, prior-mean rows), one dependent global
 // load after the other; after an L2 flush (or any eviction) each is an HBM round trip in every CTA's
@@ -810,6 +873,34 @@ SLB_DEV void lyapunov_state_terms(const slb_sweep& cfg, const double* x, int64_t
         lf = tmp[0];
     }
     *threshold_out = f64mul(f64mul(-lvx, f64add(1.0, lf)), cfg.tau);   // :288
+}
+
+// ... the same for the closed form (a state of D dims, V QUADRATIC, L_V and L_f absent or LINEAR with
+// the flags eval_linear_reg takes): the register-only evaluators, the arithmetic above
+template <int D>
+SLB_DEV void lyapunov_state_terms_closed(const slb_sweep& cfg, const double (&x)[D], int64_t flat_index,
+                                         double* vx_out, double* threshold_out) {
+    *vx_out = eval_quadratic_reg<D>(cfg.lyapunov, x);
+    double lvx = cfg.lv_const;
+    if (cfg.lipschitz_v.kind != SLB_FN_NONE) {
+        int nl;
+        const slb_vec<SLB_MAX_LIN_OUT> lv = eval_linear_reg<D, SLB_MAX_LIN_OUT>(cfg.lipschitz_v, x, nl);
+        lvx = lv.v[0];
+        if (nl > 1) {
+            lvx = fabs(lv.v[0]);
+#pragma unroll
+            for (int j = 1; j < SLB_MAX_LIN_OUT; ++j)
+                if (j < nl) lvx = f64add(lvx, fabs(lv.v[j]));
+        }
+    }
+    double lf = cfg.lf_const;
+    if (cfg.lf_values != nullptr && flat_index >= 0) {
+        lf = cfg.lf_values[flat_index - cfg.lf_index_base];
+    } else if (cfg.lipschitz_f.kind != SLB_FN_NONE) {
+        int nf;
+        lf = eval_linear_reg<D, SLB_MAX_LIN_OUT>(cfg.lipschitz_f, x, nf).v[0];
+    }
+    *threshold_out = f64mul(f64mul(-lvx, f64add(1.0, lf)), cfg.tau);
 }
 
 // (2) sum_j L_V(mu)_j err_j, L_V evaluated at the predicted MEAN                :344-347

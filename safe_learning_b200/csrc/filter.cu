@@ -45,6 +45,7 @@
 
 #include <atomic>
 #include <string.h>
+#include <type_traits>
 
 #include "gp_mean_staged.cuh"
 #include "gp_mean_grid.cuh"
@@ -256,6 +257,150 @@ SLB_DEV int screened_outcome(const slb_sweep& cfg, filter_side& t, double vx, co
     return decide(t, shi, cfg.gp.num_outputs);
 }
 
+// ---- the same decision in closed form ------------------------------------------------------------------
+// For the sweeps grid_mean_applicable accepts (D outputs, V QUADRATIC, L_V absent or LINEAR): the terms,
+// slack and outcome above with compile-time D and every operand in registers -- the per-point decision of
+// stage 1's grid kernel and of the head stage behind it.  Same arithmetic, same order: the outcomes equal
+// those of the generic functions bit for bit.
+template <int D>
+struct cf_terms { double dec0, thr, guard, coef[D]; };
+
+// mean_decision_terms
+template <int D>
+SLB_DEV void cf_mean_terms(const slb_sweep& cfg, cf_terms<D>& t, double vx, const double (&mu)[D],
+                           const double (&mean_err)[D]) {
+    const double vm = eval_quadratic_reg<D>(cfg.lyapunov, mu);
+    t.dec0 = f64sub(vm, vx);
+    int nl = 1;
+    slb_vec<SLB_MAX_LIN_OUT> lv;
+    lv.v[0] = cfg.lv_const;
+    if (cfg.lipschitz_v.kind != SLB_FN_NONE) lv = eval_linear_reg<D, SLB_MAX_LIN_OUT>(cfg.lipschitz_v, mu, nl);
+    double lvmu = 0.0, lverr = 0.0;
+#pragma unroll
+    for (int j = 0; j < D; ++j) {
+        const double l = nl == 1 ? lv.v[0] : lv.v[j];
+        t.coef[j] = l * cfg.gp.outputs[j].beta;
+        lvmu += fabs(l * mu[j]);
+        lverr += fabs(l) * mean_err[j];
+    }
+    t.guard = 1e-6 * (fabs(vm) + fabs(vx) + fabs(t.thr) + lvmu) + 4.0 * lverr + 1e-300;
+}
+
+// screening_slack.  The generic function pads every operand to four lanes with zeros; for D < 4 that turns
+// the slack into NaN whenever a mean or bound is not finite (0 * inf), which `poison` restates.
+template <int D>
+SLB_DEV double cf_screening_slack(const slb_sweep& cfg, const double (&mu)[D], const double (&dm)[D],
+                                  const double (&shi)[D]) {
+    const slb_function& V = cfg.lyapunov;
+    double poison = 0.0;
+    if constexpr (D < 4) {
+#pragma unroll
+        for (int i = 0; i < D; ++i) poison += 0.0 * mu[i] + 0.0 * dm[i];
+    }
+    double bs[D];                                           // beta_j shi_j
+#pragma unroll
+    for (int j = 0; j < D; ++j) bs[j] = f64mul(fabs(cfg.gp.outputs[j].beta), shi[j]);
+    double dv = 0.0;
+#pragma unroll
+    for (int i = 0; i < D; ++i) {
+        double gi = 0.0;
+#pragma unroll
+        for (int r = 0; r < D; ++r) gi += mu[r] * (__ldg(V.matrix + r * D + i) + __ldg(V.matrix + i * D + r));
+        dv += fabs(gi) * dm[i];
+#pragma unroll
+        for (int j = 0; j < D; ++j) dv += fabs(__ldg(V.matrix + i * D + j)) * dm[i] * dm[j];
+    }
+    dv += poison;
+    if (V.flags & SLB_FLAG_SCALE) dv *= fabs(V.out_scale);
+    double dl = 0.0;
+    const slb_function& L = cfg.lipschitz_v;
+    if (L.kind == SLB_FN_LINEAR) {
+        const double sc = (L.flags & SLB_FLAG_SCALE) ? fabs(L.out_scale) : 1.0;
+        const int mo = L.out_dim;
+        double row[SLB_MAX_LIN_OUT];                       // row[o] = sum_i |A_oi| dm_i
+#pragma unroll
+        for (int o = 0; o < SLB_MAX_LIN_OUT; ++o) {
+            row[o] = 0.0;
+#pragma unroll
+            for (int i = 0; i < D; ++i)
+                if (o < mo) row[o] += fabs(__ldg(L.matrix + o * D + i)) * dm[i];
+        }
+        if ((L.flags & SLB_FLAG_NORM1) || mo == 1) {
+            double sb = bs[0];
+#pragma unroll
+            for (int j = 1; j < D; ++j) sb = f64add(sb, bs[j]);
+            dl = sc * (row[0] + row[1] + row[2] + row[3]) * sb;
+        } else {                                            // mo == D
+#pragma unroll
+            for (int j = 0; j < D; ++j) dl += sc * row[j] * bs[j];
+            if constexpr (D < 4) dl += 0.0 * sc;
+        }
+    }
+    return 1.000001 * (dv + dl);
+}
+
+// decide
+template <int D>
+SLB_DEV int cf_decide(const cf_terms<D>& t, const double (&shi)[D]) {
+    double ub = 0.0, lb = 0.0;
+#pragma unroll
+    for (int j = 0; j < D; ++j) {
+        const double e = t.coef[j] * shi[j];
+        ub += fmax(e, 0.0);
+        lb += fmin(e, 0.0);
+        if (!(e == e)) { ub = e; lb = e; }                 // NaN: both sums stay NaN from here on
+    }
+    const double slack = t.guard + 1e-6 * (fabs(ub) + fabs(lb));
+    if (t.dec0 + ub + slack < t.thr) return 1;
+    if (t.dec0 + lb - slack >= t.thr) return 0;
+    return -1;
+}
+
+// screened_outcome
+template <int D>
+SLB_DEV int cf_screened_outcome(const slb_sweep& cfg, double vx, double thr, const double (&mu)[D],
+                                const double (&dm)[D], const double (&shi)[D]) {
+    cf_terms<D> t;
+    t.thr = thr;
+    double zero[D];
+#pragma unroll
+    for (int j = 0; j < D; ++j) zero[j] = 0.0;
+    cf_mean_terms<D>(cfg, t, vx, mu, zero);
+    t.guard += cf_screening_slack<D>(cfg, mu, dm, shi);
+    return cf_decide<D>(t, shi);
+}
+
+// prior_sigma_bound for plain RBF factors
+template <int D>
+SLB_DEV void cf_prior_sigma(const slb_gp_stack& gp, double (&shi)[D]) {
+#pragma unroll
+    for (int j = 0; j < D; ++j) shi[j] = sqrt(gp.factors[gp.outputs[j].factor].variance);
+}
+
+// for_outputs_on_factor over D outputs: the outputs' indices in registers
+template <int D, class Fn>
+SLB_DEV void cf_for_outputs_on_factor(const slb_gp_stack& gp, int f, Fn&& fn) {
+    unsigned mask = 0;
+#pragma unroll
+    for (int o = 0; o < D; ++o)
+        if (gp.outputs[o].factor == f) mask |= 1u << o;
+    const auto call = [&](auto no) {
+        constexpr int NO = decltype(no)::value;
+        int outs[NO];
+        unsigned m = mask;
+#pragma unroll
+        for (int q = 0; q < NO; ++q) { outs[q] = __ffs(m) - 1; m &= m - 1; }
+        fn(no, outs);
+    };
+    switch (__popc(mask)) {
+    case 1: call(std::integral_constant<int, 1>{}); break;
+    case 2: if constexpr (D >= 2) call(std::integral_constant<int, 2>{}); break;
+    case 3: if constexpr (D >= 3) call(std::integral_constant<int, 3>{}); break;
+    case 4: if constexpr (D >= 4) call(std::integral_constant<int, 4>{}); break;
+    default: break;
+    }
+}
+
 // ---- stage 1: what its three kernels share -----------------------------------------------------------
 // x of a grid point, V(x), threshold(x), u = policy(x), z = [x, u]          (lyapunov.py:436, 284-288).
 // Returns whether z is sane: the expanded squared distance needs moderate magnitudes; NaN / huge inputs
@@ -413,10 +558,14 @@ filter_mean32_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a)
 // Thread t owns point t of the tile (row-major: the flag and V(x) stores are contiguous along the grid's
 // axis 1) in the prologue and the decision; in between, the tile's work items (factor, regime) alternate
 // between the two warp groups, which meet the points' z / regime and leave their mu / dm in shared memory.
-template <int DIN>
+// D = the number of outputs (= 2, the grid's dimension).  The kernel runs the closed form only
+// (grid_mean_applicable): the prologue and the decision keep every per-point operand in registers.
+constexpr int GRID_OUTPUTS = 2;        // a 2-D grid's GP stack has two outputs (slb_validate_sweep)
+
+template <int D>
 __global__ void __launch_bounds__(GT, 2)
 filter_grid_mean_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
-    static_assert(DIN == 3, "the factored grid mean is written for z = [x0, x1, u]");
+    static_assert(D == GRID_OUTPUTS, "the factored grid mean is written for z = [x0, x1, u]");
     stage1_mark(a, S1_ENTRY);
     extern __shared__ __align__(16) unsigned char smem_raw[];
     double* smem = reinterpret_cast<double*>(smem_raw);
@@ -434,12 +583,14 @@ filter_grid_mean_kernel(const __grid_constant__ slb_sweep cfg, const filter_args
         for (size_t off = (size_t)threadIdx.x * 128; off < bytes; off += (size_t)GT * 128)
             asm volatile("prefetch.global.L2 [%0];" ::"l"(reinterpret_cast<const char*>(cfg.gp.factors[f].Xf) + off));
     }
-    for (int o = 0; o < cfg.gp.num_outputs; ++o) {
+#pragma unroll
+    for (int o = 0; o < D; ++o) {
         const size_t bytes = (size_t)padded_rows(cfg.gp.factors[cfg.gp.outputs[o].factor].M) * sizeof(double);
         for (size_t off = (size_t)threadIdx.x * 128; off < bytes; off += (size_t)GT * 128)
             asm volatile("prefetch.global.L2 [%0];" ::"l"(reinterpret_cast<const char*>(cfg.gp.outputs[o].gamma_f) + off));
     }
-    const int64_t n0 = cfg.grid.num_points[0], n1 = cfg.grid.num_points[1];
+    const slb_grid& g = cfg.grid;
+    const int64_t n0 = g.num_points[0], n1 = g.num_points[1];
     const int64_t ntc = (n1 + GC - 1) / GC;
     const int64_t row0 = a.idx_begin / n1 + (int64_t)(blockIdx.x / ntc) * GR;
     const int64_t col0 = (int64_t)(blockIdx.x % ntc) * GC;
@@ -451,26 +602,32 @@ filter_grid_mean_kernel(const __grid_constant__ slb_sweep cfg, const filter_args
     const int64_t flat = gi * n1 + gk;
     const bool valid = gi < n0 && gk < n1 && flat >= a.idx_begin && flat < a.idx_begin + a.n;
     const int64_t rel = valid ? flat - a.idx_begin : 0;   // every thread stays for the block barriers
+    // grid_index_to_state of (gi, gk) (a point outside the range computes a state it never uses)
+    const double x[D] = {f64add(f64mul((double)gi, g.unit_maxes[0]), g.offset[0]),
+                         f64add(f64mul((double)gk, g.unit_maxes[1]), g.offset[1])};
     double vx, thr;
-    int reg;
-    bool sane;
+    lyapunov_state_terms_closed<D>(cfg, x, a.idx_begin + rel, &vx, &thr);
+    int cols;
+    const double u = eval_linear_reg<D, 1>(pol, x, cols).v[0];
+    // z must be sane: the expanded squared distance needs moderate magnitudes; NaN / huge inputs go to the
+    // full path
+    const bool sane = fabs(x[0]) < 1e100 && fabs(x[1]) < 1e100 && fabs(u) < 1e100;
+    zs[pt * 3 + 0] = x[0];
+    zs[pt * 3 + 1] = x[1];
+    zs[pt * 3 + 2] = u;
+    // the regime is the clip the policy computed: saturated points carry the constant itself
     {
-        double x[SLB_MAX_IN];
-        sane = stage1_point<DIN>(cfg, a.idx_begin + rel, x, &vx, &thr);
-#pragma unroll
-        for (int c = 0; c < 3; ++c) zs[pt * 3 + c] = x[c];
-        // the regime is the clip the policy computed: saturated points carry the constant itself
         const double ulo = (pol.flags & SLB_FLAG_SCALE) ? f64mul(pol.lower, pol.out_scale) : pol.lower;
         const double uhi = (pol.flags & SLB_FLAG_SCALE) ? f64mul(pol.upper, pol.out_scale) : pol.upper;
-        reg = !(valid && sane) ? -1
-              : (pol.flags & SLB_FLAG_SATURATE) && x[2] == ulo ? 0
-              : (pol.flags & SLB_FLAG_SATURATE) && x[2] == uhi ? 1 : 2;
+        const int reg = !(valid && sane) ? -1
+                        : (pol.flags & SLB_FLAG_SATURATE) && u == ulo ? 0
+                        : (pol.flags & SLB_FLAG_SATURATE) && u == uhi ? 1 : 2;
+        regs[pt] = (int8_t)reg;
+        const unsigned rbits = __reduce_or_sync(0xffffffffu, reg >= 0 ? 1u << reg : 0u);
+        if ((threadIdx.x & 31) == 0) present[threadIdx.x >> 5] = (int)rbits;
     }
-    regs[pt] = (int8_t)reg;
 #pragma unroll
     for (int o = 0; o < GNO; ++o) { mus[pt * GNO + o] = 0.0; dms[pt * GNO + o] = f64_inf(); }
-    const unsigned rbits = __reduce_or_sync(0xffffffffu, reg >= 0 ? 1u << reg : 0u);
-    if ((threadIdx.x & 31) == 0) present[threadIdx.x >> 5] = (int)rbits;
     __syncthreads();                              // z, regimes and the exp table visible
     stage1_mark(a, S1_PROLOGUE);
 
@@ -481,42 +638,98 @@ filter_grid_mean_kernel(const __grid_constant__ slb_sweep cfg, const filter_args
     const int grp = threadIdx.x / GGT;
     int item = 0;
     for (int f = 0; f < cfg.gp.num_factors; ++f) {
-        int outs[SLB_MAX_OUT], no = 0;                // the outputs on factor f (none: no item)
-        for (int o = 0; o < cfg.gp.num_outputs; ++o)
-            if (cfg.gp.outputs[o].factor == f) outs[no++] = o;
-        if (no == 0 || no > GNO) continue;
-        for (int r = 0; r < 3; ++r) {
-            if (!((regimes >> r) & 1)) continue;
-            if (item % GG == grp) {
-                // four outputs in two passes of two: four accumulator sets do not fit 128 registers.  Every
-                // output's sum is its own, so its mean is the same in either pass.
-                const int np = no == 4 ? 2 : no;
-                for (int q0 = 0; q0 < no; q0 += np) {
-                    double* gsm = smem + grp * GGRP;
-                    if (np == 1) grid_mean_item<1>(cfg, f, r, outs + q0, gsm, tab, row0, col0, zs, regs, mus, dms);
-                    else if (np == 2) grid_mean_item<2>(cfg, f, r, outs + q0, gsm, tab, row0, col0, zs, regs, mus, dms);
-                    else grid_mean_item<3>(cfg, f, r, outs + q0, gsm, tab, row0, col0, zs, regs, mus, dms);
+        cf_for_outputs_on_factor<D>(cfg.gp, f, [&](auto no, const int* outs) {
+            constexpr int NO = decltype(no)::value;
+            for (int r = 0; r < 3; ++r) {
+                if (!((regimes >> r) & 1)) continue;
+                if (item % GG == grp) {
+                    // four outputs in two passes of two: four accumulator sets do not fit 128 registers.  Every
+                    // output's sum is its own, so its mean is the same in either pass.
+                    constexpr int NP = NO == 4 ? 2 : NO;
+#pragma unroll
+                    for (int q0 = 0; q0 < NO; q0 += NP)
+                        grid_mean_item<NP>(cfg, f, r, outs + q0, smem + grp * GGRP, tab, row0, col0, zs, regs, mus,
+                                           dms);
+                    stage1_mark(a, S1_ITEM + min(item, 3));
                 }
-                stage1_mark(a, S1_ITEM + min(item, 3));
+                ++item;
             }
-            ++item;
-        }
+        });
     }
     __syncthreads();                              // every item's mu / dm visible
     stage1_mark(a, S1_MEANS);
 
     // ---- the comparison over mu +- dm and sigma_j in [0, prior sigma_j] (as filter_mean32_kernel)
-    double m[SLB_MAX_OUT], d[SLB_MAX_OUT];
+    double mu[D], dm[D], shi[D];
 #pragma unroll
-    for (int j = 0; j < SLB_MAX_OUT; ++j) {
-        m[j] = j < GNO ? mus[pt * GNO + j] : 0.0;
-        d[j] = j < GNO ? dms[pt * GNO + j] : 0.0;
+    for (int j = 0; j < D; ++j) {
+        mu[j] = mus[pt * GNO + j];
+        dm[j] = sane ? dms[pt * GNO + j] : f64_inf();
     }
-    filter_side t;
-    t.thr = thr;
+    if (a.probe_mu != nullptr && valid) {
 #pragma unroll
-    for (int c = 0; c < DIN; ++c) t.z[c] = zs[pt * 3 + c];
-    stage1_screened_finish<DIN>(cfg, a, valid, sane, rel, t, vx, m, d);
+        for (int o = 0; o < D; ++o) {
+            a.probe_mu[rel * D + o] = mu[o];
+            a.probe_dm[rel * D + o] = dm[o];
+        }
+    }
+    cf_prior_sigma<D>(cfg.gp, shi);
+    const int outcome = sane ? cf_screened_outcome<D>(cfg, vx, thr, mu, dm, shi) : -1;
+    const bool undecided = valid && outcome < 0;
+    if (valid) {
+        a.negative[rel] = outcome > 0 ? 1 : 0;
+        if (a.values != nullptr) a.values[rel] = vx;
+    }
+    bool fp64 = sane;                             // every bound finite: an fp64-class mean
+#pragma unroll
+    for (int j = 0; j < D; ++j) fp64 &= dm[j] < f64_inf();
+    // per warp: list A entries, decided points, valid points, entries without an fp64-class mean; then the
+    // CTA's first list A slot.  One global atomic per counter and CTA instead of one per warp.  They take
+    // the place of z, which no one reads after the means.
+    constexpr int NW = GT / 32;
+    unsigned* s_cnt = reinterpret_cast<unsigned*>(zs);                       // [4][NW]
+    unsigned long long* s_base = reinterpret_cast<unsigned long long*>(s_cnt + 4 * NW);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const unsigned und = __ballot_sync(0xffffffffu, undecided);
+    {
+        const unsigned dec = __ballot_sync(0xffffffffu, valid && !undecided);
+        const unsigned val = __ballot_sync(0xffffffffu, valid);
+        const unsigned open = __ballot_sync(0xffffffffu, undecided && !fp64);
+        if (lane == 0) {
+            s_cnt[0 * NW + warp] = __popc(und);
+            s_cnt[1 * NW + warp] = __popc(dec);
+            s_cnt[2 * NW + warp] = __popc(val);
+            s_cnt[3 * NW + warp] = __popc(open);
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x < 4) {
+        unsigned total = 0;
+#pragma unroll
+        for (int w = 0; w < NW; ++w) total += s_cnt[threadIdx.x * NW + w];
+        if (threadIdx.x == 0) *s_base = total != 0 ? atomicAdd(a.counts + 0, (unsigned long long)total) : 0;
+        else if (total != 0 && threadIdx.x == 3) atomicAdd(a.counts + 2, (unsigned long long)total);
+        else if (total != 0 && a.stats != nullptr) atomicAdd(a.stats + (threadIdx.x == 1 ? 0 : 3), (unsigned long long)total);
+    }
+    __syncthreads();
+    if (undecided) {
+        // the list A entry in the screened layout: V(x) in dec0, the threshold, z, the mean and its bound (the
+        // head stage rebuilds the mean-dependent terms)
+        unsigned long long slot = *s_base + __popc(und & ((1u << lane) - 1));
+        for (int w = 0; w < warp; ++w) slot += s_cnt[w];
+        a.list_a[slot] = rel;
+        filter_side* dst = a.side_a + slot;
+        dst->dec0 = vx;
+        dst->thr = thr;
+        dst->z[0] = x[0];
+        dst->z[1] = x[1];
+        dst->z[2] = u;
+#pragma unroll
+        for (int j = 0; j < D; ++j) {
+            dst->coef[j] = mu[j];
+            dst->dm[j] = dm[j];
+        }
+    }
     timing_mark(a, HEAD_CTAS * 8);
     stage1_mark(a, S1_EXIT);
 }
@@ -582,7 +795,7 @@ SLB_DEV void head_mean_factor(const double* __restrict__ xf, int Mp, const doubl
 // duration is the latency of one group) still spreads the M exps per point and factor over its threads.
 // Results: mu_s / merr_s [slot][SLB_MAX_OUT] in shared memory.  The threads [tid0, tid0 + nthreads) of
 // the CTA (whole warps) take part; `slots` nullptr: the entries are slots 0 .. nneed - 1.
-template <int DIN>
+template <int DIN, int CD>
 SLB_DEV void head_round_means(const slb_sweep& cfg, const filter_args& a, const int* slots, int nneed,
                               int64_t grp0, int64_t count, const double* mbuf, const double* tab512,
                               double* mu_s, double* merr_s, int tid0, int nthreads) {
@@ -611,18 +824,27 @@ SLB_DEV void head_round_means(const slb_sweep& cfg, const filter_args& a, const 
             zz *= -0.5;
             const int Mp = padded_rows(F.M);
             const double* xf = mbuf + a.plan.mean_off[f];
-            for_outputs_on_factor(cfg.gp, f, [&](auto no, const int* outs) {
+            const auto factor_means = [&](auto no, const int* outs) {
                 constexpr int NO = decltype(no)::value;
                 double dot[NO];
                 head_mean_factor<DIN, NO>(xf, Mp, zs, zz, r, L, tab512, dot);
                 if (r == 0 && live) {
-#pragma unroll 1                                   // cold, once per entry: one copy of the finish per NO
-                    for (int q = 0; q < NO; ++q)
+                    const auto finish = [&](int q) {
                         mean_output_finish<DIN>(F, cfg.gp.outputs[outs[q]], z, dot[q], zz, 1.0, false,
                                                 &mu_s[slot * SLB_MAX_OUT + outs[q]],
                                                 &merr_s[slot * SLB_MAX_OUT + outs[q]]);
+                    };
+                    if constexpr (CD > 0) {
+#pragma unroll                                     // closed form: dot and outs stay in registers
+                        for (int q = 0; q < NO; ++q) finish(q);
+                    } else {
+#pragma unroll 1                                   // cold, once per entry: one copy of the finish per NO
+                        for (int q = 0; q < NO; ++q) finish(q);
+                    }
                 }
-            });
+            };
+            if constexpr (CD == 0) for_outputs_on_factor(cfg.gp, f, factor_means);
+            else cf_for_outputs_on_factor<CD>(cfg.gp, f, factor_means);
         }
     }
 }
@@ -644,14 +866,14 @@ SLB_DEV void head_group_entries(const slb_sweep& cfg, const filter_args& a, int6
 
 // sigma of factor f (head_rows > 0) given its head subset, for the HP entries of a group on one warp
 // (lane p: entry p's; the other lanes' values are meaningless)
-template <int DIN, bool ALL_STAGED>
-SLB_DEV double head_factor_sdev(const slb_sweep& cfg, const filter_args& a, int f, const filter_side& t,
+template <int DIN, bool ALL_STAGED, bool PLAIN>
+SLB_DEV double head_factor_sdev(const slb_sweep& cfg, const filter_args& a, int f, const double* z,
                                 bool mine, const double* exptab, double* kw, const double* wbuf,
                                 const double* xbuf, uint64_t* bar) {
     const int lane = threadIdx.x & 31;
     const slb_gp_factor& F = cfg.gp.factors[f];
     const int rows = F.head_rows;
-    const bool general = F.kernel.num_prims > 0;
+    const bool general = !PLAIN && F.kernel.num_prims > 0;
     const double s2 = f64mul(F.scale, F.scale);
     // ALL_STAGED: the tables are known to be in shared memory (LDS instead of generic loads)
     const bool staged = ALL_STAGED || f < a.plan.factors_staged;
@@ -661,7 +883,7 @@ SLB_DEV double head_factor_sdev(const slb_sweep& cfg, const filter_args& a, int 
     // (functions.py:438); entries beyond the list carry zeros (never decided)
     double zown[DIN];                       // this lane's point in the factor's units (one division
 #pragma unroll                              // per lane and dimension instead of one per point)
-    for (int c = 0; c < DIN; ++c) zown[c] = general ? t.z[c] : t.z[c] / F.lengthscales[c];
+    for (int c = 0; c < DIN; ++c) zown[c] = general ? z[c] : z[c] / F.lengthscales[c];
 #pragma unroll
     for (int p = 0; p < HP; ++p) {
         double zs[DIN];
@@ -723,24 +945,26 @@ SLB_DEV double head_factor_sdev(const slb_sweep& cfg, const filter_args& a, int 
     const double s1 = __shfl_sync(0xffffffffu, v1, (lane >> 1) & 3);
     ssp = (lane & 1) ? s1 : s0;
     double kss = F.kss;
-    if (general && mine) kss = s2 * kernel_expr_diag<DIN>(F.kernel, t.z);
+    if (general && mine) kss = s2 * kernel_expr_diag<DIN>(F.kernel, z);
     const double sdev = sqrt(f64sub(kss, ssp) / s2);          // NaN if negative
     return sdev;
 }
 
-// one group of HP list entries [g HP, g HP + HP) on one warp, factor after factor
-template <int DIN, bool ALL_STAGED>
-SLB_DEV void head_group_bound(const slb_sweep& cfg, const filter_args& a, int64_t grp, int64_t count,
+// the sigma bounds of one group of HP list entries [g HP, g HP + HP) on one warp (lane p: entry p, loaded by
+// head_group_entries), factor after factor; D outputs (CD > 0: the closed form)
+template <int DIN, bool ALL_STAGED, int CD, int D>
+SLB_DEV void head_group_bound(const slb_sweep& cfg, const filter_args& a, const double* z, bool mine,
                               const double* exptab, double* kw, const double* wbuf, const double* xbuf,
-                              uint64_t* bar, filter_side& t, int64_t& rel, bool& mine, double* shi) {
-    head_group_entries<DIN>(cfg, a, grp, count, t, rel, mine, shi);
+                              uint64_t* bar, double (&shi)[D]) {
     slb_bulk::mbar_wait(bar + 0, 0);            // exp tables and subset inputs have landed
     head_mark(a, HM_TABLES);
     for (int f = 0; f < cfg.gp.num_factors; ++f) {
         if (cfg.gp.factors[f].head_rows <= 0) continue;
-        const double sdev = head_factor_sdev<DIN, ALL_STAGED>(cfg, a, f, t, mine, exptab, kw, wbuf, xbuf, bar);
-        for (int j = 0; j < cfg.gp.num_outputs; ++j)
-            if (cfg.gp.outputs[j].factor == f) shi[j] = sdev;
+        const double sdev = head_factor_sdev<DIN, ALL_STAGED, (CD > 0)>(cfg, a, f, z, mine, exptab, kw, wbuf, xbuf,
+                                                                        bar);
+#pragma unroll
+        for (int j = 0; j < D; ++j)
+            if (j < cfg.gp.num_outputs && cfg.gp.outputs[j].factor == f) shi[j] = sdev;
         if (f == 0) head_mark(a, HM_BOUND0);
     }
     head_mark(a, HM_BOUND);
@@ -786,6 +1010,76 @@ SLB_DEV int head_mean_decision(const slb_sweep& cfg, filter_side& t, double vx, 
     return decide(t, shi, cfg.gp.num_outputs);
 }
 
+// The three functions above for the closed form (head stage behind the grid kernel, D outputs): the
+// entry's fields in registers, the decision of stage 1 (cf_screened_outcome).  Only z goes in before the
+// sigma bounds; the other fields are loaded for the decision (fewer registers live across the DMMA chain).
+template <int DIN, int D>
+struct cf_entry { int k; int64_t rel; double vx, thr, z[DIN], mu[D], dm[D]; };   // k: list index, -1: none
+
+template <int DIN, int D>
+SLB_DEV void head_group_entries(const slb_sweep& cfg, const filter_args& a, int64_t grp, int64_t count,
+                                cf_entry<DIN, D>& t, int64_t& rel, bool& mine, double (&shi)[D]) {
+    const int lane = threadIdx.x & 31;
+    const int64_t k = grp * HP + min(lane, HP - 1);
+    mine = lane < HP && k < count;
+    t.k = mine ? (int)k : -1;
+#pragma unroll
+    for (int c = 0; c < DIN; ++c) t.z[c] = mine ? a.side_a[k].z[c] : 0.0;
+    rel = 0;                                    // t.rel, loaded with the decision's fields
+    cf_prior_sigma<D>(cfg.gp, shi);
+    if (!mine) {
+#pragma unroll
+        for (int j = 0; j < D; ++j) shi[j] = 0.0;
+    }
+}
+
+template <int DIN, int D>
+SLB_DEV int head_entry_decision(const slb_sweep& cfg, const filter_args& a, cf_entry<DIN, D>& t,
+                                const double (&shi)[D], bool mine, double& vx, bool& need) {
+    t.rel = 0;
+    t.vx = 0.0;
+    t.thr = 0.0;
+#pragma unroll
+    for (int j = 0; j < D; ++j) { t.mu[j] = 0.0; t.dm[j] = 0.0; }
+    if (t.k >= 0) {
+        t.rel = a.list_a[t.k];
+        const filter_side* e = a.side_a + t.k;
+        t.vx = e->dec0;
+        t.thr = e->thr;
+#pragma unroll
+        for (int j = 0; j < D; ++j) { t.mu[j] = e->coef[j]; t.dm[j] = e->dm[j]; }
+    }
+    vx = t.vx;
+    const int screened = cf_screened_outcome<D>(cfg, vx, t.thr, t.mu, t.dm, shi);
+    const int outcome = mine ? screened : 0;
+    bool finite = true;                         // an fp64-class mean (the grid kernel's entries)
+#pragma unroll
+    for (int j = 0; j < D; ++j) finite &= t.dm[j] < f64_inf();
+    need = mine && outcome < 0 && !finite;
+    head_mark(a, HM_SCREENED);
+    return outcome;
+}
+
+template <int DIN, int D>
+SLB_DEV int head_mean_decision(const slb_sweep& cfg, cf_entry<DIN, D>& t, double vx, const double (&shi)[D],
+                               const double* mu_s, const double* merr_s, int slot) {
+    double mu[D], merr[D];
+#pragma unroll
+    for (int j = 0; j < D; ++j) {
+        mu[j] = mu_s[slot * SLB_MAX_OUT + j];
+        merr[j] = merr_s[slot * SLB_MAX_OUT + j];
+    }
+    cf_terms<D> terms;
+    terms.thr = t.thr;
+    cf_mean_terms<D>(cfg, terms, vx, mu, merr);
+    return cf_decide<D>(terms, shi);
+}
+
+// the grid index of an entry (generic: the one head_group_entries loaded)
+SLB_DEV int64_t entry_rel(const filter_side&, int64_t rel) { return rel; }
+template <int DIN, int D>
+SLB_DEV int64_t entry_rel(const cf_entry<DIN, D>& t, int64_t) { return t.rel; }
+
 // every copy lands in this CTA's shared memory before the CTA may leave
 SLB_DEV void head_wait_landings(uint64_t* bar) {
     for (int b = 0; b < 3; ++b) slb_bulk::mbar_wait(bar + b, 0);
@@ -806,9 +1100,13 @@ SLB_DEV void head_group_finish(const filter_args& a, bool mine, int outcome, int
     }
 }
 
-template <int DIN>
+// CD = 0: every plan.  CD = D > 0: the closed form behind the grid kernel (SLB_MEAN_GRID_FACTORED, D outputs):
+// list entries loaded into registers, the decision of stage 1
+template <int DIN, int CD>
 __global__ void __launch_bounds__(HT, 1)
 filter_head_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
+    constexpr int ND = CD > 0 ? CD : SLB_MAX_OUT;
+    using entry_t = std::conditional_t<(CD > 0), cf_entry<DIN, ND>, filter_side>;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     if (threadIdx.x == 0) head_mark(a, HM_ENTRY);
     prefetch_descriptor_operands(cfg);
@@ -934,15 +1232,13 @@ filter_head_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
                     if (cfg.gp.factors[f].head_rows <= 0) continue;
                     const int64_t k = (grp0 + (int64_t)i * gridDim.x) * HP + min(lane, HP - 1);
                     const bool mine = lane < HP && k < count;
-                    filter_side tz = {};
-                    if (mine) {
+                    double tz[DIN];
 #pragma unroll
-                        for (int c = 0; c < DIN; ++c) tz.z[c] = a.side_a[k].z[c];
-                    }
+                    for (int c = 0; c < DIN; ++c) tz[c] = mine ? a.side_a[k].z[c] : 0.0;
                     const double sd =
                         lay.factors_staged == nf
-                            ? head_factor_sdev<DIN, true>(cfg, a, f, tz, mine, exptab, kw, wbuf, xbuf, bar)
-                            : head_factor_sdev<DIN, false>(cfg, a, f, tz, mine, exptab, kw, wbuf, xbuf, bar);
+                            ? head_factor_sdev<DIN, true, (CD > 0)>(cfg, a, f, tz, mine, exptab, kw, wbuf, xbuf, bar)
+                            : head_factor_sdev<DIN, false, (CD > 0)>(cfg, a, f, tz, mine, exptab, kw, wbuf, xbuf, bar);
                     if (lane < HP) sd_s[(i * HP + lane) * SLB_MAX_OUT + f] = sd;
                     if (f == 0) head_mark(a, HM_BOUND0);
                 }
@@ -950,7 +1246,7 @@ filter_head_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
             } else if (early_means) {
                 slb_bulk::mbar_wait(bar + 0, 0);
                 slb_bulk::mbar_wait(bar + 2, 0);
-                head_round_means<DIN>(cfg, a, nullptr, ngr * HP, grp0, count, mbuf, tab512, mu_s, merr_s,
+                head_round_means<DIN, CD>(cfg, a, nullptr, ngr * HP, grp0, count, mbuf, tab512, mu_s, merr_s,
                                       nbw * 32, HT - nbw * 32);
                 head_mark(a, HM_MEANS);
             }
@@ -958,18 +1254,20 @@ filter_head_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
             if (means && !early_means) {                  // no warp to spare: the means after the bounds
                 slb_bulk::mbar_wait(bar + 0, 0);
                 slb_bulk::mbar_wait(bar + 2, 0);
-                head_round_means<DIN>(cfg, a, nullptr, ngr * HP, grp0, count, mbuf, tab512, mu_s, merr_s, 0, HT);
+                head_round_means<DIN, CD>(cfg, a, nullptr, ngr * HP, grp0, count, mbuf, tab512, mu_s, merr_s, 0, HT);
                 head_mark(a, HM_MEANS);
                 __syncthreads();
             }
             if (warp < ngr) {
-                filter_side t;
+                entry_t t;
                 int64_t rel;
                 bool mine;
-                double shi[SLB_MAX_OUT];
+                double shi[ND];
                 head_group_entries<DIN>(cfg, a, grp0 + (int64_t)warp * gridDim.x, count, t, rel, mine, shi);
                 const int slot = warp * HP + min(lane, HP - 1);
-                for (int j = 0; j < cfg.gp.num_outputs; ++j) {
+#pragma unroll
+                for (int j = 0; j < ND; ++j) {
+                    if (j >= cfg.gp.num_outputs) break;
                     const int f = cfg.gp.outputs[j].factor;
                     if (cfg.gp.factors[f].head_rows > 0) shi[j] = sd_s[slot * SLB_MAX_OUT + f];
                 }
@@ -978,7 +1276,7 @@ filter_head_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
                 int outcome = head_entry_decision(cfg, a, t, shi, mine, vx, need);
                 if (need) outcome = head_mean_decision(cfg, t, vx, shi, mu_s, merr_s, slot);
                 head_mark(a, HM_DECIDED);
-                head_group_finish(a, mine, outcome, rel, s_stat);
+                head_group_finish(a, mine, outcome, entry_rel(t, rel), s_stat);
             }
             __syncthreads();                              // sd_s, mu_s are the next round's
         }
@@ -989,17 +1287,18 @@ filter_head_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
             const int64_t grp = grp0 + (int64_t)warp * gridDim.x;
             const bool active = grp < ngroups;
             const int lane = threadIdx.x & 31;
-            filter_side t;
+            entry_t t;
             int64_t rel = 0;
             bool mine = false, need = false;
-            double shi[SLB_MAX_OUT];
+            double shi[ND];
             double vx = 0.0;
             int outcome = 0;
             if (active) {
+                head_group_entries<DIN>(cfg, a, grp, count, t, rel, mine, shi);
                 if (lay.factors_staged == nf)
-                    head_group_bound<DIN, true>(cfg, a, grp, count, exptab, kw, wbuf, xbuf, bar, t, rel, mine, shi);
+                    head_group_bound<DIN, true, CD>(cfg, a, t.z, mine, exptab, kw, wbuf, xbuf, bar, shi);
                 else
-                    head_group_bound<DIN, false>(cfg, a, grp, count, exptab, kw, wbuf, xbuf, bar, t, rel, mine, shi);
+                    head_group_bound<DIN, false, CD>(cfg, a, t.z, mine, exptab, kw, wbuf, xbuf, bar, shi);
                 outcome = head_entry_decision(cfg, a, t, shi, mine, vx, need);
                 if (need) need_s[2 + atomicAdd(need_s + (round & 1), 1)] = warp * HP + lane;
             }
@@ -1010,7 +1309,7 @@ filter_head_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
                 if (nneed > 0) {
                     // the rest gets its mean in fp64 (all warps), then the same comparison as the fp64 path
                     slb_bulk::mbar_wait(bar + 2, 0);
-                    head_round_means<DIN>(cfg, a, need_s + 2, nneed, grp0, count, mbuf, tab512, mu_s, merr_s, 0, HT);
+                    head_round_means<DIN, CD>(cfg, a, need_s + 2, nneed, grp0, count, mbuf, tab512, mu_s, merr_s, 0, HT);
                     head_mark(a, HM_MEANS);
                     __syncthreads();
                     if (need) outcome = head_mean_decision(cfg, t, vx, shi, mu_s, merr_s, warp * HP + lane);
@@ -1018,7 +1317,7 @@ filter_head_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
             }
             if (active) {
                 head_mark(a, HM_DECIDED);
-                head_group_finish(a, mine, outcome, rel, s_stat);
+                head_group_finish(a, mine, outcome, entry_rel(t, rel), s_stat);
             }
         }
     }
@@ -1059,14 +1358,22 @@ bool screening_applicable(const slb_sweep& cfg) {
 }
 
 // The factored grid kernel replaces the fp32 screening kernel (same list A layout) where kernel values
-// factor over the grid axes: a 2-D grid, z = [x0, x1, u] with plain RBF factors (screening_applicable)
-// and u = a x0 + b x1, optionally saturated and scaled.
+// factor over the grid axes: a 2-D grid (so two outputs), z = [x0, x1, u] with plain RBF factors
+// (screening_applicable) and u = a x0 + b x1, optionally saturated and scaled.  Its per-point terms are
+// the closed form of the register-only evaluators (common.cuh), so L_f is a constant, a table or a LINEAR
+// map as well.
 bool grid_mean_applicable(const slb_sweep& cfg) {
     if (g_filter_stages & 32) return false;
     const slb_function& P = cfg.policy;
+    const slb_function& Lf = cfg.lipschitz_f;
+    const bool lf_closed = Lf.kind == SLB_FN_NONE || cfg.lf_values != nullptr ||
+                           (Lf.kind == SLB_FN_LINEAR && Lf.in_dim == 2 && Lf.out_dim <= SLB_MAX_LIN_OUT &&
+                            Lf.matrix != nullptr &&
+                            !(Lf.flags & ~(uint32_t)(SLB_FLAG_SATURATE | SLB_FLAG_ABS | SLB_FLAG_NORM1 |
+                                                     SLB_FLAG_SCALE)));
     return screening_applicable(cfg) && cfg.grid.ndim == 2 && cfg.gp.input_dim == 3 &&
            P.kind == SLB_FN_LINEAR && P.in_dim == 2 && P.out_dim == 1 && P.matrix != nullptr &&
-           !(P.flags & ~(uint32_t)(SLB_FLAG_SATURATE | SLB_FLAG_SCALE));
+           !(P.flags & ~(uint32_t)(SLB_FLAG_SATURATE | SLB_FLAG_SCALE)) && lf_closed;
 }
 
 // Which stage 1 runs and the shared-memory layout of the head stage (one CTA per SM): which factors' head
@@ -1118,28 +1425,34 @@ int launch_filter(cudaStream_t st, const slb_sweep& cfg, const filter_args& a) {
                                       cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
         SLB_CUDA(cudaFuncSetAttribute(filter_mean32_kernel<DIN>,
                                       cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-        SLB_CUDA(cudaFuncSetAttribute(filter_head_kernel<DIN>,
+        SLB_CUDA(cudaFuncSetAttribute(filter_head_kernel<DIN, 0>,
                                       cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
         if constexpr (DIN == 3) {
-            SLB_CUDA(cudaFuncSetAttribute(filter_grid_mean_kernel<DIN>,
+            SLB_CUDA(cudaFuncSetAttribute(filter_head_kernel<DIN, GRID_OUTPUTS>,
+                                          cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+            SLB_CUDA(cudaFuncSetAttribute(filter_grid_mean_kernel<GRID_OUTPUTS>,
                                           cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           (int)grid_mean_smem_bytes()));
             // all of the unified L1 / shared memory as shared: two 111 KB CTAs per SM
-            SLB_CUDA(cudaFuncSetAttribute(filter_grid_mean_kernel<DIN>,
+            SLB_CUDA(cudaFuncSetAttribute(filter_grid_mean_kernel<GRID_OUTPUTS>,
                                           cudaFuncAttributePreferredSharedMemoryCarveout,
                                           (int)cudaSharedmemCarveoutMaxShared));
         }
         if (device >= 0 && device < 64) configured[device].store(true, std::memory_order_release);
     }
     const int64_t blocks = (a.n + FT - 1) / FT;
+    // the grid kernel and the head stage behind it run the closed form: d_in = 3 and two outputs
+    const bool closed = a.plan.mean_scheme == SLB_MEAN_GRID_FACTORED;
+    SLB_CHECK(!closed || (DIN == 3 && cfg.gp.num_outputs == GRID_OUTPUTS),
+              "filtered sweep: the factored grid mean needs d_in = 3 and %d outputs", GRID_OUTPUTS);
     switch (a.plan.mean_scheme) {
-    case SLB_MEAN_GRID_FACTORED:                  // d_in = 3 (grid_mean_applicable)
+    case SLB_MEAN_GRID_FACTORED:
         if constexpr (DIN == 3) {
             // tiles of GR rows x GC columns over the rows the range touches (it may start and end mid-row)
             const int64_t n1 = cfg.grid.num_points[1];
             const int64_t r0 = a.idx_begin / n1, r1 = (a.idx_begin + a.n - 1) / n1;
             const int64_t tiles = ((r1 - r0) / GR + 1) * ((n1 + GC - 1) / GC);
-            filter_grid_mean_kernel<DIN><<<(unsigned)tiles, GT, grid_mean_smem_bytes(), st>>>(cfg, a);
+            filter_grid_mean_kernel<GRID_OUTPUTS><<<(unsigned)tiles, GT, grid_mean_smem_bytes(), st>>>(cfg, a);
         }
         break;
     case SLB_MEAN_FP32_SCREENED:
@@ -1152,7 +1465,13 @@ int launch_filter(cudaStream_t st, const slb_sweep& cfg, const filter_args& a) {
     }
     SLB_LAUNCH_CHECK();
     if (!(g_filter_stages & 1)) return 0;
-    filter_head_kernel<DIN><<<HEAD_CTAS, HT, (size_t)a.plan.doubles * sizeof(double), st>>>(cfg, a);
+    const size_t head_smem = (size_t)a.plan.doubles * sizeof(double);
+    if constexpr (DIN == 3) {
+        if (closed) filter_head_kernel<DIN, GRID_OUTPUTS><<<HEAD_CTAS, HT, head_smem, st>>>(cfg, a);
+        else filter_head_kernel<DIN, 0><<<HEAD_CTAS, HT, head_smem, st>>>(cfg, a);
+    } else {
+        filter_head_kernel<DIN, 0><<<HEAD_CTAS, HT, head_smem, st>>>(cfg, a);
+    }
     SLB_LAUNCH_CHECK();
     return 0;
 }
