@@ -69,7 +69,13 @@ enum slb_fn_kind {
     SLB_FN_PENDULUM = 5,       /* InvertedPendulum            examples/utilities.py:144-289 */
     SLB_FN_CARTPOLE = 6,       /* CartPole                    examples/utilities.py:292-437 */
     SLB_FN_LYAPUNOV_NN = 7,    /* LyapunovNetwork             examples/utilities.py:48-104  */
-    SLB_FN_MLP = 8             /* NeuralNetwork               functions.py:1702-1729        */
+    SLB_FN_MLP = 8,            /* NeuralNetwork               functions.py:1702-1729        */
+    SLB_FN_VANDERPOL = 9       /* VanDerPol (reverse time)    examples/utilities.py:440-519
+                                  maps [x, y, u] (3 inputs, u ignored) to 2 columns; cparams:
+                                  [0] damping, [1] dt / 10, [2] 1 if normalised, [3..4] Tx,
+                                  [5..6] 1 / Tx.  The normalisation is the reference's
+                                  state . diag(T): column j = s_j T_j + s_(1-j) 0, so an inf or
+                                  NaN component makes the other column NaN */
 };
 /* post-ops, applied in this order: saturate -> abs -> norm1 | maxabs -> out_scale */
 #define SLB_FLAG_SATURATE 1u   /* Saturation  functions.py:349-354                     */
@@ -213,7 +219,7 @@ typedef struct slb_gp_stack {
 
 /* ---- one Lyapunov sweep: the graph of lyapunov.py:433-441 -----------------------------
  * Shapes.  A function's COLUMNS are what it returns after its post-ops: out_dim, except 1 for
- * QUADRATIC and LYAPUNOV_NN, 2 for PENDULUM, 4 for CARTPOLE, in_dim for a network gradient
+ * QUADRATIC and LYAPUNOV_NN, 2 for PENDULUM and VANDERPOL, 4 for CARTPOLE, in_dim for a network gradient
  * (SLB_FLAG_GRADIENT on LYAPUNOV_NN / MLP with out_dim = in_dim), and 1 after NORM1 or MAXABS.  With
  * d = grid.ndim and m = the policy's columns:
  *   policy        d inputs, m = 1..SLB_MAX_ACT columns
@@ -605,7 +611,8 @@ int slb_value_solve(void* stream, int64_t n, int32_t ncols, const void* cols_dev
  *                                   the plants, which have no parameters
  *        out_dev         [n, out] = the forward pass recomputed by the gradient kernel, bit-identical to
  *                                   slb_eval_function (or NULL)
- *      Kinds MLP, LYAPUNOV_NN, PENDULUM and CARTPOLE (and TRIANGULATION, below) without post-op flags.  Gradient conventions: ReLU' = 0
+ *      Kinds MLP, LYAPUNOV_NN, PENDULUM, CARTPOLE and VANDERPOL (and TRIANGULATION, below) without post-op
+ *      flags; VANDERPOL's action column gets a zero gradient.  Gradient conventions: ReLU' = 0
  *      at 0, tanh' = 1 - tanh^2.  The parameter gradient is reduced in a fixed order without atomics: two
  *      calls with the same inputs give bit-identical results.  n == 0 zeroes grad_params and launches
  *      nothing.  workspace_dev: >= slb_function_vjp_workspace(fn, n) bytes when grad_params_dev is

@@ -20,7 +20,7 @@ SLB_HEAD_RANK = 64
 SLB_MAX_RANKS = 16
 
 FN_NONE, FN_CONSTANT, FN_LINEAR, FN_QUADRATIC, FN_TRIANGULATION, FN_PENDULUM, FN_CARTPOLE, \
-    FN_LYAPUNOV_NN, FN_MLP = range(9)
+    FN_LYAPUNOV_NN, FN_MLP, FN_VANDERPOL = range(10)
 FLAG_SATURATE, FLAG_ABS, FLAG_NORM1, FLAG_PROJECT, FLAG_SCALE, FLAG_GRADIENT, FLAG_MAXABS = \
     1, 2, 4, 8, 16, 32, 64
 K_RBF, K_MATERN12, K_MATERN32, K_MATERN52, K_LINEAR, K_CONSTANT, K_WHITE = range(7)

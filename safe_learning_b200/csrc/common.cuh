@@ -479,6 +479,31 @@ SLB_DEV void eval_cartpole(const slb_function& f, const double* in, double* out)
     for (int c = 0; c < 4; ++c) out[c] = s[c];
 }
 
+// reverse-time Van der Pol (examples/utilities.py:440-519); cparams layout in include/slb200.h.  The
+// (de)normalisation is the reference's tf.matmul(state, diag(T)), written out: each column adds the other
+// component times 0, so an inf or NaN component turns the other column into NaN, as the matmul does.
+SLB_DEV void vanderpol_scale(double& x, double& y, double tx, double ty) {
+    const double xs = f64add(f64mul(x, tx), f64mul(y, 0.0));
+    y = f64add(f64mul(x, 0.0), f64mul(y, ty));
+    x = xs;
+}
+
+SLB_DEV void eval_vanderpol(const slb_function& f, const double* in, double* out) {
+    const double* p = f.cparams;
+    const double damping = p[0], dt = p[1];
+    const bool has_norm = p[2] != 0.0;
+    double x = in[0], y = in[1];
+    if (has_norm) vanderpol_scale(x, y, p[3], p[4]);
+    for (int i = 0; i < 10; ++i) {
+        // x' = -y, y' = x + damping (x^2 - 1) y, rounded left to right; state + dt * derivative
+        const double y_dot = f64add(x, f64mul(f64mul(damping, f64sub(f64mul(x, x), 1.0)), y));
+        x = f64add(x, f64mul(dt, -y));
+        y = f64add(y, f64mul(dt, y_dot));
+    }
+    if (has_norm) vanderpol_scale(x, y, p[5], p[6]);
+    out[0] = x; out[1] = y;
+}
+
 // ---- the fused networks: LyapunovNetwork (examples/utilities.py:85-104: h <- act(h . K_l^T), V = |h|^2)
 // and NeuralNetwork (functions.py:1702-1729: dense layers, output multiplied by output_scale).
 // Descriptor layout, written by _TrainableNetwork._network_descriptor (functions.py) and read only through
@@ -656,6 +681,9 @@ SLB_EVAL_ATTR int eval_fn(const slb_function& f, const double* in, double* out) 
         break;
     case SLB_FN_CARTPOLE:
         eval_cartpole(f, in, out); od = 4;
+        break;
+    case SLB_FN_VANDERPOL:
+        eval_vanderpol(f, in, out); od = 2;
         break;
     // SLB_NO_NETWORK_GRADIENT (value_opt.cu): the unit's host entry points reject network gradients, and
     // its kernels are compiled without the call (with it, ptxas gives value_operator_kernel<5, 6> 128

@@ -107,6 +107,9 @@ int slb_validate_function(const slb_function* f, const char* what, int expect_in
     case SLB_FN_CARTPOLE:
         SLB_CHECK(f->in_dim == 5 && f->out_dim == 4, "%s: cart-pole must map 5 -> 4", what);
         break;
+    case SLB_FN_VANDERPOL:
+        SLB_CHECK(f->in_dim == 3 && f->out_dim == 2, "%s: Van der Pol must map 3 -> 2", what);
+        break;
     case SLB_FN_LYAPUNOV_NN:
     case SLB_FN_MLP: {        // LyapunovNetwork has one output, NeuralNetwork its last layer's width
         const char* name = f->kind == SLB_FN_MLP ? "NeuralNetwork" : "LyapunovNetwork";
@@ -151,7 +154,7 @@ int slb_fn_columns(const slb_function& f) {
         if ((f.flags & SLB_FLAG_GRADIENT) && f.out_dim == f.in_dim) return f.in_dim;
         return f.kind == SLB_FN_MLP ? f.out_dim : 1;
     case SLB_FN_QUADRATIC: return 1;
-    case SLB_FN_PENDULUM: return 2;
+    case SLB_FN_PENDULUM: case SLB_FN_VANDERPOL: return 2;
     case SLB_FN_CARTPOLE: return 4;
     default: return f.out_dim;
     }

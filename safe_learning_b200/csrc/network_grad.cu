@@ -16,8 +16,9 @@
 // atomic; a second launch adds the G partial rows in CTA order.  Two calls with the same inputs give
 // bit-identical gradients.  With G == 1 the CTA writes grad_params directly (no workspace).
 //
-// Plants (SLB_FN_PENDULUM, SLB_FN_CARTPOLE): one thread per point, forward mode over the 3 or 5
-// inputs through the ten Euler sub-steps (state and tangents in registers), then grad_in = g^T J.
+// Plants (SLB_FN_PENDULUM, SLB_FN_CARTPOLE, SLB_FN_VANDERPOL): one thread per point, forward mode over
+// the 3 or 5 inputs through the ten Euler sub-steps (state and tangents in registers), then
+// grad_in = g^T J.
 //
 // SLB_FN_TRIANGULATION: the vertex-value gradient of triangulation_grad.cu.
 #include "common.cuh"
@@ -254,6 +255,34 @@ SLB_DEV void cartpole_jacobian(const slb_function& f, const double* in, double J
         for (int i = 0; i < 5; ++i) J[c][i] = ds[c][i] * (has_norm ? p[11 + c] : 1.0);
 }
 
+// Van der Pol: the state's two inputs (the action column does not enter, its column of J is 0).  The
+// (de)normalisation is diagonal, so its tangent is the scale itself.
+SLB_DEV void vanderpol_jacobian(const slb_function& f, const double* in, double J[2][3]) {
+    const double* p = f.cparams;
+    const double damping = p[0], dt = p[1];
+    const bool has_norm = p[2] != 0.0;
+    const double s_x = has_norm ? p[3] : 1.0, s_y = has_norm ? p[4] : 1.0;
+    double x = in[0] * s_x, y = in[1] * s_y;
+    double dx[2] = {s_x, 0.0}, dy[2] = {0.0, s_y};
+    for (int it = 0; it < 10; ++it) {
+        const double y_dot = x + damping * (x * x - 1.0) * y;
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const double dy_dot = dx[i] + damping * (2.0 * x * dx[i] * y + (x * x - 1.0) * dy[i]);
+            const double dx_n = dx[i] - dt * dy[i];
+            dy[i] = dy[i] + dt * dy_dot;
+            dx[i] = dx_n;
+        }
+        const double x_n = x - dt * y;
+        y = y + dt * y_dot;
+        x = x_n;
+    }
+    const double o_x = has_norm ? p[5] : 1.0, o_y = has_norm ? p[6] : 1.0;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) { J[0][i] = dx[i] * o_x; J[1][i] = dy[i] * o_y; }
+    J[0][2] = 0.0; J[1][2] = 0.0;
+}
+
 __global__ void __launch_bounds__(NT) vjp_plant_kernel(const __grid_constant__ slb_function f,
                                                        const double* __restrict__ x, int64_t n,
                                                        const double* __restrict__ gout,
@@ -261,12 +290,16 @@ __global__ void __launch_bounds__(NT) vjp_plant_kernel(const __grid_constant__ s
     const int64_t i = (int64_t)blockIdx.x * NT + threadIdx.x;
     if (i >= n) return;
     double z[5], y[4];
-    if (f.kind == SLB_FN_PENDULUM) {
+    if (f.kind == SLB_FN_PENDULUM || f.kind == SLB_FN_VANDERPOL) {
+        const bool vdp = f.kind == SLB_FN_VANDERPOL;
         for (int c = 0; c < 3; ++c) z[c] = x[i * 3 + c];
-        if (out != nullptr) { eval_pendulum(f, z, y); out[i * 2] = y[0]; out[i * 2 + 1] = y[1]; }
+        if (out != nullptr) {
+            if (vdp) eval_vanderpol(f, z, y); else eval_pendulum(f, z, y);
+            out[i * 2] = y[0]; out[i * 2 + 1] = y[1];
+        }
         if (gin != nullptr) {
             double J[2][3];
-            pendulum_jacobian(f, z, J);
+            if (vdp) vanderpol_jacobian(f, z, J); else pendulum_jacobian(f, z, J);
             const double g0 = gout[i * 2], g1 = gout[i * 2 + 1];
             for (int c = 0; c < 3; ++c) gin[i * 3 + c] = g0 * J[0][c] + g1 * J[1][c];
         }
@@ -326,12 +359,16 @@ int network_ctas(const net_shape& S, int64_t n) {
     return (int)(ntiles < (int64_t)SLB_NUM_SMS * per_sm ? ntiles : (int64_t)SLB_NUM_SMS * per_sm);
 }
 
+bool is_plant(int kind) {
+    return kind == SLB_FN_PENDULUM || kind == SLB_FN_CARTPOLE || kind == SLB_FN_VANDERPOL;
+}
+
 int vjp_validate(const slb_function* fn, const char* what) {
     SLB_CHECK(fn != nullptr, "%s: null function", what);
     SLB_CHECK(fn->kind == SLB_FN_MLP || fn->kind == SLB_FN_LYAPUNOV_NN || fn->kind == SLB_FN_PENDULUM ||
-              fn->kind == SLB_FN_CARTPOLE || fn->kind == SLB_FN_TRIANGULATION,
+              fn->kind == SLB_FN_CARTPOLE || fn->kind == SLB_FN_VANDERPOL || fn->kind == SLB_FN_TRIANGULATION,
               "%s: function kind %d has no VJP (NeuralNetwork, LyapunovNetwork, InvertedPendulum, CartPole, "
-              "Triangulation)", what, fn->kind);
+              "VanDerPol, Triangulation)", what, fn->kind);
     SLB_CHECK(!(fn->flags & SLB_FLAG_GRADIENT) || (fn->kind != SLB_FN_MLP && fn->kind != SLB_FN_LYAPUNOV_NN),
               "%s: the VJP of a network gradient (SLB_FLAG_GRADIENT) is a Hessian-vector product, which is "
               "not implemented", what);
@@ -347,7 +384,7 @@ extern "C" int64_t slb_function_vjp_workspace(const slb_function* fn, int64_t n)
     if (vjp_validate(fn, "slb_function_vjp_workspace")) return -1;
     if (n < 0) { slb_set_error("slb_function_vjp_workspace: negative n"); return -1; }
     if (fn->kind == SLB_FN_TRIANGULATION) return slb_triangulation_vjp_workspace(fn, n);
-    if (fn->kind == SLB_FN_PENDULUM || fn->kind == SLB_FN_CARTPOLE) return 0;
+    if (is_plant(fn->kind)) return 0;
     net_shape S;
     network_shape(*fn, &S);
     const int G = network_ctas(S, n);
@@ -366,7 +403,7 @@ extern "C" int slb_function_vjp(void* stream, const slb_function* fn, const doub
         return slb_triangulation_vjp(st, fn, points_dev, n, grad_out_dev, grad_in_dev, grad_params_dev, out_dev,
                                      workspace_dev);
     }
-    const bool plant = fn->kind == SLB_FN_PENDULUM || fn->kind == SLB_FN_CARTPOLE;
+    const bool plant = is_plant(fn->kind);
     SLB_CHECK(!plant || grad_params_dev == nullptr,
               "slb_function_vjp: the plants have no parameters (grad_params must be NULL)");
     SLB_CHECK(n == 0 || (points_dev != nullptr && grad_out_dev != nullptr),

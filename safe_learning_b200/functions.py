@@ -37,7 +37,7 @@ __all__ = ["DimensionError", "GridWorld", "Function", "DeterministicFunction",
            "Kernel", "RBF", "Matern12", "Matern32", "Matern52", "Linear", "Constant", "Bias",
            "White", "Sum", "Add", "Product", "Prod", "kernels", "Likelihood", "GPRCached", "GPR",
            "GaussianProcess", "FunctionStack",
-           "InvertedPendulum", "CartPole", "LyapunovNetwork", "NeuralNetwork",
+           "InvertedPendulum", "CartPole", "VanDerPol", "LyapunovNetwork", "NeuralNetwork",
            "concatenate_inputs"]
 
 
@@ -972,6 +972,68 @@ class CartPole(DeterministicFunction):
 
     def jacobian_device(self, points):
         """d x+ / d [x, u] through the ten Euler sub-steps, [n, 4, 5] (``slb_function_vjp``)."""
+        return _unit_vjp_jacobian(self, points)
+
+    _vjp = InvertedPendulum._vjp
+
+
+class VanDerPol(DeterministicFunction):
+    """Van der Pol oscillator in reverse time, ``x' = -y``, ``y' = x + damping (x^2 - 1) y``, 10
+    explicit-Euler sub-steps (``examples/utilities.py:440-519``).  Its region of attraction is
+    bounded by the unstable limit cycle.
+
+    Called as ``vdp(states, actions)`` with a one-column action that does not enter (the reference
+    splits ``[x, u]`` as ``[2, 1]``); pair it with a one-column policy such as
+    ``LinearSystem(np.zeros((1, 2)))``.  ``normalization`` is the state scale ``Tx`` only: the
+    plant runs on ``x diag(Tx)`` and returns its result times ``diag(1 / Tx)``, as matrix products,
+    so an infinite or NaN component makes the other column NaN."""
+
+    def __init__(self, damping=1, dt=0.01, normalization=None, name="VanDerPol"):
+        super().__init__(name)
+        self.damping, self.dt = damping, dt
+        self.state_dim, self.action_dim = 2, 0
+        self.normalization = normalization
+        if normalization is not None:
+            self.normalization = np.array(normalization, dtype=np.float64)
+            self.inv_norm = self.normalization ** -1
+        self.input_dim, self.output_dim = 3, 2
+
+    def normalize(self, state):
+        """``state . diag(1 / Tx)`` on a numpy ``[n, 2]`` array (``:455-461``)."""
+        if self.normalization is None:
+            return state
+        return np.matmul(state, np.diag(self.inv_norm))
+
+    def denormalize(self, state):
+        """``state . diag(Tx)`` on a numpy ``[n, 2]`` array (``:463-469``)."""
+        if self.normalization is None:
+            return state
+        return np.matmul(state, np.diag(self.normalization))
+
+    def linearize(self):
+        """The discretised (zero-order hold), normalised linearisation ``Ad`` (``:471-487``)."""
+        A = np.array([[0, -1], [1, -1]], dtype=np.float64)
+        if self.normalization is not None:
+            Tx, Tx_inv = np.diag(self.normalization), np.diag(self.inv_norm)
+            A = np.linalg.multi_dot((Tx_inv, A, Tx))
+        Ad, _, _, _, _ = scipy.signal.cont2discrete((A, np.zeros([2, 1]), 0, 0), self.dt, method="zoh")
+        return Ad
+
+    def descriptor(self):
+        d = nat.SlbFunction()
+        d.kind, d.in_dim, d.out_dim = nat.FN_VANDERPOL, 3, 2
+        cp = d.cparams
+        cp[0] = self.damping
+        cp[1] = self.dt / 10
+        if self.normalization is not None:                      # [2] flag, [3..4] Tx, [5..6] 1/Tx
+            cp[2] = 1.0
+            cp[3], cp[4] = (float(t) for t in self.normalization)
+            cp[5], cp[6] = (float(t) for t in self.inv_norm)
+        return d
+
+    def jacobian_device(self, points):
+        """d x+ / d [x, u] through the ten Euler sub-steps, [n, 2, 3] with a zero action column
+        (``slb_function_vjp``)."""
         return _unit_vjp_jacobian(self, points)
 
     _vjp = InvertedPendulum._vjp
