@@ -512,6 +512,29 @@ int slb_apply_prefix(void* stream, const double* values_dev, const uint8_t* init
                      int64_t n, int64_t idx_begin, const slb_fail_key* key_dev,
                      uint8_t* safe_dev, void* workspace_dev, slb_prefix_stats* stats_dev);
 
+/* ---- update_safe_set(can_shrink=False) (lyapunov.py:497-606 with :507-510, :540-582): the V-sorted
+ *      batch loop resolved per batch on the device, single process.  order_dev [n]: stable sort of V
+ *      (sorted position -> grid index); batch = config.gp_batch_size >= 1; max_refinement R >= 1
+ *      (1: the plain branch).  negative_dev, prev_safe_dev [n]: the sweep's flags and the current safe
+ *      set; initial_dev may be NULL; n_req_dev [n] = ceil(max(s thr / dec, 0)), NaN -> 0, may be NULL
+ *      only when R == 1.  All arrays are in grid order.
+ *      slb_no_shrink_scan writes candidates_dev [n]: 1 where the refined check (tau / n_req on the
+ *      cell's mesh) can decide the result.  The caller writes that check into refined_dev [n]
+ *      (1 = verified; read at candidates only), then slb_no_shrink_resolve writes safe_dev and
+ *      refinement_dev [n], c_max's sorted position (-1: the largest V) and c_max.
+ *      workspace_dev: >= slb_no_shrink_workspace(n, batch) bytes, kept between the two calls.      */
+int64_t slb_no_shrink_workspace(int64_t n, int64_t batch);
+int slb_no_shrink_scan(void* stream, const int64_t* order_dev, const uint8_t* negative_dev,
+                       const uint8_t* prev_safe_dev, const uint8_t* initial_dev, const double* n_req_dev,
+                       int64_t n, int64_t batch, int64_t max_refinement, void* workspace_dev,
+                       uint8_t* candidates_dev);
+int slb_no_shrink_resolve(void* stream, const int64_t* order_dev, const double* values_dev,
+                          const uint8_t* negative_dev, const uint8_t* prev_safe_dev,
+                          const int64_t* prev_refinement_dev, const uint8_t* initial_dev,
+                          const double* n_req_dev, const uint8_t* refined_dev, int64_t n, int64_t batch,
+                          int64_t max_refinement, void* workspace_dev, uint8_t* safe_dev,
+                          int64_t* refinement_dev, int64_t* cmax_position_dev, double* cmax_dev);
+
 /* ---- generic evaluation of a fused function object on explicit points:
  *      DeterministicFunction.__call__, Lyapunov.update_values (lyapunov.py:305-322).
  *      points_dev [n, fn->in_dim] -> out_dev [n, out columns]. ---------------------------- */

@@ -32,7 +32,8 @@ UNITS += [("gp_sweep.o", "gp_sweep.cu", [], ["gp_args.h"]),
           ("network_grad.o", "network_grad.cu", [], []),
           ("triangulation_grad.o", "triangulation_grad.cu", [], []),
           ("gp_grad.o", "gp_grad.cu", [], []),
-          ("gp_hyper.o", "gp_hyper.cu", [], [])]
+          ("gp_hyper.o", "gp_hyper.cu", [], []),
+          ("no_shrink.o", "no_shrink.cu", [], [])]
 SOURCES = sorted({u[1] for u in UNITS})
 
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]

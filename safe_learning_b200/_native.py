@@ -167,6 +167,10 @@ SIGNATURES = {
     "slb_first_fail": (C.c_int, [_vp, _dp, _dp, _dp, _i64, _i64, _vp, _vp]),
     "slb_combine_fail_keys": (C.c_int, [_vp, _vp, _i32, _vp]),
     "slb_apply_prefix": (C.c_int, [_vp, _dp, _dp, _i64, _i64, _vp, _dp, _vp, _vp]),
+    "slb_no_shrink_workspace": (C.c_int64, [_i64, _i64]),
+    "slb_no_shrink_scan": (C.c_int, [_vp, _dp, _dp, _dp, _dp, _dp, _i64, _i64, _i64, _vp, _dp]),
+    "slb_no_shrink_resolve": (C.c_int, [_vp, _dp, _dp, _dp, _dp, _dp, _dp, _dp, _dp, _i64, _i64, _i64,
+                                        _vp, _dp, _dp, _dp, _dp]),
     "slb_eval_function": (C.c_int, [_vp, C.POINTER(SlbFunction), _dp, _i64, _dp]),
     "slb_function_columns": (C.c_int, [C.POINTER(SlbFunction)]),
     "slb_index_to_state": (C.c_int, [_vp, C.POINTER(SlbGrid), _i64, _i64, _dp]),

@@ -200,17 +200,20 @@ def _key_to_value(bits):
 
 
 def adaptive_as_written(values, negative, decrease, threshold, coef, initial, tau, batch,
-                        max_refinement, safety_factor):
+                        max_refinement, safety_factor, safe_set=None, refinement=None):
     """Host loop of the reference's adaptive branch, as written (``lyapunov.py:497-606`` with
     ``:540-582``), over per-point quantities of the whole grid: ``negative``, ``decrease``,
     ``threshold`` (at ``tau``) and ``coef = -L_V(x)(1 + L_f)`` so that ``threshold(x, tau / n) =
     coef * (tau / n)``.  ``refined_safety_check`` (``:457-481``) compares the decrease of EVERY
     state fed in the slice with the cell's own refined threshold, i.e. a cell passes iff the
     largest decrease of the slice is below it.  Returns (safe [N] bool, refinement [N] int,
-    sorted position of c_max)."""
+    sorted position of c_max).  ``safe_set`` / ``refinement`` are the previous safe set and
+    refinement the loop starts from (``can_shrink=False``, ``:507-510``); by default the initial
+    set with refinement 1 (``can_shrink=True``)."""
     n_total = len(values)
     order = np.argsort(values, kind="stable")
-    safe_s, refine_s = initial[order].copy(), initial[order].astype(int)
+    safe_s = (initial if safe_set is None else np.asarray(safe_set, dtype=bool))[order].copy()
+    refine_s = (initial if refinement is None else np.asarray(refinement))[order].astype(int)
     start = bound = refine_bound = 0
     for start in range(0, n_total, batch):
         sel = order[start:start + batch]
@@ -706,30 +709,19 @@ class Lyapunov(object):
         mesh = np.meshgrid(*border, indexing="ij")
         return np.stack([col.reshape(-1) for col in mesh], axis=1)
 
-    def _adaptive_ok(self, max_refinement, safety_factor, initial):
-        """Adaptive discretisation (``lyapunov.py:445-487, 540-582``) in closed form.
-
-        ``n_req = ceil(max(safety_factor * threshold / decrease, 0))`` (NaN -> 0, ``:447-455``).  A
-        point counts as verified if ``negative``, or if ``2 <= n_req <= max_refinement`` and the
-        decrease condition holds with ``tau / n_req`` on all ``n_req^d`` mesh points of its cell
-        (``:459-472``).  The reference's graph builds that mesh but compares the outer
-        ``decrease`` tensor (``:474-478``, dead code); this implements the evident intent, the
-        same as ``oracle.Lyapunov.update_safe_set(refinement_mode="mesh")``.  The V-sorted prefix
-        rule then runs on the verified flags; refined candidates are only evaluated up to the
-        first point that cannot be verified at all.  Returns (flags uint8, n_req int64) slabs.
-        """
-        neg, det = self.compute_negative(want_details=True)
-        negb = neg.to(torch.bool)
-        ratio = float(safety_factor) * det["threshold"] / det["decrease"]
+    @staticmethod
+    def _required_refinement(details, safety_factor):
+        """``n_req = ceil(max(safety_factor * threshold / decrease, 0))``, NaN -> 0 (``:447-455``),
+        as a float64 slab."""
+        ratio = float(safety_factor) * details["threshold"] / details["decrease"]
         ratio = torch.where(torch.isnan(ratio), torch.zeros_like(ratio), ratio)
-        n_req = torch.ceil(torch.clamp(ratio, min=0.0))
-        known = negb if initial is None else negb | initial.to(torch.bool)
-        cand = ~known & (n_req >= 2) & (n_req <= max_refinement)
-        hopeless = ~known & ~cand
+        return torch.ceil(torch.clamp(ratio, min=0.0))
+
+    def _refined_mesh_check(self, cand, n_req, max_refinement, ok):
+        """The refined check of ``lyapunov.py:459-472`` at the candidates (bool slab ``cand``): the
+        decrease condition with ``tau / n_req`` on all ``n_req^d`` mesh points of the cell.  Writes
+        the verdict into ``ok`` at the candidates; one host synchronisation per mesh size."""
         values = self._values_dev
-        if bool(hopeless.any()):
-            cand &= values <= values[hopeless].min()
-        ok = negb.clone()
         grid = self.discretization
         d = grid.ndim
         num = torch.as_tensor(np.asarray(grid.num_points, dtype=np.int64), device=values.device)
@@ -752,6 +744,30 @@ class Lyapunov(object):
                 points = (offsets[None, :, :] + centers[:, None, :]).reshape(-1, d)
                 fine = self.negative_at_points(points, self.tau / n)
                 ok[part] = fine.view(part.numel(), -1).to(torch.bool).all(dim=1)
+
+    def _adaptive_ok(self, max_refinement, safety_factor, initial):
+        """Adaptive discretisation (``lyapunov.py:445-487, 540-582``) in closed form.
+
+        ``n_req = ceil(max(safety_factor * threshold / decrease, 0))`` (NaN -> 0, ``:447-455``).  A
+        point counts as verified if ``negative``, or if ``2 <= n_req <= max_refinement`` and the
+        decrease condition holds with ``tau / n_req`` on all ``n_req^d`` mesh points of its cell
+        (``:459-472``).  The reference's graph builds that mesh but compares the outer
+        ``decrease`` tensor (``:474-478``, dead code); this implements the evident intent, the
+        same as ``oracle.Lyapunov.update_safe_set(refinement_mode="mesh")``.  The V-sorted prefix
+        rule then runs on the verified flags; refined candidates are only evaluated up to the
+        first point that cannot be verified at all.  Returns (flags uint8, n_req int64) slabs.
+        """
+        neg, det = self.compute_negative(want_details=True)
+        negb = neg.to(torch.bool)
+        n_req = self._required_refinement(det, safety_factor)
+        known = negb if initial is None else negb | initial.to(torch.bool)
+        cand = ~known & (n_req >= 2) & (n_req <= max_refinement)
+        hopeless = ~known & ~cand
+        values = self._values_dev
+        if bool(hopeless.any()):
+            cand &= values <= values[hopeless].min()
+        ok = negb.clone()
+        self._refined_mesh_check(cand, n_req, max_refinement, ok)
         return ok.to(torch.uint8), n_req.to(torch.int64), negb
 
     def update_safe_set(self, can_shrink=True, max_refinement=1, safety_factor=1.,
@@ -760,20 +776,30 @@ class Lyapunov(object):
 
         The call only ENQUEUES the sweep (fused decision kernel(s), first-fail reduction with the
         inter-rank key exchange, prefix application); ``safe_set``, ``c_max`` (through
-        ``feed_dict``), ``_refinement`` and ``last_sweep`` synchronise when they are read."""
+        ``feed_dict``), ``_refinement`` and ``last_sweep`` synchronise when they are read.
+
+        ``can_shrink=False`` keeps the previous safe set and refinement as the starting point and
+        resolves the reference's V-sorted batch loop on the device (``_update_no_shrink``); it is
+        complete when the call returns.  ``parallel_iterations`` (the reference's ``tf.map_fn``
+        parallelism) is accepted and ignored."""
         adaptive = bool(self.adaptive and max_refinement > 1)
-        if adaptive and not can_shrink:
-            raise NotImplementedError("adaptive refinement with can_shrink=False is not "
-                                      "implemented")
+        if not can_shrink:
+            if adaptive and self.initial_safe_set is None:
+                raise NotImplementedError(
+                    "adaptive refinement with can_shrink=False needs an initial safe set: the "
+                    "reference's branch indexes initial_safe_set[indices] (lyapunov.py:547-548)")
+            if dev.dist_info()[1] > 1:
+                raise NotImplementedError("can_shrink=False needs global ranks: replicas only")
         safety_factor = max(float(safety_factor), 1.)
         self._pending = None
         if adaptive and self.refinement_mode == "reference":
-            return self._update_adaptive_as_written(max_refinement, safety_factor)
+            return self._update_adaptive_as_written(max_refinement, safety_factor, can_shrink)
         lib = nat.load()
         n_local = self._end - self._begin
         initial = self._initial_device()
         if not can_shrink:
-            return self._update_no_shrink(self.compute_negative())
+            return self._update_no_shrink(int(max_refinement) if adaptive else 1, safety_factor,
+                                          initial)
 
         rank, world = dev.dist_info()
         if self._workspace is None:
@@ -916,7 +942,7 @@ class Lyapunov(object):
     def last_sweep(self, value):
         self._last_sweep = value
 
-    def _update_adaptive_as_written(self, max_refinement, safety_factor):
+    def _update_adaptive_as_written(self, max_refinement, safety_factor, can_shrink=True):
         """``refinement_mode="reference"``: the adaptive branch exactly as the reference's graph and
         host loop evaluate it (``lyapunov.py:457-481, 540-582``) -- ``refined_safety_check`` builds
         the mesh but compares the OUTER ``decrease`` tensor of every state fed in the slice with
@@ -924,7 +950,8 @@ class Lyapunov(object):
         fed slice is below its own refined threshold, and initial-safe states are re-checked with
         n = 1.  The per-point quantities (``negative``, ``decrease``, the threshold coefficient
         ``-L_V(x)(1 + L_f)``) come from the fused sweep; the batch loop, which depends on
-        ``config.gp_batch_size`` and on sorted ranks, is replayed on the host over them."""
+        ``config.gp_batch_size`` and on sorted ranks, is replayed on the host over them, from the
+        previous safe set and refinement when ``can_shrink`` is False."""
         lib = nat.load()
         neg, det = self.compute_negative(want_details=True)
         # threshold(x, tau / n) = (-L_V(x) (1 + L_f)) * (tau / n): the coefficient is the sweep's
@@ -954,9 +981,11 @@ class Lyapunov(object):
         initial = np.zeros(n_total, dtype=bool)
         if self.initial_safe_set is not None:
             initial[self.initial_safe_set] = True
+        previous = {} if can_shrink else {"safe_set": self.safe_set,
+                                          "refinement": np.asarray(self._refinement)}
         safe, refinement, position = adaptive_as_written(
             values, negative, decrease, threshold, coef, initial, self.tau,
-            int(config.gp_batch_size), max_refinement, safety_factor)
+            int(config.gp_batch_size), max_refinement, safety_factor, **previous)
         c_max = float(values[np.argsort(values, kind="stable")[position]])
         self._safe_host = safe
         self._safe_dirty = False
@@ -993,50 +1022,61 @@ class Lyapunov(object):
         values = self._gather(self._values_dev)
         return float(torch.kthvalue(values, position + 1).values.item())
 
-    def _update_no_shrink(self, negative):
-        """``can_shrink=False`` (``lyapunov.py:507-510, 583-587``; SURVEY.md Q3): previously
-        safe states seed the result and the batch size decides which trailing states keep their
-        old label, so this mode needs sorted ranks -- a stable device sort (torch), single GPU."""
-        rank, world = dev.dist_info()
-        if world > 1:
-            raise NotImplementedError("can_shrink=False needs global ranks: replicas only")
+    def _update_no_shrink(self, max_refinement, safety_factor, initial):
+        """``can_shrink=False`` (``lyapunov.py:497-606`` with ``:507-510, :540-587``; SURVEY.md Q3):
+        the previous safe set and refinement seed the result and the batch size decides which
+        trailing states keep their old label, so this mode needs sorted ranks -- a stable device
+        sort (torch), single GPU.  ``slb_no_shrink_scan`` finds each batch's first unverified
+        position and marks the cells whose refined check can still matter; the mesh checks run on
+        those only (``max_refinement > 1``); ``slb_no_shrink_resolve`` replays the loop's outcome
+        in grid order.  One read-back at the end; no host loop over batches."""
+        lib = nat.load()
+        n = self._end - self._begin
+        batch = int(config.gp_batch_size)
+        if max_refinement > 1:
+            neg, det = self.compute_negative(want_details=True)
+            n_req = self._required_refinement(det, safety_factor)
+        else:
+            neg, n_req = self.compute_negative(), None
         values = self._values_dev
         order = torch.sort(values, stable=True).indices
-        prev = dev.to_device(self.safe_set.astype(np.uint8), torch.uint8).to(torch.bool)
+        prev = dev.to_device(self.safe_set.astype(np.uint8), torch.uint8)
         refine_prev = dev.to_device(np.asarray(self._refinement, dtype=np.int64), torch.int64)
-        neg = negative.to(torch.bool)
-        prev_s, neg_s = prev[order], neg[order]
-        ok = prev_s | neg_s
-        n = ok.numel()
-        batch = int(config.gp_batch_size)
-        bad = torch.nonzero(~ok)
-        safe_s = prev_s.clone()
-        ref_s = refine_prev[order].clone()
-        if bad.numel() == 0:
-            safe_s = ok
-            ref_s[neg_s] = 1
-            position = ((n - 1) // batch) * batch - 1
-        else:
-            p = int(bad[0].item())
-            stop = min((p // batch + 1) * batch, n)
-            safe_s[:stop] = ok[:stop]
-            sel = neg_s.clone()
-            sel[stop:] = False
-            ref_s[sel] = 1
-            safe_s[p:stop] = False
-            ref_s[p:stop] = 0
-            position = p - 1
-        dict.__setitem__(self.feed_dict, self.c_max, float(values[order[position]].item()))
-        safe = torch.zeros_like(prev)
-        safe[order] = safe_s
-        refinement = torch.zeros_like(refine_prev)
-        refinement[order] = ref_s
-        safe_host = safe.cpu().numpy()
-        ref_host = refinement.cpu().numpy().astype(int)
-        if self.initial_safe_set is not None:
-            safe_host[self.initial_safe_set] = True
-            ref_host[self.initial_safe_set] = 1
-        self._safe_host = safe_host
+        workspace = dev.empty((int(lib.slb_no_shrink_workspace(n, batch)) // 8,), torch.int64)
+        cand = dev.empty((n,), torch.bool)
+        refined = dev.zeros((n,), torch.bool)
+        nat.check(lib.slb_no_shrink_scan(dev.stream(), order.data_ptr(), neg.data_ptr(),
+                                         prev.data_ptr(), dev.ptr(initial), dev.ptr(n_req), n,
+                                         batch, max_refinement, workspace.data_ptr(),
+                                         cand.data_ptr()), "slb_no_shrink_scan")
+        if max_refinement > 1:
+            self._refined_mesh_check(cand, n_req, max_refinement, refined)
+        # written in place: a captured sweep graph of can_shrink=True holds this buffer's address
+        if self._safe_dev is None or self._safe_dev.numel() != n:
+            self._safe_dev = dev.empty((n,), torch.uint8)
+        safe = self._safe_dev
+        refinement = dev.empty((n,), torch.int64)
+        result = dev.empty((2,), torch.int64)          # [c_max position, c_max bits]
+        nat.check(lib.slb_no_shrink_resolve(dev.stream(), order.data_ptr(), values.data_ptr(),
+                                            neg.data_ptr(), prev.data_ptr(),
+                                            refine_prev.data_ptr(), dev.ptr(initial),
+                                            dev.ptr(n_req), refined.data_ptr(), n, batch,
+                                            max_refinement, workspace.data_ptr(),
+                                            safe.data_ptr(), refinement.data_ptr(),
+                                            result[0:1].data_ptr(), result[1:2].data_ptr()),
+                  "slb_no_shrink_resolve")
+        host = self.__dict__.get("_no_shrink_bufs")
+        if host is None or host[0].numel() != n:
+            host = (torch.empty((n,), dtype=torch.uint8).pin_memory(),
+                    torch.empty((n,), dtype=torch.int64).pin_memory(),
+                    torch.empty((2,), dtype=torch.int64).pin_memory())
+            self.__dict__["_no_shrink_bufs"] = host
+        for dst, src in zip(host, (safe, refinement, result)):
+            dst.copy_(src, non_blocking=True)
+        torch.cuda.current_stream().synchronize()
+        self._safe_host = host[0].numpy().astype(bool)
         self._safe_dirty = False
-        self._safe_dev = dev.to_device(safe_host.astype(np.uint8), torch.uint8)
-        self._refinement = ref_host
+        self._refinement = host[1].numpy().astype(int)
+        self.__dict__["_adaptive_state"] = None
+        c_max = float(host[2].numpy()[1:2].view(np.float64)[0])
+        dict.__setitem__(self.feed_dict, self.c_max, c_max)
