@@ -70,12 +70,20 @@ enum slb_fn_kind {
     SLB_FN_CARTPOLE = 6,       /* CartPole                    examples/utilities.py:292-437 */
     SLB_FN_LYAPUNOV_NN = 7,    /* LyapunovNetwork             examples/utilities.py:48-104  */
     SLB_FN_MLP = 8,            /* NeuralNetwork               functions.py:1702-1729        */
-    SLB_FN_VANDERPOL = 9       /* VanDerPol (reverse time)    examples/utilities.py:440-519
+    SLB_FN_VANDERPOL = 9,      /* VanDerPol (reverse time)    examples/utilities.py:440-519
                                   maps [x, y, u] (3 inputs, u ignored) to 2 columns; cparams:
                                   [0] damping, [1] dt / 10, [2] 1 if normalised, [3..4] Tx,
                                   [5..6] 1 / Tx.  The normalisation is the reference's
                                   state . diag(T): column j = s_j T_j + s_(1-j) 0, so an inf or
                                   NaN component makes the other column NaN */
+    SLB_FN_PIECEWISE_CONSTANT = 10  /* PiecewiseConstant      functions.py:820-932
+                                  the row of the nearest grid vertex (GridWorld.state_to_index,
+                                  functions.py:733-752): clip to the limits, (x - offset) * inv,
+                                  np.rint (half to even), ravel.  matrix = vertex values
+                                  [nindex, out]; grid = the discretization (discrete_points not
+                                  needed); in_dim = grid.ndim; cparams[0..d-1] = inv = 1. /
+                                  unit_maxes as numpy computes it.  A row with a NaN coordinate
+                                  gives NaN in every column (the reference raises) */
 };
 /* post-ops, applied in this order: saturate -> abs -> norm1 | maxabs -> out_scale */
 #define SLB_FLAG_SATURATE 1u   /* Saturation  functions.py:349-354                     */
@@ -109,8 +117,9 @@ typedef struct slb_function {
                                    [0] layers, [1+i] width of layer i (<= 64), [9+i] activation
                                    (0 tanh, 1 relu, 2 identity); MLP: [17] output_scale, [18] 1 if
                                    hidden layers carry a bias (matrix = [W_i (out x in), b_i] ...) */
-    const double*  matrix;      /* LINEAR [out,in]; QUADRATIC [in,in]; TRIANGULATION
-                                   vertex values [nindex,out]; LYAPUNOV_NN packed kernels */
+    const double*  matrix;      /* LINEAR [out,in]; QUADRATIC [in,in]; TRIANGULATION and
+                                   PIECEWISE_CONSTANT vertex values [nindex,out]; LYAPUNOV_NN
+                                   packed kernels */
     const double*  hyperplanes; /* TRIANGULATION [nsimplex, d, d]  (functions.py:1090-1101) */
     const int64_t* unit_simplices; /* TRIANGULATION [nsimplex, d+1] (functions.py:1064-1088) */
     const int32_t* corner_simplex; /* TRIANGULATION [2^d] or NULL: Qhull's find_simplex answer for
@@ -119,7 +128,7 @@ typedef struct slb_function {
                                       where several simplices meet and extrapolation differs  */
     int32_t nsimplex;
     int32_t _pad;
-    slb_grid grid;              /* TRIANGULATION discretization                        */
+    slb_grid grid;              /* TRIANGULATION / PIECEWISE_CONSTANT discretization   */
 } slb_function;
 
 /* ---- covariance functions ------------------------------------------------------------------
@@ -264,7 +273,8 @@ typedef struct slb_bellman {
     slb_function dynamics;      /* deterministic dynamics when gp.num_outputs == 0      */
     slb_gp_stack gp;            /* GP dynamics: mean only               (:98-99)        */
     slb_function reward;        /* r([x,u])                             (:95)           */
-    slb_function value;         /* V as Triangulation (vertex table = `matrix`) (:101)  */
+    slb_function value;         /* V as Triangulation or PiecewiseConstant (vertex table =
+                                   `matrix`)                           (:101)           */
     double gamma;               /*                                      (:104)          */
     int32_t fixed_action;       /* 1 => use `action` for every state (:266-270)         */
     int32_t _pad;
@@ -591,10 +601,13 @@ int slb_reward_rollout(void* stream, const slb_bellman* cfg, const double* state
                        double* sums_dev, int64_t* stop_dev, void* workspace_dev);
 
 /* ---- exact policy evaluation (reinforcement_learning.py:142-211 optimize_value_function): the
- *      fixed point of  v = r + gamma T v,  T = the value Triangulation's barycentric rows at the mean
- *      next states (DESIGN.md §3.9).  Row i of T: cols_dev[i * (d + 1) + j] (int32, or int64 when the
- *      value grid has more than 2^31 - 1 vertices), weights_dev[i * (d + 1) + j] (fp64), d = the
- *      value grid's dimension.  stats_dev: SLB_VALUE_STATS uint64 slots:
+ *      fixed point of  v = r + gamma T v,  T = the value table's rows at the mean next states
+ *      (DESIGN.md §3.9, §3.15).  Row i of T has ncols entries: cols_dev[i * ncols + j] (int32, or int64
+ *      when the value grid has more than 2^31 - 1 vertices), weights_dev[i * ncols + j] (fp64).  A
+ *      Triangulation gives ncols = d + 1 barycentric weights, d = the value grid's dimension; a
+ *      PiecewiseConstant gives ncols = 2: the next state's nearest vertex with weight 1, then the same
+ *      vertex with weight 0 (slb_value_solve's narrowest row; a NaN next state: vertex 0 with weights NaN,
+ *      0).  stats_dev: SLB_VALUE_STATS uint64 slots:
  *        [0] ~key(min weight)  (order-preserving key of the smallest weight, complemented)
  *        [1] rho = max_i sum_j |w_ij|, fp64 bits     [2] rows re-searched (grid-line lookups, Q6)
  *        [3] rows with a NaN next state / reward     [4] iterations   [5] last ||dv||_inf, fp64 bits
@@ -608,7 +621,7 @@ int slb_reward_rollout(void* stream, const slb_bellman* cfg, const double* state
 #define SLB_VALUE_NAN 4
 /* fused assembly for flat indices [idx_begin, idx_end): u = policy(x), x+ = mean dynamics(x, u)
  * (deterministic function or GP stack), rewards_dev[i] = reward(x, u); cfg->value is a one-output
- * Triangulation; fixed_action must be 0 */
+ * Triangulation (projection allowed) or PiecewiseConstant, without post-op flags; fixed_action must be 0 */
 int slb_value_operator(void* stream, const slb_bellman* cfg, int64_t idx_begin, int64_t idx_end,
                        void* cols_dev, double* weights_dev, double* rewards_dev, uint64_t* stats_dev);
 /* composed assembly: the rows of next_states_dev [n, d] */
@@ -634,7 +647,7 @@ int slb_value_solve(void* stream, int64_t n, int32_t ncols, const void* cols_dev
  *                                   the plants, which have no parameters
  *        out_dev         [n, out] = the forward pass recomputed by the gradient kernel, bit-identical to
  *                                   slb_eval_function (or NULL)
- *      Kinds MLP, LYAPUNOV_NN, PENDULUM, CARTPOLE and VANDERPOL (and TRIANGULATION, below) without post-op
+ *      Kinds MLP, LYAPUNOV_NN, PENDULUM, CARTPOLE and VANDERPOL (and TRIANGULATION, PIECEWISE_CONSTANT, below) without post-op
  *      flags; VANDERPOL's action column gets a zero gradient.  Gradient conventions: ReLU' = 0
  *      at 0, tanh' = 1 - tanh^2.  The parameter gradient is reduced in a fixed order without atomics: two
  *      calls with the same inputs give bit-identical results.  n == 0 zeroes grad_params and launches
@@ -655,6 +668,16 @@ int slb_function_vjp(void* stream, const slb_function* fn, const double* points_
  *      is needed when grad_params_dev is given and n > 0; a batch whose sort key (bits of nindex - 1 plus
  *      bits of n (d + 1) - 1) exceeds 64 bits is rejected.  One thread sums each vertex, so a batch whose
  *      points all land on one vertex costs n (d + 1) serial additions. */
+/* ---- SLB_FN_PIECEWISE_CONSTANT in slb_function_vjp: the same transpose with one row per point, its
+ *      nearest vertex with weight 1: grad_params_dev [nindex, out] = sum over the points p of grad_out[p]
+ *      scattered to that vertex, OVERWRITTEN, summed in ascending p from +0.0 without atomics (bit for bit
+ *      np.add.at(G, idx, grad_out)).  A point with a NaN coordinate (NaN forward, no vertex) adds nothing.
+ *      grad_in_dev must be NULL (the point gradient is 0); no flags; workspace and key limit as above. */
+/* GridWorld.state_to_index (functions.py:733-752) on the device, the lookup of SLB_FN_PIECEWISE_CONSTANT:
+ * idx_dev [n] (int64) = the flat index of the nearest vertex of points_dev [n, grid->ndim], or -1 for a
+ * row with a NaN coordinate (PiecewiseConstant.parameter_derivative, functions.py:889-913) */
+int slb_grid_nearest_index(void* stream, const slb_grid* grid, const double* points_dev, int64_t n,
+                           int64_t* idx_dev);
 /* the rows of _Triangulation.parameter_derivative (functions.py:1228-1259) at points_dev [n, d]:
  * cols_dev int64 [n, d + 1] vertex indices and weights_dev [n, d + 1] barycentric weights of the forward
  * evaluation (projection, corner table and simplex choice included) */

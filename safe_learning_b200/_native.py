@@ -20,7 +20,7 @@ SLB_HEAD_RANK = 64
 SLB_MAX_RANKS = 16
 
 FN_NONE, FN_CONSTANT, FN_LINEAR, FN_QUADRATIC, FN_TRIANGULATION, FN_PENDULUM, FN_CARTPOLE, \
-    FN_LYAPUNOV_NN, FN_MLP, FN_VANDERPOL = range(10)
+    FN_LYAPUNOV_NN, FN_MLP, FN_VANDERPOL, FN_PIECEWISE_CONSTANT = range(11)
 FLAG_SATURATE, FLAG_ABS, FLAG_NORM1, FLAG_PROJECT, FLAG_SCALE, FLAG_GRADIENT, FLAG_MAXABS = \
     1, 2, 4, 8, 16, 32, 64
 K_RBF, K_MATERN12, K_MATERN32, K_MATERN52, K_LINEAR, K_CONSTANT, K_WHITE = range(7)
@@ -192,6 +192,7 @@ SIGNATURES = {
     "slb_function_vjp_workspace": (C.c_int64, [C.POINTER(SlbFunction), _i64]),
     "slb_function_vjp": (C.c_int, [_vp, C.POINTER(SlbFunction), _dp, _i64, _dp, _dp, _dp, _dp, _vp]),
     "slb_triangulation_rows": (C.c_int, [_vp, C.POINTER(SlbFunction), _dp, _i64, _vp, _dp]),
+    "slb_grid_nearest_index": (C.c_int, [_vp, C.POINTER(SlbGrid), _dp, _i64, _vp]),
     "slb_gp_vjp_workspace": (C.c_int64, [C.POINTER(SlbGpStack), _i64]),
     "slb_gp_vjp": (C.c_int, [_vp, C.POINTER(SlbGpStack), _dp, _i64, _dp, _dp, _dp, _vp]),
     "slb_gp_lml_grad_workspace": (C.c_int64, [_i32]),

@@ -282,6 +282,26 @@ SLB_DEV void grid_index_to_state(const slb_grid& g, int64_t idx, double* x) {
     }
 }
 
+// GridWorld.state_to_index (functions.py:733-752), the nearest vertex of x: clip to [offset, upper], then
+// (x - offset) * inv with inv = 1. / unit_maxes as numpy computes it (two roundings, never contracted), then
+// rint (half to even, like np.rint), then ravel.  np.clip keeps a NaN where fmin / fmax would drop it; a
+// row with a NaN coordinate has no vertex and gives -1 (the reference raises from ravel_multi_index).  The
+// per-axis index is kept inside the grid so that a descriptor with a wrong inv cannot read out of bounds;
+// with numpy's inv it never leaves it.
+SLB_DEV int64_t grid_nearest_index(const slb_grid& g, const double* inv, const double* x) {
+    int64_t idx = 0;
+    for (int c = 0; c < g.ndim; ++c) {
+        const double xc = x[c];
+        if (xc != xc) return -1;
+        const double cl = xc < g.offset[c] ? g.offset[c] : (xc > g.upper[c] ? g.upper[c] : xc);
+        const double k = rint(f64mul(f64sub(cl, g.offset[c]), inv[c]));
+        const int64_t n = g.num_points[c];
+        const int64_t i = k > 0.0 ? (k < (double)(n - 1) ? (int64_t)k : n - 1) : 0;
+        idx = idx * n + i;
+    }
+    return idx;
+}
+
 // fmod(a, b) for a >= 0, b > 0, a / b < 2^52 -- bit-identical to fmod (whose result is exact): the
 // quotient from one division (it can only come out one too large, when a / b rounds up to an
 // integer), the remainder by an exact fma.  CUDA's fmod is a long software loop; the Triangulation
@@ -700,9 +720,15 @@ SLB_EVAL_ATTR int eval_fn(const slb_function& f, const double* in, double* out) 
 #endif
         eval_network<SLB_FN_MLP>(f, in, out);
         break;
-    default:
-        for (int o = 0; o < od; ++o) out[o] = __longlong_as_double(0x7ff8000000000000ll);
+    // SLB_FN_PIECEWISE_CONSTANT (functions.py:875-887): the nearest vertex's row, NaN without a vertex; any
+    // other kind: NaN.  The kind shares the default branch because a case of its own gave the generic
+    // filter_head_kernel 4-8 more bytes of spills.
+    default: {
+        const int64_t v = f.kind == SLB_FN_PIECEWISE_CONSTANT ? grid_nearest_index(f.grid, f.cparams, in) : -1;
+        for (int o = 0; o < od; ++o)
+            out[o] = v < 0 ? __longlong_as_double(0x7ff8000000000000ll) : f.matrix[v * od + o];
         break;
+    }
     }
     if (f.flags & SLB_FLAG_SATURATE)
         for (int o = 0; o < od; ++o) out[o] = fmin(fmax(out[o], f.lower), f.upper);

@@ -101,6 +101,20 @@ int slb_validate_function(const slb_function* f, const char* what, int expect_in
                   "%s: Triangulation gradient needs one value column and out_dim = ndim (%d), got %d",
                   what, f->grid.ndim, f->out_dim);
         break;
+    case SLB_FN_PIECEWISE_CONSTANT:
+        if (slb_validate_grid(&f->grid, false)) return 1;
+        SLB_CHECK(f->matrix != nullptr, "%s: PiecewiseConstant without vertex values", what);
+        SLB_CHECK(f->in_dim == f->grid.ndim, "%s: PiecewiseConstant in_dim %d != grid ndim %d", what,
+                  f->in_dim, f->grid.ndim);
+        SLB_CHECK(f->out_dim >= 1 && f->out_dim <= SLB_MAX_OUT, "%s: PiecewiseConstant out_dim %d", what,
+                  f->out_dim);
+        SLB_CHECK(!(f->flags & SLB_FLAG_PROJECT), "%s: PiecewiseConstant clips by itself (no projection flag)",
+                  what);
+        for (int c = 0; c < f->grid.ndim; ++c)
+            SLB_CHECK(f->cparams[c] > 0.0 && f->cparams[c] < INFINITY,
+                      "%s: PiecewiseConstant needs cparams[%d] = 1 / unit_maxes, positive and finite (got %g)",
+                      what, c, f->cparams[c]);
+        break;
     case SLB_FN_PENDULUM:
         SLB_CHECK(f->in_dim == 3 && f->out_dim == 2, "%s: pendulum must map 3 -> 2", what);
         break;

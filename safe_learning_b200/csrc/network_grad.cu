@@ -20,7 +20,7 @@
 // the 3 or 5 inputs through the ten Euler sub-steps (state and tangents in registers), then
 // grad_in = g^T J.
 //
-// SLB_FN_TRIANGULATION: the vertex-value gradient of triangulation_grad.cu.
+// SLB_FN_TRIANGULATION, SLB_FN_PIECEWISE_CONSTANT: the vertex-value gradient of triangulation_grad.cu.
 #include "common.cuh"
 
 #include <string.h>
@@ -359,6 +359,8 @@ int network_ctas(const net_shape& S, int64_t n) {
     return (int)(ntiles < (int64_t)SLB_NUM_SMS * per_sm ? ntiles : (int64_t)SLB_NUM_SMS * per_sm);
 }
 
+bool is_table(int kind) { return kind == SLB_FN_TRIANGULATION || kind == SLB_FN_PIECEWISE_CONSTANT; }
+
 bool is_plant(int kind) {
     return kind == SLB_FN_PENDULUM || kind == SLB_FN_CARTPOLE || kind == SLB_FN_VANDERPOL;
 }
@@ -366,9 +368,9 @@ bool is_plant(int kind) {
 int vjp_validate(const slb_function* fn, const char* what) {
     SLB_CHECK(fn != nullptr, "%s: null function", what);
     SLB_CHECK(fn->kind == SLB_FN_MLP || fn->kind == SLB_FN_LYAPUNOV_NN || fn->kind == SLB_FN_PENDULUM ||
-              fn->kind == SLB_FN_CARTPOLE || fn->kind == SLB_FN_VANDERPOL || fn->kind == SLB_FN_TRIANGULATION,
+              fn->kind == SLB_FN_CARTPOLE || fn->kind == SLB_FN_VANDERPOL || is_table(fn->kind),
               "%s: function kind %d has no VJP (NeuralNetwork, LyapunovNetwork, InvertedPendulum, CartPole, "
-              "VanDerPol, Triangulation)", what, fn->kind);
+              "VanDerPol, Triangulation, PiecewiseConstant)", what, fn->kind);
     SLB_CHECK(!(fn->flags & SLB_FLAG_GRADIENT) || (fn->kind != SLB_FN_MLP && fn->kind != SLB_FN_LYAPUNOV_NN),
               "%s: the VJP of a network gradient (SLB_FLAG_GRADIENT) is a Hessian-vector product, which is "
               "not implemented", what);
@@ -383,7 +385,7 @@ int vjp_validate(const slb_function* fn, const char* what) {
 extern "C" int64_t slb_function_vjp_workspace(const slb_function* fn, int64_t n) {
     if (vjp_validate(fn, "slb_function_vjp_workspace")) return -1;
     if (n < 0) { slb_set_error("slb_function_vjp_workspace: negative n"); return -1; }
-    if (fn->kind == SLB_FN_TRIANGULATION) return slb_triangulation_vjp_workspace(fn, n);
+    if (is_table(fn->kind)) return slb_triangulation_vjp_workspace(fn, n);
     if (is_plant(fn->kind)) return 0;
     net_shape S;
     network_shape(*fn, &S);
@@ -397,7 +399,7 @@ extern "C" int slb_function_vjp(void* stream, const slb_function* fn, const doub
     if (vjp_validate(fn, "slb_function_vjp")) return 1;
     SLB_CHECK(n >= 0, "slb_function_vjp: negative n (%lld)", (long long)n);
     cudaStream_t st = (cudaStream_t)stream;
-    if (fn->kind == SLB_FN_TRIANGULATION) {
+    if (is_table(fn->kind)) {
         SLB_CHECK(n == 0 || (points_dev != nullptr && grad_out_dev != nullptr),
                   "slb_function_vjp: null points or cotangent");
         return slb_triangulation_vjp(st, fn, points_dev, n, grad_out_dev, grad_in_dev, grad_params_dev, out_dev,

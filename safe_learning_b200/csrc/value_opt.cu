@@ -8,7 +8,9 @@
 //              the Bellman sweep), or x+ from a device array (composed); row i of T = the d + 1
 //              barycentric weights of x_i+ (the Triangulation lookup of common.cuh), with rows whose
 //              lookup extrapolates from the wrong simplex of the right cell (DESIGN.md §3.2 Q6)
-//              re-searched from cell-relative unit coordinates.
+//              re-searched from cell-relative unit coordinates.  A PiecewiseConstant value table gives
+//              one-hot rows: the next state's nearest vertex (grid_nearest_index) with weight 1, stored
+//              with a zero-weight second entry (the solver's narrowest row).
 //   solve      v_{k+1} = r + gamma (w_0 v_k[c_0] + ... + w_d v_k[c_d]), non-contracted, in this order
 //              (the arithmetic of one Bellman sweep), until the certified error
 //              gamma rho / (1 - gamma rho) ||v_k - v_{k-1}||_inf  <=  tol max(1, ||v_k||_inf),
@@ -59,16 +61,37 @@ SLB_DEV void stats_flush(row_stats& s, unsigned long long* __restrict__ stats) {
     }
 }
 
+// entries per row of T: d + 1 barycentric weights of a Triangulation, two for a PiecewiseConstant (its
+// one-hot row and a zero-weight filler: slb_value_solve takes rows of 2 .. SLB_MAX_DIM + 1 entries)
+SLB_DEV int operator_cols(const slb_function& f) {
+    return f.kind == SLB_FN_PIECEWISE_CONSTANT ? 2 : f.grid.ndim + 1;
+}
+
 // Row of T for the next state xp: columns (vertex indices) and weights.  The reference's lookup
 // (tri_lookup, common.cuh); when it yields a weight < -W_TOL although the point is inside the grid
 // (or projected onto it), the point lies on a grid line where `% unit_maxes` rounded to ~unit_maxes
 // and picked a simplex of the wrong side of the cell: search the cell again with unit coordinates
 // taken relative to the cell's own lowest vertex (TRI_CELL).
+// A PiecewiseConstant's row is the nearest vertex with weight 1, then the same vertex with weight 0: for a
+// finite v, w_0 v + 0 v is v bit for bit, so the solver's arithmetic is that of the one-hot row.  A NaN
+// next state has no vertex and gives vertex 0 with weight NaN, counted in the NaN slot like a
+// Triangulation's NaN row.
 template <typename IDX>
 SLB_DEV void operator_row(const slb_function& f, const double* xp, IDX* __restrict__ cols,
                           double* __restrict__ W, row_stats& st) {
     const slb_grid& g = f.grid;
     const int d = g.ndim;
+    if (f.kind == SLB_FN_PIECEWISE_CONSTANT) {
+        const int64_t v = grid_nearest_index(g, f.cparams, xp);
+        const double w = v < 0 ? __longlong_as_double(0x7ff8000000000000ll) : 1.0;
+        cols[0] = cols[1] = (IDX)(v < 0 ? 0 : v);
+        W[0] = w;
+        W[1] = 0.0;
+        st.minw_inv = umax(st.minw_inv, ~value_key(v < 0 ? w : 0.0));
+        st.rho = umax(st.rho, dbits(fabs(w)));
+        st.nan += v < 0;
+        return;
+    }
     int64_t corner;
     int s;
     double w[SLB_MAX_DIM + 1];
@@ -110,6 +133,7 @@ value_operator_kernel(const __grid_constant__ slb_bellman cfg, int64_t idx_begin
     const bool valid = i0 < n;
     const int64_t i = valid ? i0 : n - 1;       // every thread stays for the block barriers
     const int d = cfg.grid.ndim;
+    const int nc = operator_cols(cfg.value);
     double x[SLB_MAX_DIM], u[SLB_MAX_OUT], mu[SLB_MAX_OUT], r[SLB_MAX_OUT];
     grid_index_to_state(cfg.grid, idx_begin + i, x);
     const int m = eval_fn(cfg.policy, x, u);
@@ -119,9 +143,9 @@ value_operator_kernel(const __grid_constant__ slb_bellman cfg, int64_t idx_begin
         IDX c[SLB_MAX_DIM + 1];
         double w[SLB_MAX_DIM + 1];
         operator_row<IDX>(cfg.value, mu, c, w, st);
-        for (int k = 0; k <= d; ++k) {
-            cols[i * (d + 1) + k] = c[k];
-            weights[i * (d + 1) + k] = w[k];
+        for (int k = 0; k < nc; ++k) {
+            cols[i * nc + k] = c[k];
+            weights[i * nc + k] = w[k];
         }
         rewards[i] = r[0];
         st.nan += r[0] != r[0];
@@ -135,7 +159,7 @@ value_operator_points_kernel(const __grid_constant__ slb_function f, const doubl
                              int64_t n, IDX* __restrict__ cols, double* __restrict__ weights,
                              unsigned long long* __restrict__ stats) {
     const int64_t i = (int64_t)blockIdx.x * VT + threadIdx.x;
-    const int d = f.grid.ndim;
+    const int d = f.grid.ndim, nc = operator_cols(f);
     row_stats st = {0ull, 0ull, 0ull, 0ull};
     if (i < n) {
         double x[SLB_MAX_DIM];
@@ -143,9 +167,9 @@ value_operator_points_kernel(const __grid_constant__ slb_function f, const doubl
         IDX c[SLB_MAX_DIM + 1];
         double w[SLB_MAX_DIM + 1];
         operator_row<IDX>(f, x, c, w, st);
-        for (int k = 0; k <= d; ++k) {
-            cols[i * (d + 1) + k] = c[k];
-            weights[i * (d + 1) + k] = w[k];
+        for (int k = 0; k < nc; ++k) {
+            cols[i * nc + k] = c[k];
+            weights[i * nc + k] = w[k];
         }
     }
     stats_flush(st, stats);
@@ -351,10 +375,13 @@ value_solve_coop_kernel(const solve_args a, const IDX* __restrict__ cols, const 
 
 static bool wide_index(int64_t nindex) { return nindex > 0x7fffffffll; }
 
-// the rows of T are the barycentric weights of a one-output Triangulation (projection allowed)
+// the rows of T are the barycentric weights of a one-output Triangulation (projection allowed) or the
+// one-hot rows of a one-output PiecewiseConstant, without post-op flags
 static int validate_value_table(const slb_function& value, const char* who) {
-    SLB_CHECK(value.kind == SLB_FN_TRIANGULATION && value.out_dim == 1 && !(value.flags & ~SLB_FLAG_PROJECT),
-              "%s: the value function must be a plain one-output Triangulation", who);
+    const bool tri = value.kind == SLB_FN_TRIANGULATION && !(value.flags & ~SLB_FLAG_PROJECT);
+    const bool table = value.kind == SLB_FN_PIECEWISE_CONSTANT && value.flags == 0;
+    SLB_CHECK((tri || table) && value.out_dim == 1,
+              "%s: the value function must be a plain one-output Triangulation or PiecewiseConstant", who);
     return 0;
 }
 

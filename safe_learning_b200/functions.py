@@ -33,7 +33,7 @@ config = Configuration()
 __all__ = ["DimensionError", "GridWorld", "Function", "DeterministicFunction",
            "UncertainFunction", "ConstantFunction", "LinearSystem", "QuadraticFunction",
            "Saturation", "AbsFunction", "Norm1Function", "MaxAbsFunction", "ScaledFunction",
-           "Triangulation", "TriangulationGradient", "NetworkGradient",
+           "Triangulation", "TriangulationGradient", "PiecewiseConstant", "NetworkGradient",
            "Kernel", "RBF", "Matern12", "Matern32", "Matern52", "Linear", "Constant", "Bias",
            "White", "Sum", "Add", "Product", "Prod", "kernels", "Likelihood", "GPRCached", "GPR",
            "GaussianProcess", "FunctionStack",
@@ -684,18 +684,84 @@ class _TriangulationTables(object):
                                        shape=(n, self.nindex))
 
 
-class Triangulation(DeterministicFunction):
+class _VertexTable(object):
+    """The device vertex table [nindex, out] of ``Triangulation`` and ``PiecewiseConstant``: one buffer
+    (``_param_dev``) that the descriptor points at, one writer (``_store``) and one trainable leaf.
+
+    ``vertex_values`` hands out that buffer as a float64 leaf tensor with ``requires_grad``, for
+    ``torch.optim``: from then on every writer (the ``parameters`` setter, ``value_iteration``,
+    ``optimize_value_function``, ``discrete_policy_optimization``) copies into it in place, so the
+    leaf, the descriptor and the optimizer keep seeing one tensor, and the version follows its
+    in-place updates."""
+
+    _param_dev = None
+    _version = 0
+
+    def _set_table(self, values):
+        """Upload ``values`` (numpy or torch, reshaped to [nindex, -1])."""
+        if isinstance(values, (list, tuple)) and len(values) == 1:
+            values = values[0]
+        if isinstance(values, torch.Tensor):
+            vals = values.detach().to(dtype=torch.float64).reshape(self.nindex, -1)
+            self._store(vals.to(dev.device()).contiguous().clone())
+        else:
+            vals = np.asarray(values, dtype=np.float64).reshape(self.nindex, -1)
+            self._store(dev.to_device(vals))
+        self._version += 1
+
+    @property
+    def vertex_values(self):
+        """The vertex table [nindex, out] as a float64 leaf tensor with ``requires_grad`` -- the
+        descriptor's buffer itself, so in-place ``torch.optim`` steps are what the fused sweeps read."""
+        if self._param_dev is None:
+            raise ValueError("%s has no vertex values" % type(self).__name__)
+        if not self._param_dev.requires_grad:
+            self._param_dev = self._param_dev.detach().clone().requires_grad_(True)
+        return self._param_dev
+
+    def _store(self, values):
+        """The one writer of the vertex table (a device tensor [nindex, out]): swaps the buffer until
+        ``vertex_values`` has been handed out, then copies into that leaf in place."""
+        leaf = self._param_dev
+        if leaf is not None and leaf.requires_grad:
+            if tuple(values.shape) != tuple(leaf.shape):
+                raise DimensionError("vertex values of shape %s for a table of shape %s (the "
+                                     "vertex_values leaf keeps its shape)"
+                                     % (tuple(values.shape), tuple(leaf.shape)))
+            with torch.no_grad():
+                leaf.copy_(values)
+            return
+        self._param_dev = values
+        self.output_dim = int(values.shape[1])
+
+    def _trainable_tensors(self):
+        leaf = self._param_dev
+        return [leaf] if leaf is not None and leaf.requires_grad else []
+
+    def _table_vjp(self, points, grad_out):
+        """The vertex table's gradient: one ``slb_function_vjp`` call (the transpose of the lookup,
+        summed in a fixed order)."""
+        _, gflat, _ = _function_vjp(self, points, grad_out, want_in=False, nparams=self._param_dev.numel())
+        return [gflat.view(self._param_dev.shape).to(self._param_dev.device)]
+
+    def _table_version(self):
+        # the table is swapped (new device buffer) by value_iteration until vertex_values is handed out,
+        # and updated in place after, so its address and its version counter are part of the descriptor
+        # identity
+        if self._param_dev is None:
+            return (self._version, 0, 0)
+        return (self._version, self._param_dev.data_ptr(), self._param_dev._version)
+
+
+class Triangulation(_VertexTable, DeterministicFunction):
     """Piecewise-linear interpolation on a GridWorld (``functions.py:1372-1510``).
 
     The vertex values live in HBM (``_param_dev`` [nindex, out]); ``parameters`` exposes
     them like the reference's single tf.Variable: ``tri.parameters[0]`` is the [nindex, out]
     array, and assigning ``tri.parameters = values`` re-uploads.
 
-    ``vertex_values`` hands out that buffer as a float64 leaf tensor with ``requires_grad``, for
-    ``torch.optim``: from then on every writer (the ``parameters`` setter, ``value_iteration``,
-    ``optimize_value_function``, ``discrete_policy_optimization``) copies into it in place, so the
-    leaf, the descriptor and the optimizer keep seeing one tensor, and ``version`` follows its
-    in-place updates.  ``torch(points)`` differentiates the points and the vertex values.
+    ``vertex_values`` hands out that buffer as a trainable leaf (``_VertexTable``).  ``torch(points)``
+    differentiates the points and the vertex values.
     """
 
     def __init__(self, discretization, vertex_values, project=False, name="triangulation"):
@@ -735,63 +801,18 @@ class Triangulation(DeterministicFunction):
 
     @parameters.setter
     def parameters(self, values):
-        if isinstance(values, (list, tuple)) and len(values) == 1:
-            values = values[0]
-        if isinstance(values, torch.Tensor):
-            vals = values.detach().to(dtype=torch.float64).reshape(self.nindex, -1)
-            self._store(vals.to(dev.device()).contiguous().clone())
-        else:
-            vals = np.asarray(values, dtype=np.float64).reshape(self.nindex, -1)
-            self._store(dev.to_device(vals))
-        self._version += 1
-
-    @property
-    def vertex_values(self):
-        """The vertex table [nindex, out] as a float64 leaf tensor with ``requires_grad`` -- the
-        descriptor's buffer itself, so in-place ``torch.optim`` steps are what the fused sweeps read."""
-        if self._param_dev is None:
-            raise ValueError("Triangulation has no vertex values")
-        if not self._param_dev.requires_grad:
-            self._param_dev = self._param_dev.detach().clone().requires_grad_(True)
-        return self._param_dev
-
-    def _store(self, values):
-        """The one writer of the vertex table (a device tensor [nindex, out]): swaps the buffer until
-        ``vertex_values`` has been handed out, then copies into that leaf in place."""
-        leaf = self._param_dev
-        if leaf is not None and leaf.requires_grad:
-            if tuple(values.shape) != tuple(leaf.shape):
-                raise DimensionError("vertex values of shape %s for a table of shape %s (the "
-                                     "vertex_values leaf keeps its shape)"
-                                     % (tuple(values.shape), tuple(leaf.shape)))
-            with torch.no_grad():
-                leaf.copy_(values)
-            return
-        self._param_dev = values
-        self.output_dim = int(values.shape[1])
-
-    def _trainable_tensors(self):
-        leaf = self._param_dev
-        return [leaf] if leaf is not None and leaf.requires_grad else []
+        self._set_table(values)
 
     def _vjp(self, points, grad_out, want_in, want_params):
-        """The points' gradient from ``jacobian_device``; the vertex table's is one
-        ``slb_function_vjp`` call (the transpose of the lookup, summed in a fixed order)."""
+        """The points' gradient from ``jacobian_device``; the vertex table's from ``_table_vjp``."""
         gin, grads = super()._vjp(points, grad_out, want_in, False)
         if want_params:
-            _, gflat, _ = _function_vjp(self, points, grad_out, want_in=False,
-                                        nparams=self._param_dev.numel())
-            grads = [gflat.view(self._param_dev.shape).to(self._param_dev.device)]
+            grads = self._table_vjp(points, grad_out)
         return gin, grads
 
     @property
     def version(self):
-        # the vertex table is swapped (new device buffer) by value_iteration until vertex_values is
-        # handed out, and updated in place after, so its address and its version counter are part of
-        # the descriptor identity
-        if self._param_dev is None:
-            return (self._version, self.project, 0, 0)
-        return (self._version, self.project, self._param_dev.data_ptr(), self._param_dev._version)
+        return (self.project,) + self._table_version()
 
     def descriptor(self):
         if self._param_dev is None:
@@ -860,6 +881,97 @@ class TriangulationGradient(DeterministicFunction):
         d.flags |= nat.FLAG_GRADIENT
         d.out_dim = self.input_dim
         return d
+
+
+class PiecewiseConstant(_VertexTable, DeterministicFunction):
+    """Nearest-vertex table on a GridWorld (``functions.py:820-932``): ``pwc(x)`` is the row of
+    ``vertex_values`` at ``discretization.state_to_index(x)``, evaluated on the GPU by the same lookup in
+    every sweep, rollout, Bellman kernel and VJP (``SLB_FN_PIECEWISE_CONSTANT``, DESIGN.md §3.15).
+
+    ``parameters`` is the bare [nindex, out] array, as in the reference (the setter reshapes to
+    ``(nindex, -1)``); ``vertex_values`` hands the device table out as a trainable leaf, as for
+    ``Triangulation``.  A point with a NaN coordinate evaluates to NaN in every column (the reference
+    raises from ``ravel_multi_index``); ``parameter_derivative`` raises ``ValueError`` for it, as the
+    reference does.
+    """
+
+    def __init__(self, discretization, vertex_values=None, name="piecewise_constant"):
+        super().__init__(name)
+        self.discretization = discretization
+        self.input_dim = discretization.ndim
+        self.output_dim = None
+        self.parameters = vertex_values
+
+    @property
+    def parameters(self):
+        if self._param_dev is None:
+            return None
+        return self._param_dev.detach().cpu().numpy()
+
+    @parameters.setter
+    def parameters(self, values):
+        if values is None:
+            self._param_dev, self.output_dim = None, None
+            self._version += 1
+            return
+        self._set_table(values)
+
+    @property
+    def limits(self):
+        return self.discretization.limits
+
+    @property
+    def nindex(self):
+        return self.discretization.nindex
+
+    @property
+    def version(self):
+        return self._table_version()
+
+    def descriptor(self):
+        if self._param_dev is None:
+            raise ValueError("PiecewiseConstant has no vertex values")
+        d = nat.SlbFunction()
+        d.kind, d.in_dim, d.out_dim = nat.FN_PIECEWISE_CONSTANT, self.input_dim, self.output_dim
+        d.matrix = self._param_dev.data_ptr()
+        d.grid = self.discretization.descriptor()
+        for c, inv in enumerate(1. / self.discretization.unit_maxes):     # numpy's, as in state_to_index
+            d.cparams[c] = float(inv)
+        return d
+
+    def parameter_derivative(self, points):
+        """``PiecewiseConstant.parameter_derivative`` (``functions.py:889-913``): the sparse [n, nindex]
+        matrix of ones with ``pwc(points) = B @ parameters``; the columns come from the device lookup
+        (``slb_grid_nearest_index``)."""
+        lib = nat.load()
+        pts = dev.to_device(np.atleast_2d(np.asarray(points, dtype=np.float64)))
+        if pts.shape[1] != self.input_dim:
+            raise DimensionError("the input argument has the wrong dimensions.")
+        n = pts.shape[0]
+        idx = dev.empty((n,), torch.int64)
+        nat.check(lib.slb_grid_nearest_index(dev.stream(), self.discretization.descriptor(), pts.data_ptr(),
+                                             n, idx.data_ptr()), "slb_grid_nearest_index")
+        cols = idx.cpu().numpy()
+        if np.any(cols < 0):
+            raise ValueError("invalid entry in coordinates array (a point with a NaN coordinate)")
+        return scipy.sparse.coo_matrix((np.ones(n, dtype=np.int64), (np.arange(n), cols)),
+                                       shape=(n, self.nindex))
+
+    def gradient(self, points):
+        """Always zero (``functions.py:915-932``): the reference's broadcast ``[n, input_dim]``."""
+        return np.broadcast_to(0, (len(points), self.input_dim))
+
+    def gradient_function(self):
+        """The gradient as a fusable function object: the constant 0 in ``input_dim`` columns."""
+        return ConstantFunction(np.zeros(self.input_dim), input_dim=self.input_dim)
+
+    def jacobian_device(self, points):
+        return dev.zeros((points.shape[0], self.output_dim, self.input_dim))
+
+    def _vjp(self, points, grad_out, want_in, want_params):
+        """The points' gradient is zero; the vertex table's comes from ``_table_vjp``."""
+        gin = dev.zeros((points.shape[0], self.input_dim)) if want_in else None
+        return gin, (self._table_vjp(points, grad_out) if want_params else [])
 
 
 # =============================================================================== plants

@@ -16,8 +16,8 @@ import torch
 
 from . import _device as dev
 from . import _native as nat
-from .functions import (Function, FunctionStack, GaussianProcess, ScaledFunction, Triangulation,
-                        TriangulationGradient, UncertainFunction, _PostOp)
+from .functions import (Function, FunctionStack, GaussianProcess, PiecewiseConstant, ScaledFunction,
+                        Triangulation, TriangulationGradient, UncertainFunction, _PostOp)
 
 __all__ = ["PolicyIteration", "OptimizationError"]
 
@@ -49,13 +49,14 @@ def _on_triangulation_gradient(fn):
     return isinstance(fn, TriangulationGradient)
 
 
-def _triangulation_of(value_function):
-    """The Triangulation under an optional ``-V`` / ``c * V`` wrapper."""
+def _table_of(value_function):
+    """The vertex table (Triangulation or PiecewiseConstant) under an optional ``-V`` / ``c * V``
+    wrapper."""
     base = value_function
     while isinstance(base, ScaledFunction):
         base = base.fun
-    if not isinstance(base, Triangulation):
-        raise TypeError("value_function must be a Triangulation (possibly scaled)")
+    if not isinstance(base, (Triangulation, PiecewiseConstant)):
+        raise TypeError("value_function must be a Triangulation or a PiecewiseConstant (possibly scaled)")
     return base
 
 
@@ -79,7 +80,7 @@ class PolicyIteration(object):
         self.feed_dict = {}
         self._storage = {}
         self.factor_actions = True        # discrete_policy_optimization: see csrc/bellman_tile.cu
-        self._grid = _triangulation_of(value_function).discretization
+        self._grid = _table_of(value_function).discretization
         self._begin, self._end = dev.shard_range(self._grid.nindex)
 
     @property
@@ -211,7 +212,7 @@ class PolicyIteration(object):
         the OLD table, then the table is replaced.  Returns ``max |V_new - V_old|`` (the
         convergence test user code applies, ``tests/test_rl.py:66-69``)."""
         lib = nat.load()
-        tri = _triangulation_of(self.value_function)
+        tri = _table_of(self.value_function)
         scale = 1.0
         base = self.value_function
         while isinstance(base, ScaledFunction):
@@ -230,10 +231,11 @@ class PolicyIteration(object):
         return float(residual.item())
 
     def discrete_policy_optimization(self, action_space, constraint=None):
-        """Greedy policy over a discrete action set (``:213-279``): the piecewise-linear
-        policy's vertex values become ``action_space[argmax_a future_values(x, a)]``."""
+        """Greedy policy over a discrete action set (``:213-279``): the vertex values of the
+        piecewise-linear (Triangulation) or tabular (PiecewiseConstant) policy become
+        ``action_space[argmax_a future_values(x, a)]``."""
         lib = nat.load()
-        policy_tri = _triangulation_of(self.policy)
+        policy_tri = _table_of(self.policy)
         grid = policy_tri.discretization
         if grid.nindex != self._grid.nindex or np.any(grid.num_points != self._grid.num_points) \
                 or np.any(grid.limits != self._grid.limits):
@@ -287,7 +289,9 @@ class PolicyIteration(object):
         next state outside the grid), when ``gamma * rho >= 1``, when a reward, a next state or a
         value of the current table (the start point) is NaN,
         or when ``max_iters`` iterations do not reach the bound; ``TypeError`` when the value
-        function is not a plain one-output ``Triangulation``.  Next states on a grid line are looked
+        function is not a plain one-output ``Triangulation`` or ``PiecewiseConstant``.  A
+        ``PiecewiseConstant`` gives one-hot rows (the next state's nearest vertex, weight 1; DESIGN.md
+        §3.15), so rho = 1.  Next states on a grid line are looked
         up in the simplex that contains them (DESIGN.md §3.2 Q6; the reference's lookup can pick a
         simplex of the wrong side of the cell there, which makes its LP unbounded).
         """
@@ -322,13 +326,13 @@ class PolicyIteration(object):
         values in one device-to-host copy."""
         lib = nat.load()
         tri = self.value_function
-        if type(tri) is not Triangulation:
-            raise TypeError("optimize_value_function needs a plain Triangulation value function "
-                            "(the reference reaches value_function.tri), got %s" % type(tri).__name__)
+        if type(tri) not in (Triangulation, PiecewiseConstant):
+            raise TypeError("optimize_value_function needs a plain Triangulation or PiecewiseConstant value "
+                            "function (the reference reaches value_function.tri), got %s" % type(tri).__name__)
         if tri._param_dev is None or tri._param_dev.shape[1] != 1:
-            raise TypeError("optimize_value_function needs a one-output Triangulation")
+            raise TypeError("optimize_value_function needs a one-output %s" % type(tri).__name__)
         n, d = self._grid.nindex, self._grid.ndim
-        ncols = d + 1
+        ncols = 2 if type(tri) is PiecewiseConstant else d + 1         # value_opt.cu: operator_cols
         idx = torch.int64 if n > 0x7fffffff else torch.int32
         cols = dev.empty((n, ncols), idx)
         weights = dev.empty((n, ncols))
