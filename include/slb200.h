@@ -407,6 +407,16 @@ int slb_gp_predict(void* stream, const slb_gp_stack* gp, const double* points_de
  *      inf or NaN).  Every sum runs in a fixed order without atomics: two calls give bit-identical results.
  *      n == 0 launches nothing.  workspace_dev: >= slb_gp_vjp_workspace(gp, n) bytes (0 for every stack
  *      here); the size function returns -1 for a stack it rejects. */
+/* ---- posterior mean only (GaussianProcess.to_mean_function(), DESIGN.md §3.16): mean_dev [n, D] of the
+ *      stack at points_dev [n, d_in], d_in = 1..6, one point per thread on the Bellman sweep's staged
+ *      pipeline (slb_gp_factor.Xf and slb_gp_output.gamma_f, which must be present and 16-byte aligned
+ *      wherever a factor has data):  mean_o = (sum_j k_j gamma_f[o][j] + scale m_o(z)) / scale.
+ *      This is a different fp64 form from the full posterior's  a^T alpha  (the mean of the predict entry
+ *      point above): the two agree within the mean's rounding bound (DESIGN.md §3.16), not bit for bit.
+ *      A point's mean depends only on the training rows' order: not on n, the block or the slice size.
+ *      The closed-loop rollouts of the mean (slb_rollout_gp_mean) evaluate exactly this form.
+ *      Host checks (before any launch): the stack, its staged tables, n >= 0, non-null buffers. */
+int slb_gp_mean(void* stream, const slb_gp_stack* gp, const double* points_dev, int64_t n, double* mean_dev);
 int64_t slb_gp_vjp_workspace(const slb_gp_stack* gp, int64_t n);
 int slb_gp_vjp(void* stream, const slb_gp_stack* gp, const double* points_dev, int64_t n,
                const double* grad_mean_dev, const double* grad_err_dev, double* grad_points_dev,
@@ -578,7 +588,8 @@ int slb_max_abs_diff(void* stream, const double* a_dev, const double* b_dev, int
 
 /* ---- closed-loop rollouts x <- f(x, pi(x)) (examples/utilities.py:654-686 compute_roa,
  *      :522-545 reward_rollout).  The slb_bellman descriptor carries the closed loop: `policy`,
- *      deterministic `dynamics` (gp.num_outputs must be 0), and `reward` for slb_reward_rollout;
+ *      deterministic `dynamics` (gp.num_outputs must be 0; the _gp_mean forms below take the GP mean),
+ *      and `reward` for slb_reward_rollout;
  *      `value`, `gamma` and `action` are ignored, fixed_action must be 0.  The state dimension d is
  *      grid.ndim.  Start states: the device array states_dev [n, d], or, when states_dev is NULL,
  *      the grid points of flat indices [idx_begin, idx_begin + n).
@@ -599,6 +610,17 @@ int slb_rollout(void* stream, const slb_bellman* cfg, const double* states_dev, 
 int slb_reward_rollout(void* stream, const slb_bellman* cfg, const double* states_dev, int64_t idx_begin,
                        int64_t n, int32_t horizon, const double* discount_dev, double tol,
                        double* sums_dev, int64_t* stop_dev, void* workspace_dev);
+/* The same two rollouts with the GP posterior mean as the dynamics: cfg->gp holds the stack with
+ * num_outputs == d and input_dim == d + m (at most 6), cfg->dynamics.kind must be SLB_FN_NONE and the
+ * staged tables present (as for slb_gp_mean).  Every step evaluates slb_gp_mean's form, so a rollout of
+ * h steps is bit-identical to h compositions of the policy's evaluation and slb_gp_mean.  Workspace:
+ * slb_rollout_workspace, as above. */
+int slb_rollout_gp_mean(void* stream, const slb_bellman* cfg, const double* states_dev, int64_t idx_begin,
+                        int64_t n, int32_t horizon, const double* equilibrium_host, double tol,
+                        uint8_t* roa_dev, double* end_states_dev, double* traj_dev, void* workspace_dev);
+int slb_reward_rollout_gp_mean(void* stream, const slb_bellman* cfg, const double* states_dev,
+                               int64_t idx_begin, int64_t n, int32_t horizon, const double* discount_dev,
+                               double tol, double* sums_dev, int64_t* stop_dev, void* workspace_dev);
 
 /* ---- exact policy evaluation (reinforcement_learning.py:142-211 optimize_value_function): the
  *      fixed point of  v = r + gamma T v,  T = the value table's rows at the mean next states

@@ -12,5 +12,6 @@ from .lyapunov import *  # noqa: F401,F403
 from .reinforcement_learning import *  # noqa: F401,F403
 from .rollout import *  # noqa: F401,F403
 from . import utilities  # noqa: F401
+from .utilities import compute_trajectory  # noqa: F401
 
 __version__ = "0.1.0"

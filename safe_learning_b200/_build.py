@@ -26,7 +26,7 @@ UNITS += [("gp_sweep.o", "gp_sweep.cu", [], ["gp_args.h"]),
                                          "gp_args.h"]),
           ("light.o", "light.cu", [], ["bulk_copy.cuh", "exp2_tab512.cuh", "gp_mean_staged.cuh", "bellman.cuh"]),
           ("bellman_tile.o", "bellman_tile.cu", [], []),
-          ("rollout.o", "rollout.cu", [], []),
+          ("rollout.o", "rollout.cu", [], ["bulk_copy.cuh", "exp2_tab512.cuh", "gp_mean_staged.cuh", "bellman.cuh"]),
           ("value_opt.o", "value_opt.cu", [], ["bulk_copy.cuh", "exp2_tab512.cuh", "gp_mean_staged.cuh",
                                                "bellman.cuh"]),
           ("network_grad.o", "network_grad.cu", [], []),

@@ -184,6 +184,10 @@ SIGNATURES = {
                               _vp, _dp, _dp, _vp]),
     "slb_reward_rollout": (C.c_int, [_vp, C.POINTER(SlbBellman), _dp, _i64, _i64, _i32, _dp,
                                      C.c_double, _dp, _vp, _vp]),
+    "slb_rollout_gp_mean": (C.c_int, [_vp, C.POINTER(SlbBellman), _dp, _i64, _i64, _i32, _dp, C.c_double,
+                                      _vp, _dp, _dp, _vp]),
+    "slb_reward_rollout_gp_mean": (C.c_int, [_vp, C.POINTER(SlbBellman), _dp, _i64, _i64, _i32, _dp,
+                                             C.c_double, _dp, _vp, _vp]),
     "slb_value_operator": (C.c_int, [_vp, C.POINTER(SlbBellman), _i64, _i64, _vp, _dp, _dp, _vp]),
     "slb_value_operator_points": (C.c_int, [_vp, C.POINTER(SlbFunction), _dp, _i64, _vp, _dp, _vp]),
     "slb_value_solve_workspace": (C.c_int64, [_i64, _i32]),
@@ -193,6 +197,7 @@ SIGNATURES = {
     "slb_function_vjp": (C.c_int, [_vp, C.POINTER(SlbFunction), _dp, _i64, _dp, _dp, _dp, _dp, _vp]),
     "slb_triangulation_rows": (C.c_int, [_vp, C.POINTER(SlbFunction), _dp, _i64, _vp, _dp]),
     "slb_grid_nearest_index": (C.c_int, [_vp, C.POINTER(SlbGrid), _dp, _i64, _vp]),
+    "slb_gp_mean": (C.c_int, [_vp, C.POINTER(SlbGpStack), _dp, _i64, _dp]),
     "slb_gp_vjp_workspace": (C.c_int64, [C.POINTER(SlbGpStack), _i64]),
     "slb_gp_vjp": (C.c_int, [_vp, C.POINTER(SlbGpStack), _dp, _i64, _dp, _dp, _dp, _vp]),
     "slb_gp_lml_grad_workspace": (C.c_int64, [_i32]),

@@ -11,13 +11,19 @@
 // stores are coalesced.  Every step is eval_fn's arithmetic, so a rollout of h steps is bit-identical
 // to h compositions of the library's one-step evaluations (slb_eval_function).
 //
+// The dynamics are either a fused function (DIN = 0: eval_fn) or the posterior mean of a GP stack
+// (DIN = d_in = d + m, 1..6: the Bellman sweep's staged pipeline, bellman.cuh, set up once per launch
+// and restarted per step; slb_gp_mean is its one-step form, so the same bit-identity holds).  The
+// pipeline has block barriers: in the GP instantiations every thread stays to the end, threads past
+// n clamp their index and store nothing.
+//
 // Early stop of reward_rollout without a host round trip per chunk: each chunk kernel writes, per
 // step and per block, the maximum of |temp| (doubles >= 0 ordered by their bit patterns, so a NaN
 // sorts above inf and never passes `< tol`, like np.max); a one-block finish kernel reduces the
 // chunk's table and records the first step T* whose maximum is below tol.  The chunk after it
 // re-runs the chunk holding T* from its saved start state and sums exactly up to T*; every later
 // launch sees the control word and exits at once.  Cost: at most one extra chunk.
-#include "common.cuh"
+#include "bellman.cuh"
 
 #include <string.h>
 
@@ -60,6 +66,15 @@ SLB_DEV void apply_dynamics(const slb_bellman& cfg, double* z, int d) {
     for (int c = 0; c < d; ++c) z[c] = y[c];
 }
 
+// x <- mean f([x, u]) of the GP stack (every thread of the block takes part: barriers)
+template <int DIN>
+SLB_DEV void apply_gp_mean(const slb_bellman& cfg, bellman_smem& S, double* z, int d) {
+    double mu[SLB_MAX_OUT], err[SLB_MAX_OUT];
+    mean_pipe_start<DIN>(cfg.gp, S.P);
+    gp_mean_staged<DIN, false>(cfg.gp, z, mu, err, S.tab512, S.tab64, S.P);
+    for (int c = 0; c < d; ++c) z[c] = mu[c];
+}
+
 // Trajectory output [n, d, horizon] (the reference's layout): consecutive steps of one coordinate
 // are contiguous, so a thread's per-step stores are d * horizon * 8 B apart from its neighbours'.
 // Each thread stages up to SECTOR steps per coordinate in shared memory and writes them once it
@@ -90,15 +105,29 @@ struct traj_stage {
 
 // compute_roa: steps t in [t_begin, t_end) of x_t = f(x_{t-1}, pi(x_{t-1})), t >= 1.  The first
 // launch (t_begin == 1) reads the start states; the last one applies the distance test
-// norm(x - eq, 2) <= tol (numpy's row norm: sqrt of the sequential sum of squares).
+// norm(x - eq, 2) <= tol (numpy's row norm: sqrt of the sequential sum of squares).  DIN > 0: the GP
+// mean's slices in dynamic shared memory (chunk_rows, nomax of bellman_stage_config), the trajectory
+// staging behind them.
+template <int DIN>
 __global__ void __launch_bounds__(RT_MAX)
 roa_chunk_kernel(const __grid_constant__ slb_bellman cfg, const double* __restrict__ states,
                  int64_t idx_begin, int64_t n, int t_begin, int t_end, int horizon,
                  const double* __restrict__ x_in, double* __restrict__ x_out, double* __restrict__ traj,
-                 const roa_epilogue ep, uint8_t* __restrict__ roa, double* __restrict__ end_states) {
+                 const roa_epilogue ep, uint8_t* __restrict__ roa, double* __restrict__ end_states,
+                 int chunk_rows, int nomax) {
     extern __shared__ double s_traj[];
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;                                   // no block barrier below
+    const int64_t i0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    bellman_smem S;
+    double* stage = s_traj;
+    if constexpr (DIN == 0) {
+        if (i0 >= n) return;                              // no block barrier below
+    } else {
+        extern __shared__ __align__(16) unsigned char smem_raw[];
+        bellman_setup<DIN>(S, smem_raw, cfg, chunk_rows, nomax);
+        stage = S.P.gbuf + 2 * S.P.gstride;
+    }
+    const bool valid = DIN == 0 || i0 < n;
+    const int64_t i = valid ? i0 : n - 1;                 // every thread stays for the block barriers
     const int d = cfg.grid.ndim;
     double z[SLB_MAX_IN];
     if (t_begin == 1) {
@@ -107,8 +136,9 @@ roa_chunk_kernel(const __grid_constant__ slb_bellman cfg, const double* __restri
         for (int c = 0; c < d; ++c) z[c] = x_in[c * n + i];
     }
     traj_stage ts;
-    if (traj != nullptr) {
-        ts.s = s_traj;
+    const bool write_traj = traj != nullptr && valid;
+    if (write_traj) {
+        ts.s = stage;
         ts.row = i * d * (int64_t)horizon;
         ts.out = traj + ts.row;
         ts.horizon = horizon;
@@ -118,10 +148,12 @@ roa_chunk_kernel(const __grid_constant__ slb_bellman cfg, const double* __restri
     }
     for (int t = t_begin; t < t_end; ++t) {
         apply_policy(cfg, z, d);
-        apply_dynamics(cfg, z, d);
-        if (traj != nullptr)
+        if constexpr (DIN == 0) apply_dynamics(cfg, z, d);
+        else apply_gp_mean<DIN>(cfg, S, z, d);
+        if (write_traj)
             for (int c = 0; c < d; ++c) ts.put(c, t, z[c], t_end - 1);
     }
+    if (!valid) return;
     if (ep.last) {
         double ss = 0.0;
         for (int c = 0; c < d; ++c) {
@@ -142,12 +174,15 @@ roa_chunk_kernel(const __grid_constant__ slb_bellman cfg, const double* __restri
 // with the per-block maximum of |temp| per step into partial[step][block].  Chunk c reads
 // buf[c & 1] (chunk 0 the start states) and writes buf[(c + 1) & 1] = [x (d rows); sum] of [n].
 // After the finish kernel found T* in chunk c, launch c + 1 re-runs chunk c up to T* instead.
+// DIN > 0: the GP mean's slices in dynamic shared memory, as in roa_chunk_kernel.
+template <int DIN>
 __global__ void __launch_bounds__(RT_MAX)
 reward_chunk_kernel(const __grid_constant__ slb_bellman cfg, const double* __restrict__ states,
                     int64_t idx_begin, int64_t n, int chunk, int nchunks, int horizon,
                     const double* __restrict__ discount, double* __restrict__ buf0,
                     double* __restrict__ buf1, double* __restrict__ sums,
-                    uint64_t* __restrict__ partial, const roll_ctrl* __restrict__ ctrl) {
+                    uint64_t* __restrict__ partial, const roll_ctrl* __restrict__ ctrl,
+                    int chunk_rows, int nomax) {
     __shared__ uint64_t s_max[RK][RT_MAX / 32];
     const int phase = ctrl->phase;                        // written by the previous finish kernel
     if (phase == 2) return;
@@ -156,6 +191,11 @@ reward_chunk_kernel(const __grid_constant__ slb_bellman cfg, const double* __res
     const int run = fixup ? chunk - 1 : chunk;
     const int t0 = run * RK;
     const int t1 = fixup ? (int)ctrl->stop + 1 : min(t0 + RK, horizon);
+    bellman_smem S;
+    if constexpr (DIN > 0) {
+        extern __shared__ __align__(16) unsigned char smem_raw[];
+        bellman_setup<DIN>(S, smem_raw, cfg, chunk_rows, nomax);
+    }
     const int64_t i0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const bool valid = i0 < n;
     const int64_t i = valid ? i0 : n - 1;                 // every thread stays for the block maxima
@@ -176,7 +216,8 @@ reward_chunk_kernel(const __grid_constant__ slb_bellman cfg, const double* __res
         eval_fn(cfg.reward, z, r);
         const double temp = f64mul(__ldg(discount + t), r[0]);
         sum = f64add(sum, temp);
-        apply_dynamics(cfg, z, d);
+        if constexpr (DIN == 0) apply_dynamics(cfg, z, d);
+        else apply_gp_mean<DIN>(cfg, S, z, d);
         if (!fixup) {
             unsigned long long b = valid ? (unsigned long long)__double_as_longlong(fabs(temp)) : 0ull;
 #pragma unroll
@@ -256,10 +297,12 @@ int rollout_block(int64_t n) {
     return bs;
 }
 
+// gp_mean: the dynamics are the posterior mean of cfg->gp (slb_rollout_gp_mean / slb_reward_rollout_gp_mean)
 int validate_rollout(const char* who, const slb_bellman* cfg, const double* states_dev, int64_t idx_begin,
-                     int64_t n, int32_t horizon, bool reward) {
+                     int64_t n, int32_t horizon, bool reward, bool gp_mean) {
     SLB_CHECK(cfg != nullptr, "%s: null config", who);
-    SLB_CHECK(cfg->gp.num_outputs == 0, "%s: GP dynamics cannot be rolled out (gp.num_outputs must be 0)", who);
+    SLB_CHECK(gp_mean || cfg->gp.num_outputs == 0,
+              "%s: GP dynamics cannot be rolled out (gp.num_outputs must be 0)", who);
     SLB_CHECK(!cfg->fixed_action, "%s: a rollout follows the policy (fixed_action must be 0)", who);
     const int d = cfg->grid.ndim;
     SLB_CHECK(d >= 1 && d <= SLB_MAX_DIM, "%s: state dimension %d outside 1..%d", who, d, SLB_MAX_DIM);
@@ -274,7 +317,19 @@ int validate_rollout(const char* who, const slb_bellman* cfg, const double* stat
     const int m = slb_fn_columns(cfg->policy);
     SLB_CHECK(m >= 1 && d + m <= SLB_MAX_IN, "%s: state %d + action %d exceeds %d inputs", who, d, m,
               SLB_MAX_IN);
-    if (slb_validate_dynamics(&cfg->dynamics, who, d, m)) return 1;
+    if (gp_mean) {
+        SLB_CHECK(cfg->gp.num_outputs == d, "%s: the GP stack has %d outputs but the state has %d dims",
+                  who, cfg->gp.num_outputs, d);
+        if (slb_validate_gp(&cfg->gp)) return 1;
+        SLB_CHECK(cfg->gp.input_dim == d + m, "%s: GP input_dim %d != state %d + action %d", who,
+                  cfg->gp.input_dim, d, m);
+        SLB_CHECK(d + m <= 6, "%s: GP input_dim %d not compiled (1..6)", who, d + m);
+        SLB_CHECK(cfg->dynamics.kind == SLB_FN_NONE,
+                  "%s: the GP mean is the dynamics (dynamics.kind must be SLB_FN_NONE)", who);
+        if (slb_validate_staged_tables(&cfg->gp, who)) return 1;
+    } else if (slb_validate_dynamics(&cfg->dynamics, who, d, m)) {
+        return 1;
+    }
     if (reward) {
         if (slb_validate_function(&cfg->reward, "reward_function", d + m)) return 1;
         SLB_CHECK(cfg->reward.kind != SLB_FN_NONE, "%s: a reward function is required", who);
@@ -283,7 +338,124 @@ int validate_rollout(const char* who, const slb_bellman* cfg, const double* stat
     return 0;
 }
 
+// Launches the chunk kernel of the dynamics' source: launch(D, smem, chunk_rows, nomax) with D = 0
+// (fused dynamics, `extra` bytes of dynamic shared memory) or D = d_in of the GP stack (its pipeline,
+// then `extra` bytes; the kernel `kern(D)` opts in beyond 48 KB).
+template <class K, class F>
+int launch_rollout(const slb_bellman& cfg, bool gp_mean, size_t extra, K&& kern, F&& launch) {
+    if (!gp_mean) return launch(std::integral_constant<int, 0>{}, extra, 0, 0);
+    int chunk_rows, nomax;
+    const size_t smem = bellman_stage_config(cfg, cfg.gp.input_dim, &chunk_rows, &nomax) + extra;
+    return slb_dispatch_dim<1, 6>(cfg.gp.input_dim, "rollout: GP input_dim", [&](auto D) {
+        if (smem > 48 * 1024)
+            SLB_CUDA(cudaFuncSetAttribute(kern(D), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        return launch(D, smem, chunk_rows, nomax);
+    });
+}
+
+// The one-step posterior mean (slb_gp_mean): one point per thread on the Bellman sweep's pipeline.
+constexpr int GM_THREADS = 256;
+
+template <int DIN>
+__global__ void __launch_bounds__(GM_THREADS, 2)
+gp_mean_kernel(const __grid_constant__ slb_bellman cfg, const double* __restrict__ points, int64_t n,
+               double* __restrict__ mean, int chunk_rows, int nomax) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    bellman_smem S;
+    bellman_setup<DIN>(S, smem_raw, cfg, chunk_rows, nomax);
+    const int64_t i0 = (int64_t)blockIdx.x * GM_THREADS + threadIdx.x;
+    const bool valid = i0 < n;
+    const int64_t i = valid ? i0 : n - 1;                 // every thread stays for the block barriers
+    double z[SLB_MAX_IN], mu[SLB_MAX_OUT], err[SLB_MAX_OUT];
+#pragma unroll
+    for (int c = 0; c < DIN; ++c) z[c] = points[i * DIN + c];
+    mean_pipe_start<DIN>(cfg.gp, S.P);
+    gp_mean_staged<DIN, false>(cfg.gp, z, mu, err, S.tab512, S.tab64, S.P);
+    if (!valid) return;
+    const int D = cfg.gp.num_outputs;
+    for (int o = 0; o < D; ++o) mean[i * D + o] = mu[o];
+}
+
 int64_t align256(int64_t b) { return (b + 255) & ~(int64_t)255; }
+
+int rollout_impl(const char* who, bool gp_mean, void* stream, const slb_bellman* cfg,
+                 const double* states_dev, int64_t idx_begin, int64_t n, int32_t horizon,
+                 const double* equilibrium_host, double tol, uint8_t* roa_dev, double* end_states_dev,
+                 double* traj_dev, void* workspace_dev) {
+    if (validate_rollout(who, cfg, states_dev, idx_begin, n, horizon, false, gp_mean)) return 1;
+    SLB_CHECK(traj_dev == nullptr || horizon >= 1, "%s: trajectories need horizon >= 1", who);
+    if (n == 0) return 0;
+    SLB_CHECK(roa_dev != nullptr, "%s: null flag output", who);
+    const int d = cfg->grid.ndim;
+    const int steps = horizon > 1 ? horizon - 1 : 0;         // range(1, horizon)
+    const int nchunks = steps > 0 ? (steps + RK - 1) / RK : 1;
+    SLB_CHECK(nchunks == 1 || workspace_dev != nullptr, "%s: null workspace", who);
+    roa_epilogue ep;
+    memset(&ep, 0, sizeof(ep));
+    for (int c = 0; c < d; ++c) ep.eq[c] = equilibrium_host != nullptr ? equilibrium_host[c] : 0.0;
+    ep.tol = tol;
+    double* buf[2] = {static_cast<double*>(workspace_dev), nullptr};
+    if (workspace_dev != nullptr) buf[1] = buf[0] + align256(n * d * 8) / 8;
+    const int bs = rollout_block(n);
+    const unsigned nb = (unsigned)((n + bs - 1) / bs);
+    const size_t traj_smem = traj_dev != nullptr ? (size_t)bs * d * SECTOR * sizeof(double) : 0;
+    cudaStream_t st = (cudaStream_t)stream;
+    return launch_rollout(*cfg, gp_mean, traj_smem, [](auto D) { return roa_chunk_kernel<decltype(D)::value>; },
+                          [&](auto D, size_t smem, int chunk_rows, int nomax) {
+        for (int c = 0; c < nchunks; ++c) {
+            const int t_begin = 1 + c * RK;
+            const int t_end = steps > 0 ? min(t_begin + RK, horizon) : 1;
+            ep.last = c == nchunks - 1;
+            roa_chunk_kernel<decltype(D)::value><<<nb, bs, smem, st>>>(
+                *cfg, states_dev, idx_begin, n, t_begin, t_end, horizon, buf[c & 1], buf[(c + 1) & 1], traj_dev,
+                ep, roa_dev, end_states_dev, chunk_rows, nomax);
+            SLB_LAUNCH_CHECK();
+        }
+        return 0;
+    });
+}
+
+int reward_rollout_impl(const char* who, bool gp_mean, void* stream, const slb_bellman* cfg,
+                        const double* states_dev, int64_t idx_begin, int64_t n, int32_t horizon,
+                        const double* discount_dev, double tol, double* sums_dev, int64_t* stop_dev,
+                        void* workspace_dev) {
+    if (validate_rollout(who, cfg, states_dev, idx_begin, n, horizon, true, gp_mean)) return 1;
+    SLB_CHECK(stop_dev != nullptr, "%s: null stop output", who);
+    cudaStream_t st = (cudaStream_t)stream;
+    SLB_CUDA(cudaMemsetAsync(stop_dev, 0xff, sizeof(int64_t), st));          // -1: not converged
+    if (n == 0) return 0;
+    SLB_CHECK(sums_dev != nullptr, "%s: null output", who);
+    if (horizon == 0) {
+        SLB_CUDA(cudaMemsetAsync(sums_dev, 0, (size_t)n * sizeof(double), st));
+        return 0;
+    }
+    SLB_CHECK(discount_dev != nullptr && workspace_dev != nullptr, "%s: null discount/workspace", who);
+    const int d = cfg->grid.ndim;
+    const int bs = rollout_block(n);
+    const int nb = (int)((n + bs - 1) / bs);
+    char* w = static_cast<char*>(workspace_dev);
+    double* buf0 = reinterpret_cast<double*>(w);
+    double* buf1 = reinterpret_cast<double*>(w + align256(n * (d + 1) * 8));
+    uint64_t* partial = reinterpret_cast<uint64_t*>(w + 2 * align256(n * (d + 1) * 8));
+    roll_ctrl* ctrl = reinterpret_cast<roll_ctrl*>(reinterpret_cast<char*>(partial) + align256(RK * (int64_t)nb * 8));
+    SLB_CUDA(cudaMemsetAsync(ctrl, 0, sizeof(roll_ctrl), st));
+    uint64_t tol_bits = 0;                                 // max |temp| < tol: never when tol <= 0 or NaN
+    if (tol > 0.0) memcpy(&tol_bits, &tol, sizeof(tol_bits));
+    const int nchunks = (horizon + RK - 1) / RK;
+    return launch_rollout(*cfg, gp_mean, 0, [](auto D) { return reward_chunk_kernel<decltype(D)::value>; },
+                          [&](auto D, size_t smem, int chunk_rows, int nomax) {
+        for (int c = 0; c <= nchunks; ++c) {               // launch nchunks: the re-run of the last chunk
+            reward_chunk_kernel<decltype(D)::value><<<nb, bs, smem, st>>>(
+                *cfg, states_dev, idx_begin, n, c, nchunks, horizon, discount_dev, buf0, buf1, sums_dev, partial,
+                ctrl, chunk_rows, nomax);
+            SLB_LAUNCH_CHECK();
+            if (c == nchunks) break;
+            reward_finish_kernel<<<1, FIN_THREADS, 0, st>>>(partial, nb, c, horizon, tol_bits, ctrl, stop_dev);
+            SLB_LAUNCH_CHECK();
+        }
+        return 0;
+    });
+}
 
 }  // namespace
 
@@ -300,71 +472,53 @@ int64_t slb_rollout_workspace(const slb_bellman* cfg, int64_t n, int32_t reward)
 int slb_rollout(void* stream, const slb_bellman* cfg, const double* states_dev, int64_t idx_begin,
                 int64_t n, int32_t horizon, const double* equilibrium_host, double tol,
                 uint8_t* roa_dev, double* end_states_dev, double* traj_dev, void* workspace_dev) {
-    if (validate_rollout("slb_rollout", cfg, states_dev, idx_begin, n, horizon, false)) return 1;
-    SLB_CHECK(traj_dev == nullptr || horizon >= 1, "slb_rollout: trajectories need horizon >= 1");
-    if (n == 0) return 0;
-    SLB_CHECK(roa_dev != nullptr, "slb_rollout: null flag output");
-    const int d = cfg->grid.ndim;
-    const int steps = horizon > 1 ? horizon - 1 : 0;         // range(1, horizon)
-    const int nchunks = steps > 0 ? (steps + RK - 1) / RK : 1;
-    SLB_CHECK(nchunks == 1 || workspace_dev != nullptr, "slb_rollout: null workspace");
-    roa_epilogue ep;
-    memset(&ep, 0, sizeof(ep));
-    for (int c = 0; c < d; ++c) ep.eq[c] = equilibrium_host != nullptr ? equilibrium_host[c] : 0.0;
-    ep.tol = tol;
-    double* buf[2] = {static_cast<double*>(workspace_dev), nullptr};
-    if (workspace_dev != nullptr) buf[1] = buf[0] + align256(n * d * 8) / 8;
-    const int bs = rollout_block(n);
-    const unsigned nb = (unsigned)((n + bs - 1) / bs);
-    const size_t smem = traj_dev != nullptr ? (size_t)bs * d * SECTOR * sizeof(double) : 0;
-    cudaStream_t st = (cudaStream_t)stream;
-    for (int c = 0; c < nchunks; ++c) {
-        const int t_begin = 1 + c * RK;
-        const int t_end = steps > 0 ? min(t_begin + RK, horizon) : 1;
-        ep.last = c == nchunks - 1;
-        roa_chunk_kernel<<<nb, bs, smem, st>>>(*cfg, states_dev, idx_begin, n, t_begin, t_end, horizon,
-                                              buf[c & 1], buf[(c + 1) & 1], traj_dev, ep, roa_dev,
-                                              end_states_dev);
-        SLB_LAUNCH_CHECK();
-    }
-    return 0;
+    return rollout_impl("slb_rollout", false, stream, cfg, states_dev, idx_begin, n, horizon, equilibrium_host, tol,
+                   roa_dev, end_states_dev, traj_dev, workspace_dev);
+}
+
+int slb_rollout_gp_mean(void* stream, const slb_bellman* cfg, const double* states_dev, int64_t idx_begin,
+                        int64_t n, int32_t horizon, const double* equilibrium_host, double tol,
+                        uint8_t* roa_dev, double* end_states_dev, double* traj_dev, void* workspace_dev) {
+    return rollout_impl("slb_rollout_gp_mean", true, stream, cfg, states_dev, idx_begin, n, horizon, equilibrium_host,
+                   tol, roa_dev, end_states_dev, traj_dev, workspace_dev);
 }
 
 int slb_reward_rollout(void* stream, const slb_bellman* cfg, const double* states_dev, int64_t idx_begin,
                        int64_t n, int32_t horizon, const double* discount_dev, double tol,
                        double* sums_dev, int64_t* stop_dev, void* workspace_dev) {
-    if (validate_rollout("slb_reward_rollout", cfg, states_dev, idx_begin, n, horizon, true)) return 1;
-    SLB_CHECK(stop_dev != nullptr, "slb_reward_rollout: null stop output");
-    cudaStream_t st = (cudaStream_t)stream;
-    SLB_CUDA(cudaMemsetAsync(stop_dev, 0xff, sizeof(int64_t), st));          // -1: not converged
+    return reward_rollout_impl("slb_reward_rollout", false, stream, cfg, states_dev, idx_begin, n, horizon,
+                          discount_dev, tol, sums_dev, stop_dev, workspace_dev);
+}
+
+int slb_reward_rollout_gp_mean(void* stream, const slb_bellman* cfg, const double* states_dev,
+                               int64_t idx_begin, int64_t n, int32_t horizon, const double* discount_dev,
+                               double tol, double* sums_dev, int64_t* stop_dev, void* workspace_dev) {
+    return reward_rollout_impl("slb_reward_rollout_gp_mean", true, stream, cfg, states_dev, idx_begin, n, horizon,
+                          discount_dev, tol, sums_dev, stop_dev, workspace_dev);
+}
+
+int slb_gp_mean(void* stream, const slb_gp_stack* gp, const double* points_dev, int64_t n, double* mean_dev) {
+    SLB_CHECK(gp != nullptr, "slb_gp_mean: null gp");
+    if (slb_validate_gp(gp)) return 1;
+    SLB_CHECK(gp->num_outputs > 0, "slb_gp_mean: GP stack has no outputs");
+    SLB_CHECK(gp->input_dim >= 1 && gp->input_dim <= 6, "slb_gp_mean: GP input_dim %d not compiled (1..6)",
+              gp->input_dim);
+    if (slb_validate_staged_tables(gp, "slb_gp_mean")) return 1;
+    SLB_CHECK(n >= 0, "slb_gp_mean: negative n");
+    SLB_CHECK(n == 0 || (points_dev != nullptr && mean_dev != nullptr), "slb_gp_mean: null buffer");
     if (n == 0) return 0;
-    SLB_CHECK(sums_dev != nullptr, "slb_reward_rollout: null output");
-    if (horizon == 0) {
-        SLB_CUDA(cudaMemsetAsync(sums_dev, 0, (size_t)n * sizeof(double), st));
+    slb_bellman cfg;
+    memset(&cfg, 0, sizeof(cfg));
+    cfg.gp = *gp;
+    int chunk_rows, nomax;
+    const size_t smem = bellman_stage_config(cfg, gp->input_dim, &chunk_rows, &nomax);
+    const unsigned nb = (unsigned)((n + GM_THREADS - 1) / GM_THREADS);
+    return slb_dispatch_dim<1, 6>(gp->input_dim, "slb_gp_mean: GP input_dim", [&](auto D) {
+        gp_mean_kernel<decltype(D)::value><<<nb, GM_THREADS, smem, (cudaStream_t)stream>>>(
+            cfg, points_dev, n, mean_dev, chunk_rows, nomax);
+        SLB_LAUNCH_CHECK();
         return 0;
-    }
-    SLB_CHECK(discount_dev != nullptr && workspace_dev != nullptr, "slb_reward_rollout: null discount/workspace");
-    const int d = cfg->grid.ndim;
-    const int bs = rollout_block(n);
-    const int nb = (int)((n + bs - 1) / bs);
-    char* w = static_cast<char*>(workspace_dev);
-    double* buf0 = reinterpret_cast<double*>(w);
-    double* buf1 = reinterpret_cast<double*>(w + align256(n * (d + 1) * 8));
-    uint64_t* partial = reinterpret_cast<uint64_t*>(w + 2 * align256(n * (d + 1) * 8));
-    roll_ctrl* ctrl = reinterpret_cast<roll_ctrl*>(reinterpret_cast<char*>(partial) + align256(RK * (int64_t)nb * 8));
-    SLB_CUDA(cudaMemsetAsync(ctrl, 0, sizeof(roll_ctrl), st));
-    uint64_t tol_bits = 0;                                 // max |temp| < tol: never when tol <= 0 or NaN
-    if (tol > 0.0) memcpy(&tol_bits, &tol, sizeof(tol_bits));
-    const int nchunks = (horizon + RK - 1) / RK;
-    for (int c = 0; c <= nchunks; ++c) {                   // launch nchunks: the re-run of the last chunk
-        reward_chunk_kernel<<<nb, bs, 0, st>>>(*cfg, states_dev, idx_begin, n, c, nchunks, horizon,
-                                               discount_dev, buf0, buf1, sums_dev, partial, ctrl);
-        SLB_LAUNCH_CHECK();
-        if (c == nchunks) break;
-        reward_finish_kernel<<<1, FIN_THREADS, 0, st>>>(partial, nb, c, horizon, tol_bits, ctrl, stop_dev);
-        SLB_LAUNCH_CHECK();
-    }
-    return 0;
+    });
 }
 
 }  // extern "C"

@@ -36,7 +36,7 @@ __all__ = ["DimensionError", "GridWorld", "Function", "DeterministicFunction",
            "Triangulation", "TriangulationGradient", "PiecewiseConstant", "NetworkGradient",
            "Kernel", "RBF", "Matern12", "Matern32", "Matern52", "Linear", "Constant", "Bias",
            "White", "Sum", "Add", "Product", "Prod", "kernels", "Likelihood", "GPRCached", "GPR",
-           "GaussianProcess", "FunctionStack",
+           "GaussianProcess", "FunctionStack", "PosteriorMean",
            "InvertedPendulum", "CartPole", "VanDerPol", "LyapunovNetwork", "NeuralNetwork",
            "concatenate_inputs"]
 
@@ -355,6 +355,12 @@ class DeterministicFunction(Function):
 
 class UncertainFunction(Function):
     """``functions.py:202-230``."""
+
+    def to_mean_function(self):
+        """A callable returning only the first output, ``lambda *points: self(*points)[0]``
+        (``functions.py:209-230``); ``GaussianProcess`` and ``FunctionStack`` return a fused
+        ``PosteriorMean`` instead."""
+        return lambda *points: self(*points)[0]
 
 
 class ConstantFunction(DeterministicFunction):
@@ -2689,6 +2695,11 @@ class _GaussianProcessNode(UncertainFunction):
         grad_mean, grad_err = grad_out
         return _gp_vjp(self.gp_stack(), points.detach(), grad_mean, grad_err), []
 
+    def to_mean_function(self):
+        """The posterior mean as a deterministic function (``functions.py:209-230``): a
+        ``PosteriorMean`` on this GP, which the rollouts and the Bellman sweeps fuse as dynamics."""
+        return PosteriorMean(self)
+
 
 class GaussianProcess(_GaussianProcessNode):
     """``(mean, beta * sqrt(var))`` of a one-output GP (``functions.py:461-546``)."""
@@ -2802,3 +2813,75 @@ class FunctionStack(_GaussianProcessNode):
     def add_data_point(self, x, y):
         for fun, yi in zip(self.functions, np.asarray(y).squeeze()):
             fun.add_data_point(x, yi)
+
+
+def _gp_mean(stack, points):
+    """One ``slb_gp_mean`` call: the posterior mean [n, D] (device tensor) at device points."""
+    lib = nat.load()
+    pts = dev.to_device(points).contiguous()
+    if pts.dim() != 2 or pts.shape[1] != stack.input_dim:
+        raise DimensionError("GP expects %d input columns, got %s"
+                             % (stack.input_dim, tuple(pts.shape)))
+    n = pts.shape[0]
+    mean = dev.empty((n, stack.num_outputs))
+    nat.check(lib.slb_gp_mean(dev.stream(), stack, pts.data_ptr() if n else None, n,
+                              mean.data_ptr() if n else None), "slb_gp_mean")
+    return mean
+
+
+class PosteriorMean(DeterministicFunction):
+    """The posterior mean of a ``GaussianProcess`` or ``FunctionStack`` as a deterministic function,
+    ``gp.to_mean_function()`` (``functions.py:209-230``): ``f(x, u)`` or ``f(z)`` returns the numpy
+    mean ``[n, D]``.  ``compute_roa``, ``reward_rollout``, ``compute_trajectory`` and ``PolicyIteration``
+    fuse it as dynamics; ``Lyapunov`` takes it down the composed path (a nominal decrease, no error
+    term).  It has no ``descriptor``: the kernels take it as a GP stack (``gp_stack()``), as dynamics
+    only.
+
+    The mean is ``(sum_j k_j gamma_j + scale m(z)) / scale`` with ``gamma = scale^2 v L^-T alpha``
+    folded per output (``slb_gp_mean``, the form of the Bellman sweep), not the full posterior's
+    ``a^T alpha``: it agrees with ``gp(z)[0]`` within the bound of DESIGN.md §3.16, not bit for bit.
+    It is the same function in every entry point, so a rollout of h steps equals h compositions of
+    one-step evaluations bit for bit.  The GP is held, not copied: ``add_data_point`` on it is
+    picked up (``version`` follows the GP's)."""
+
+    def __init__(self, gaussian_process, name="mean_function"):
+        super().__init__(name)
+        if not isinstance(gaussian_process, _GaussianProcessNode):
+            raise TypeError("PosteriorMean takes a GaussianProcess or FunctionStack")
+        self.gaussian_process = gaussian_process
+        self.input_dim = gaussian_process.input_dim
+        self.output_dim = gaussian_process.output_dim
+
+    def gp_stack(self):
+        return self.gaussian_process.gp_stack()
+
+    @property
+    def version(self):
+        return self.gaussian_process.version
+
+    def __call__(self, *inputs):
+        return self.evaluate_device(concatenate_inputs(inputs)).cpu().numpy()
+
+    def evaluate_device(self, points):
+        return _gp_mean(self.gp_stack(), points)
+
+    def _torch_expression(self, points):
+        """The mean in torch operations on the cached factor (for create_graph=True backwards)."""
+        return self.gaussian_process._torch_expression(points)[0]
+
+    def _vjp(self, points, grad_out, want_in, want_params):
+        if not want_in:
+            return None, []
+        return _gp_vjp(self.gp_stack(), points.detach(), grad_out, None), []
+
+    def jacobian_device(self, points):
+        """[n, D, d_in] from D mean-only VJPs with unit cotangents."""
+        pts = dev.to_device(points).contiguous()
+        stack = self.gp_stack()
+        n, nout = pts.shape[0], stack.num_outputs
+        rows = []
+        for o in range(nout):
+            cot = dev.zeros((n, nout))
+            cot[:, o] = 1.0
+            rows.append(_gp_vjp(stack, pts, cot, None))
+        return torch.stack(rows, dim=1)

@@ -20,7 +20,7 @@ import torch
 
 from . import _device as dev
 from . import _native as nat
-from .functions import Function, FunctionStack, GaussianProcess, UncertainFunction, config
+from .functions import Function, FunctionStack, GaussianProcess, PosteriorMean, UncertainFunction, config
 
 __all__ = ["Lyapunov", "get_safe_sample", "perturb_actions", "smallest_boundary_value",
            "combine_fail_keys", "combine_prefix_stats", "adaptive_as_written"]
@@ -417,11 +417,14 @@ class Lyapunov(object):
 
     # ------------------------------------------------------------------ composed (callable) path
     def _is_composed(self):
-        """True if a member is a plain Python callable, i.e. the sweep cannot be fused."""
+        """True if a member is a plain Python callable, i.e. the sweep cannot be fused.  A GP's
+        ``PosteriorMean`` as the dynamics is composed too: its decrease is nominal (no error term),
+        as the reference computes it for deterministic dynamics, with the mean on the device."""
         def plain(obj):
             return callable(obj) and not isinstance(obj, Function)
         return (plain(self.policy) or plain(self.lyapunov_function)
-                or plain(self._lipschitz_lyapunov) or plain(self.dynamics))
+                or plain(self._lipschitz_lyapunov) or plain(self.dynamics)
+                or isinstance(self.dynamics, PosteriorMean))
 
     def _negative_composed(self, states, tau=None, want_details=False):
         """The graph of ``lyapunov.py:433-441`` on a numpy array of states with the members

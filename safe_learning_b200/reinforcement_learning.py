@@ -16,8 +16,8 @@ import torch
 
 from . import _device as dev
 from . import _native as nat
-from .functions import (Function, FunctionStack, GaussianProcess, PiecewiseConstant, ScaledFunction,
-                        Triangulation, TriangulationGradient, UncertainFunction, _PostOp)
+from .functions import (Function, FunctionStack, GaussianProcess, PiecewiseConstant, PosteriorMean,
+                        ScaledFunction, Triangulation, TriangulationGradient, UncertainFunction, _PostOp)
 
 __all__ = ["PolicyIteration", "OptimizationError"]
 
@@ -173,10 +173,11 @@ class PolicyIteration(object):
             cfg.policy.out_dim = len(action)
             for i, a in enumerate(action):
                 cfg.action[i] = float(a)
-        if isinstance(self.dynamics, (FunctionStack, GaussianProcess)):
-            cfg.gp = self.dynamics.gp_stack()
+        if isinstance(self.dynamics, (FunctionStack, GaussianProcess, PosteriorMean)):
+            cfg.gp = self.dynamics.gp_stack()           # the sweeps use the mean only
         elif isinstance(self.dynamics, UncertainFunction) or not isinstance(self.dynamics, Function):
-            raise TypeError("dynamics must be a fusable Function, GaussianProcess or FunctionStack")
+            raise TypeError("dynamics must be a fusable Function, GaussianProcess, FunctionStack or "
+                            "PosteriorMean")
         else:
             cfg.dynamics = self.dynamics.descriptor()
         cfg.reward = self.reward_function.descriptor()
@@ -338,7 +339,8 @@ class PolicyIteration(object):
         weights = dev.empty((n, ncols))
         stats = dev.zeros((nat.VALUE_STATS,), torch.int64)
         if all(_fusable(f) for f in (self.policy, self.reward_function)) and (
-                isinstance(self.dynamics, (FunctionStack, GaussianProcess)) or _fusable(self.dynamics)):
+                isinstance(self.dynamics, (FunctionStack, GaussianProcess, PosteriorMean))
+                or _fusable(self.dynamics)):
             # every rank assembles and solves the whole system: no collective, identical tables
             rewards = dev.empty((n,))
             nat.check(lib.slb_value_operator(dev.stream(), self.bellman_descriptor(), 0, n,

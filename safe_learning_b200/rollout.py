@@ -5,7 +5,9 @@ against (``examples/utilities.py:654-686`` ``compute_roa``, ``:522-545`` ``rewar
 build as a TF lambda.  When both ``fun`` and ``policy`` are fused function objects (they have
 descriptors) and ``fun`` is deterministic, ``compute_roa`` / ``reward_rollout`` run the whole
 rollout in one CUDA pass per chunk of steps (``csrc/rollout.cu``): one thread per start state,
-the state in registers, start states generated from the grid index.  Any other callable runs the
+the state in registers, start states generated from the grid index.  The posterior mean of a GP
+(``gp.to_mean_function()``, a ``PosteriorMean``) is fused as dynamics too: the rollout kernels
+evaluate it on the Bellman sweep's staged pipeline (DESIGN.md §3.16).  Any other callable runs the
 reference's algorithm on the host, calling it once per step.
 """
 
@@ -17,7 +19,7 @@ import torch
 from . import _device as dev
 from . import _native as nat
 from .functions import (DeterministicFunction, Function, FunctionStack, GaussianProcess, GridWorld,
-                        UncertainFunction, _PostOp, concatenate_inputs)
+                        PosteriorMean, UncertainFunction, _PostOp, concatenate_inputs)
 
 __all__ = ["ClosedLoop", "compute_roa", "reward_rollout"]
 
@@ -51,8 +53,14 @@ class ClosedLoop(DeterministicFunction):
 
     @property
     def fused(self):
-        """Both parts run inside the rollout kernels."""
-        return _fusable(self.fun) and _fusable(self.policy)
+        """Both parts run inside the rollout kernels (a ``PosteriorMean`` as the dynamics only: a
+        closed-loop reward on one is not fused, ``reward_rollout`` checks that)."""
+        return (_fusable(self.fun) or self.gp_mean) and _fusable(self.policy)
+
+    @property
+    def gp_mean(self):
+        """The dynamics are a GP's posterior mean (the rollouts' ``_gp_mean`` entry points)."""
+        return isinstance(self.fun, PosteriorMean)
 
     def __call__(self, *inputs):
         states = concatenate_inputs(inputs)
@@ -88,7 +96,10 @@ def _descriptor(grid_world, d, closed_loop, reward=None):
     else:
         cfg.grid.ndim = d
     cfg.policy = closed_loop.policy.descriptor()
-    cfg.dynamics = closed_loop.fun.descriptor()
+    if closed_loop.gp_mean:
+        cfg.gp = closed_loop.fun.gp_stack()
+    else:
+        cfg.dynamics = closed_loop.fun.descriptor()
     if reward is not None:
         cfg.reward = reward.fun.descriptor()
     return cfg
@@ -127,6 +138,7 @@ def compute_roa(grid, closed_loop_dynamics, horizon=100, tol=1e-3, equilibrium=N
         return roa if no_traj else (roa, traj_host)
     lib = nat.load()
     cfg = _descriptor(grid_world, d, closed_loop_dynamics)
+    entry = "slb_rollout_gp_mean" if closed_loop_dynamics.gp_mean else "slb_rollout"
     src = _source(states, d)
     eq_host = np.ascontiguousarray(eq.ravel())
     h = max(horizon, 0)
@@ -141,11 +153,11 @@ def compute_roa(grid, closed_loop_dynamics, horizon=100, tol=1e-3, equilibrium=N
         cnt = p1 - p0
         need = int(lib.slb_rollout_workspace(cfg, cnt, 0))
         work = dev.empty((need // 8 + 1,)) if need else None
-        nat.check(lib.slb_rollout(dev.stream(), cfg,
-                                  None if src is None else src[p0:p1].data_ptr(), p0, cnt, h,
-                                  eq_host.ctypes.data, float(tol), roa[p0:p1].data_ptr(), None,
-                                  None if no_traj else traj_dev.data_ptr(), dev.ptr(work)),
-                  "slb_rollout")
+        nat.check(getattr(lib, entry)(dev.stream(), cfg,
+                                      None if src is None else src[p0:p1].data_ptr(), p0, cnt, h,
+                                      eq_host.ctypes.data, float(tol), roa[p0:p1].data_ptr(), None,
+                                      None if no_traj else traj_dev.data_ptr(), dev.ptr(work)),
+                  entry)
         if not no_traj:
             torch.from_numpy(traj_host[p0:p1]).copy_(traj_dev[:cnt])
     flags = roa.cpu().numpy().astype(bool)
@@ -188,11 +200,13 @@ def reward_rollout(grid, closed_loop_dynamics, reward_function, discount, horizo
     (``examples/utilities.py:522-545``), with the reference's two messages.
 
     Runs fused on the GPU when both arguments are fused ``ClosedLoop`` objects around the SAME
-    policy object (one policy evaluation per step feeds the reward and the dynamics)."""
+    policy object (one policy evaluation per step feeds the reward and the dynamics); the dynamics
+    may be a ``PosteriorMean``, the reward may not."""
     grid_world, states, n, d = _states_of(grid)
     horizon = int(horizon)
     fused = (isinstance(closed_loop_dynamics, ClosedLoop) and closed_loop_dynamics.fused
              and isinstance(reward_function, ClosedLoop) and reward_function.fused
+             and not reward_function.gp_mean
              and reward_function.policy is closed_loop_dynamics.policy)
     if not fused:
         return _reward_rollout_host(_host_points(grid), n, closed_loop_dynamics, reward_function,
@@ -210,9 +224,10 @@ def reward_rollout(grid, closed_loop_dynamics, reward_function, discount, horizo
     stop = dev.empty((1,), torch.int64)
     need = int(lib.slb_rollout_workspace(cfg, n, 1))
     work = dev.empty((need // 8 + 1,))
-    nat.check(lib.slb_reward_rollout(dev.stream(), cfg, dev.ptr(src), 0, n, horizon,
-                                     table.data_ptr(), float(tol), sums.data_ptr(),
-                                     stop.data_ptr(), work.data_ptr()), "slb_reward_rollout")
+    entry = "slb_reward_rollout_gp_mean" if closed_loop_dynamics.gp_mean else "slb_reward_rollout"
+    nat.check(getattr(lib, entry)(dev.stream(), cfg, dev.ptr(src), 0, n, horizon,
+                                  table.data_ptr(), float(tol), sums.data_ptr(),
+                                  stop.data_ptr(), work.data_ptr()), entry)
     out = sums.cpu().numpy()
     _report(int(stop.item()))
     return out

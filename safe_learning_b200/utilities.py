@@ -1,13 +1,14 @@
 """Host helpers kept from ``safe_learning/utilities.py``: ``batchify`` (``:224-249``, defines the
 reference's batch semantics), ``dlqr`` / ``lqr`` (``:300-356``), and the small array builders the
 callers of the path use: ``combinations`` / ``linearly_spaced_combinations`` (``:252-296``, the
-action set of ``discrete_policy_optimization``) and ``unique_rows`` (``:496-516``)."""
+action set of ``discrete_policy_optimization``), ``unique_rows`` (``:496-516``) and
+``compute_trajectory`` (``:519-583``)."""
 
 import numpy as np
 import scipy.linalg
 
 __all__ = ["batchify", "dlqr", "lqr", "concatenate_inputs", "combinations",
-           "linearly_spaced_combinations", "unique_rows"]
+           "linearly_spaced_combinations", "unique_rows", "compute_trajectory"]
 
 from .functions import concatenate_inputs  # noqa: E402,F401
 
@@ -60,3 +61,35 @@ def unique_rows(array):
     dtype = np.dtype((np.void, array.dtype.itemsize * array.shape[1]))
     _, idx = np.unique(array.view(dtype=dtype), return_index=True)
     return array[idx]
+
+
+def compute_trajectory(dynamics, policy, initial_state, num_steps):
+    """The trajectory of ``x_{t+1} = dynamics(x_t, policy(x_t))`` from one initial state
+    (``utilities.py:519-583``): returns ``states [num_steps, d]`` and ``actions [num_steps - 1, m]``
+    with ``actions[t] = policy(states[t])``, as float64 arrays.
+
+    When dynamics and policy form a fused ``ClosedLoop`` (fusable function objects, the dynamics
+    possibly a GP's ``PosteriorMean``) the states come from one rollout on the GPU and the actions
+    from one batched policy evaluation, bit-identical to the step-by-step loop; any other callables
+    run the reference's loop on the host, one call of each per step."""
+    from .functions import Function, FunctionStack, GaussianProcess
+    from .rollout import ClosedLoop, compute_roa
+
+    initial_state = np.atleast_2d(initial_state)
+    state_dim = initial_state.shape[1]
+    states = np.empty((num_steps, state_dim), dtype=np.float64)
+    actions = np.empty((num_steps - 1, policy.output_dim), dtype=np.float64)
+    states[0, :] = initial_state
+    loop = None
+    if isinstance(dynamics, Function) and not isinstance(dynamics, (GaussianProcess, FunctionStack)):
+        loop = ClosedLoop(dynamics, policy)
+    if loop is not None and loop.fused:
+        if num_steps > 1:
+            _, traj = compute_roa(states[:1], loop, horizon=num_steps, no_traj=False)
+            states[:] = traj[0].T
+            actions[:] = policy.evaluate_device(states[:-1]).cpu().numpy()
+        return states, actions
+    for i in range(num_steps - 1):
+        action = policy(states[[i], :])
+        states[i + 1, :], actions[i, :] = dynamics(states[[i], :], action), action
+    return states, actions
