@@ -190,78 +190,11 @@ SLB_DEV void mean_decision_terms(const slb_sweep& cfg, filter_side& t, double vx
     t.guard = 1e-6 * (fabs(vm[0]) + fabs(vx) + fabs(t.thr) + lvmu) + 4.0 * lverr + 1e-300;
 }
 
-// The screening stage knows the mean only to within dm_j (certified, gp_mean_staged.cuh).  For the
-// function kinds it is enabled for -- V = x^T P x (QUADRATIC, optional scale), L_V constant or a
-// LINEAR map with abs / 1-norm / scale -- the change of the comparison over the box mu +- dm is
-// bounded in closed form:  |V(mu + e) - V(mu)| <= sum_i |((P + P^T) mu)_i| dm_i + sum_ij |P_ij| dm_i
-// dm_j;  |L_V(mu + e)_j - L_V(mu)_j| <= |scale| sum_i |A_ji| dm_i (all rows for the 1-norm), which
-// enters with beta_j sigma_j <= beta_j shi_j.  Returns the amount to add to the guard band.
-SLB_DEV double screening_slack(const slb_sweep& cfg, const double* mu, const double* dm,
-                               const double* shi) {
-    // straight-line for up to 4 outputs (screening_applicable): operands in registers, all matrix
-    // entries loaded at once -- this runs once per grid point in the screening kernel's epilogue
-    constexpr int NS = 4;
-    const int D = cfg.gp.num_outputs;
-    const slb_function& V = cfg.lyapunov;
-    const int n = V.in_dim;
-    double m[NS], d[NS], bs[NS], P[NS][NS];
-#pragma unroll
-    for (int i = 0; i < NS; ++i) {
-        m[i] = i < n ? mu[i] : 0.0;
-        d[i] = i < n ? dm[i] : 0.0;
-        bs[i] = i < D ? fabs(cfg.gp.outputs[i].beta) * shi[i] : 0.0;
-#pragma unroll
-        for (int j = 0; j < NS; ++j) P[i][j] = (i < n && j < n) ? __ldg(V.matrix + i * n + j) : 0.0;
-    }
-    double dv = 0.0;
-#pragma unroll
-    for (int i = 0; i < NS; ++i) {
-        double gi = 0.0;
-#pragma unroll
-        for (int r = 0; r < NS; ++r) gi += m[r] * (P[r][i] + P[i][r]);
-        dv += fabs(gi) * d[i];
-#pragma unroll
-        for (int j = 0; j < NS; ++j) dv += fabs(P[i][j]) * d[i] * d[j];
-    }
-    if (V.flags & SLB_FLAG_SCALE) dv *= fabs(V.out_scale);
-    double dl = 0.0;
-    const slb_function& L = cfg.lipschitz_v;
-    if (L.kind == SLB_FN_LINEAR) {
-        const double sc = (L.flags & SLB_FLAG_SCALE) ? fabs(L.out_scale) : 1.0;
-        const int mi = L.in_dim, mo = L.out_dim;
-        double row[NS];                           // row[o] = sum_i |A_oi| dm_i
-#pragma unroll
-        for (int o = 0; o < NS; ++o) {
-            row[o] = 0.0;
-#pragma unroll
-            for (int i = 0; i < NS; ++i)
-                if (o < mo && i < mi) row[o] += fabs(__ldg(L.matrix + o * mi + i)) * d[i];
-        }
-        if ((L.flags & SLB_FLAG_NORM1) || mo == 1) {
-            dl = sc * (row[0] + row[1] + row[2] + row[3]) * (bs[0] + bs[1] + bs[2] + bs[3]);
-        } else {
-#pragma unroll
-            for (int j = 0; j < NS; ++j) dl += sc * row[j] * bs[j];
-        }
-    }
-    return 1.000001 * (dv + dl);
-}
-
-// the comparison over the box mu +- dm and every sigma_j in [0, shi_j]: fills t's mean-dependent terms
-SLB_DEV int screened_outcome(const slb_sweep& cfg, filter_side& t, double vx, const double* mu,
-                             const double* dm, const double* shi) {
-    double zero[SLB_MAX_OUT];
-    for (int j = 0; j < SLB_MAX_OUT; ++j) zero[j] = 0.0;
-    mean_decision_terms(cfg, t, vx, mu, zero);
-    t.guard += screening_slack(cfg, mu, dm, shi);
-    return decide(t, shi, cfg.gp.num_outputs);
-}
-
-// ---- the same decision in closed form ------------------------------------------------------------------
-// For the sweeps grid_mean_applicable accepts (D outputs, V QUADRATIC, L_V absent or LINEAR): the terms,
-// slack and outcome above with compile-time D and every operand in registers -- the per-point decision of
-// stage 1's grid kernel and of the head stage behind it.  Same arithmetic, same order: the outcomes equal
-// those of the generic functions bit for bit.
+// ---- the decision of a screened list A entry, in closed form ----------------------------------------------
+// The sweeps screening_applicable accepts (D <= 4 outputs, V QUADRATIC, L_V absent or LINEAR on them): the
+// terms and outcome above with compile-time D and every operand in registers -- the per-point decision of
+// both screened stage-1 kernels and of the head stage behind them.  Same arithmetic, same order as
+// mean_decision_terms / decide.
 template <int D>
 struct cf_terms { double dec0, thr, guard, coef[D]; };
 
@@ -286,11 +219,17 @@ SLB_DEV void cf_mean_terms(const slb_sweep& cfg, cf_terms<D>& t, double vx, cons
     t.guard = 1e-6 * (fabs(vm) + fabs(vx) + fabs(t.thr) + lvmu) + 4.0 * lverr + 1e-300;
 }
 
-// screening_slack.  The generic function pads every operand to four lanes with zeros; for D < 4 that turns
-// the slack into NaN whenever a mean or bound is not finite (0 * inf), which `poison` restates.
+// A screened stage knows the mean only to within dm_j (certified, gp_mean_staged.cuh / gp_mean_grid.cuh).
+// For V = x^T P x (QUADRATIC, optional scale) and L_V constant or a LINEAR map with abs / 1-norm / scale
+// (screening_applicable) the change of the comparison over the box mu +- dm is bounded in closed form:
+// |V(mu + e) - V(mu)| <= sum_i |((P + P^T) mu)_i| dm_i + sum_ij |P_ij| dm_i dm_j;  |L_V(mu + e)_j -
+// L_V(mu)_j| <= |scale| sum_i |A_ji| dm_i (all rows for the 1-norm), which enters with beta_j sigma_j <=
+// beta_j shi_j.  Returns the amount to add to the guard band.  The slack is that of the same sums over four
+// lanes, the lanes beyond D zero: for D < 4 a mean, bound or scale that is not finite makes it NaN (0 * inf),
+// which `poison` and `0.0 * sc` restate.
 template <int D>
-SLB_DEV double cf_screening_slack(const slb_sweep& cfg, const double (&mu)[D], const double (&dm)[D],
-                                  const double (&shi)[D]) {
+SLB_DEV double screening_slack(const slb_sweep& cfg, const double (&mu)[D], const double (&dm)[D],
+                               const double (&shi)[D]) {
     const slb_function& V = cfg.lyapunov;
     double poison = 0.0;
     if constexpr (D < 4) {
@@ -356,17 +295,17 @@ SLB_DEV int cf_decide(const cf_terms<D>& t, const double (&shi)[D]) {
     return -1;
 }
 
-// screened_outcome
+// the comparison over the box mu +- dm and every sigma_j in [0, shi_j]
 template <int D>
-SLB_DEV int cf_screened_outcome(const slb_sweep& cfg, double vx, double thr, const double (&mu)[D],
-                                const double (&dm)[D], const double (&shi)[D]) {
+SLB_DEV int screened_outcome(const slb_sweep& cfg, double vx, double thr, const double (&mu)[D],
+                             const double (&dm)[D], const double (&shi)[D]) {
     cf_terms<D> t;
     t.thr = thr;
     double zero[D];
 #pragma unroll
     for (int j = 0; j < D; ++j) zero[j] = 0.0;
     cf_mean_terms<D>(cfg, t, vx, mu, zero);
-    t.guard += cf_screening_slack<D>(cfg, mu, dm, shi);
+    t.guard += screening_slack<D>(cfg, mu, dm, shi);
     return cf_decide<D>(t, shi);
 }
 
@@ -444,37 +383,38 @@ SLB_DEV long long stage1_finish(const filter_args& a, bool valid, int64_t rel, i
     return slot;
 }
 
-// ... from a screened kernel (t: the point's z and threshold), with its mean mu and certified bound dm: the
-// comparison over the box and the prior sigma, the list A entry in the screened layout (the head stage
-// rebuilds the mean-dependent terms), the probe
-template <int DIN>
-SLB_DEV void stage1_screened_finish(const slb_sweep& cfg, const filter_args& a, bool valid, bool sane,
-                                    int64_t rel, filter_side& t, double vx, const double* mu, const double* dm) {
-    const int D = cfg.gp.num_outputs;
+// ... from the fp32 screening kernel (z, thr: the point's input and threshold), with its mean mu and certified
+// bound dm (SLB_MAX_OUT wide, D used): the comparison over the box and the prior sigma, the list A entry in
+// the screened layout (the head stage rebuilds the mean-dependent terms), the probe
+template <int DIN, int D>
+SLB_DEV void stage1_screened_finish(const slb_sweep& cfg, const filter_args& a, bool valid, bool sane, int64_t rel,
+                                    const double* z, double thr, double vx, const double* mu_in,
+                                    const double* dm_in) {
+    double mu[D], dm[D], shi[D];
+#pragma unroll
+    for (int j = 0; j < D; ++j) { mu[j] = mu_in[j]; dm[j] = dm_in[j]; }
     if (a.probe_mu != nullptr && valid) {
+#pragma unroll
         for (int o = 0; o < D; ++o) {
             a.probe_mu[rel * D + o] = mu[o];
             a.probe_dm[rel * D + o] = sane ? dm[o] : f64_inf();
         }
     }
-    double shi[SLB_MAX_OUT];
-    prior_sigma_bound<DIN>(cfg.gp, t.z, shi);
-    const int screened = screened_outcome(cfg, t, vx, mu, dm, shi);
+    cf_prior_sigma<D>(cfg.gp, shi);
+    const int screened = screened_outcome<D>(cfg, vx, thr, mu, dm, shi);
     const long long slot = stage1_finish(a, valid, rel, sane ? screened : -1, vx);
-    bool fp64 = sane;                             // every bound finite: an fp64-class mean
-    for (int j = 0; j < D; ++j) fp64 &= dm[j] < f64_inf();
     if (slot >= 0) {
         filter_side* dst = a.side_a + slot;
         dst->dec0 = vx;
-        dst->thr = t.thr;
+        dst->thr = thr;
 #pragma unroll
-        for (int c = 0; c < DIN; ++c) dst->z[c] = t.z[c];
+        for (int c = 0; c < DIN; ++c) dst->z[c] = z[c];
+#pragma unroll
         for (int j = 0; j < D; ++j) {
             dst->coef[j] = mu[j];
             dst->dm[j] = sane ? dm[j] : f64_inf();
         }
     }
-    if (a.plan.mean_scheme == SLB_MEAN_GRID_FACTORED) count_stat(slot >= 0 && !fp64, a.counts + 2);
 }
 
 template <int DIN>
@@ -519,7 +459,8 @@ filter_mean_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
 // sigma between 0 and the prior's (screening_slack).  The undecided points go to list A with z,
 // threshold and V(x) only; the head stage recomputes their mean in fp64 (warp-cooperatively, on ~8% of
 // the grid at C2), so everything downstream of this kernel is the fp64 arithmetic of the other path.
-template <int DIN>
+// D = the number of outputs (screening_applicable: 1..4): the decision is the closed form.
+template <int DIN, int D>
 __global__ void __launch_bounds__(FT, 7)
 filter_mean32_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -535,13 +476,12 @@ filter_mean32_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a)
     const int64_t rel0 = (int64_t)blockIdx.x * FT + threadIdx.x;
     const bool valid = rel0 < a.n;
     const int64_t rel = valid ? rel0 : a.n - 1;   // every thread stays for the block barriers
-    filter_side t;
-    double vx;
-    bool sane = stage1_point<DIN>(cfg, a.idx_begin + rel, t.z, &vx, &t.thr);
+    double z[SLB_MAX_IN], vx, thr;
+    bool sane = stage1_point<DIN>(cfg, a.idx_begin + rel, z, &vx, &thr);
     // the CTA's centre: the query point of its middle thread
     if (threadIdx.x == FT / 2) {
 #pragma unroll
-        for (int c = 0; c < DIN; ++c) s_cen[c] = t.z[c];
+        for (int c = 0; c < DIN; ++c) s_cen[c] = z[c];
     }
     __syncthreads();                              // centre visible; barriers initialised
     double zcen[DIN];
@@ -549,8 +489,8 @@ filter_mean32_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a)
     for (int c = 0; c < DIN; ++c) zcen[c] = s_cen[c];
 
     double mu[SLB_MAX_OUT], dm[SLB_MAX_OUT];
-    gp_mean32_staged<DIN>(cfg.gp, t.z, zcen, mu, dm, sane, P, B);
-    stage1_screened_finish<DIN>(cfg, a, valid, sane, rel, t, vx, mu, dm);
+    gp_mean32_staged<DIN>(cfg.gp, z, zcen, mu, dm, sane, P, B);
+    stage1_screened_finish<DIN, D>(cfg, a, valid, sane, rel, z, thr, vx, mu, dm);
     timing_mark(a, HEAD_CTAS * 8);
 }
 
@@ -674,7 +614,7 @@ filter_grid_mean_kernel(const __grid_constant__ slb_sweep cfg, const filter_args
         }
     }
     cf_prior_sigma<D>(cfg.gp, shi);
-    const int outcome = sane ? cf_screened_outcome<D>(cfg, vx, thr, mu, dm, shi) : -1;
+    const int outcome = sane ? screened_outcome<D>(cfg, vx, thr, mu, dm, shi) : -1;
     const bool undecided = valid && outcome < 0;
     if (valid) {
         a.negative[rel] = outcome > 0 ? 1 : 0;
@@ -794,8 +734,8 @@ SLB_DEV void head_mean_factor(const double* __restrict__ xf, int Mp, const doubl
 // CTA -- L = 512 / (number of entries) lanes per point, so a CTA with few of them (short lists: the stage's
 // duration is the latency of one group) still spreads the M exps per point and factor over its threads.
 // Results: mu_s / merr_s [slot][SLB_MAX_OUT] in shared memory.  The threads [tid0, tid0 + nthreads) of
-// the CTA (whole warps) take part; `slots` nullptr: the entries are slots 0 .. nneed - 1.
-template <int DIN, int CD>
+// the CTA (whole warps) take part; `slots` nullptr: the entries are slots 0 .. nneed - 1.  D outputs.
+template <int DIN, int D>
 SLB_DEV void head_round_means(const slb_sweep& cfg, const filter_args& a, const int* slots, int nneed,
                               int64_t grp0, int64_t count, const double* mbuf, const double* tab512,
                               double* mu_s, double* merr_s, int tid0, int nthreads) {
@@ -829,22 +769,14 @@ SLB_DEV void head_round_means(const slb_sweep& cfg, const filter_args& a, const 
                 double dot[NO];
                 head_mean_factor<DIN, NO>(xf, Mp, zs, zz, r, L, tab512, dot);
                 if (r == 0 && live) {
-                    const auto finish = [&](int q) {
+#pragma unroll                                     // dot and outs stay in registers
+                    for (int q = 0; q < NO; ++q)
                         mean_output_finish<DIN>(F, cfg.gp.outputs[outs[q]], z, dot[q], zz, 1.0, false,
                                                 &mu_s[slot * SLB_MAX_OUT + outs[q]],
                                                 &merr_s[slot * SLB_MAX_OUT + outs[q]]);
-                    };
-                    if constexpr (CD > 0) {
-#pragma unroll                                     // closed form: dot and outs stay in registers
-                        for (int q = 0; q < NO; ++q) finish(q);
-                    } else {
-#pragma unroll 1                                   // cold, once per entry: one copy of the finish per NO
-                        for (int q = 0; q < NO; ++q) finish(q);
-                    }
                 }
             };
-            if constexpr (CD == 0) for_outputs_on_factor(cfg.gp, f, factor_means);
-            else cf_for_outputs_on_factor<CD>(cfg.gp, f, factor_means);
+            cf_for_outputs_on_factor<D>(cfg.gp, f, factor_means);
         }
     }
 }
@@ -951,7 +883,7 @@ SLB_DEV double head_factor_sdev(const slb_sweep& cfg, const filter_args& a, int 
 }
 
 // the sigma bounds of one group of HP list entries [g HP, g HP + HP) on one warp (lane p: entry p, loaded by
-// head_group_entries), factor after factor; D outputs (CD > 0: the closed form)
+// head_group_entries), factor after factor; D outputs (CD > 0: screened entries, plain RBF factors)
 template <int DIN, bool ALL_STAGED, int CD, int D>
 SLB_DEV void head_group_bound(const slb_sweep& cfg, const filter_args& a, const double* z, bool mine,
                               const double* exptab, double* kw, const double* wbuf, const double* xbuf,
@@ -970,49 +902,19 @@ SLB_DEV void head_group_bound(const slb_sweep& cfg, const filter_args& a, const 
     head_mark(a, HM_BOUND);
 }
 
-// an entry of the factored grid kernel with finite bounds carries an fp64-class mean: the head stage
-// decides it from its box, or sends it to the refine pass, without recomputing the mean
-SLB_DEV bool fp64_class_entry(const filter_args& a, const filter_side& t, int D) {
-    if (a.plan.mean_scheme != SLB_MEAN_GRID_FACTORED) return false;
-    bool finite = true;
-    for (int j = 0; j < D; ++j) finite &= t.dm[j] < f64_inf();
-    return finite;
-}
-
 // The decision of a list entry from what stage 1 left in it and the bound shi of every sigma, the same in
-// both schedules.  A complete entry (fp64 mean stage): the comparison itself.  A screened entry: over the
-// box of its screened mean first -- most are decided by the tighter variance bound alone; `need`: it is
-// still open and has no fp64-class mean, so head_mean_decision follows with vx = V(x).
-SLB_DEV int head_entry_decision(const slb_sweep& cfg, const filter_args& a, filter_side& t, const double* shi,
-                                bool mine, double& vx, bool& need) {
-    const int D = cfg.gp.num_outputs;
+// both schedules.  A complete entry (fp64 mean stage): the comparison itself.
+SLB_DEV int head_entry_decision(const slb_sweep& cfg, const filter_args&, filter_side& t, const double* shi,
+                                bool mine, double&, bool& need) {
     need = false;
-    if (a.plan.mean_scheme == SLB_MEAN_FP64) return mine ? decide(t, shi, D) : 0;
-    double mu[SLB_MAX_OUT], dm[SLB_MAX_OUT];
-    for (int j = 0; j < SLB_MAX_OUT; ++j) { mu[j] = t.coef[j]; dm[j] = t.dm[j]; }
-    vx = t.dec0;
-    const int screened = screened_outcome(cfg, t, vx, mu, dm, shi);
-    const int outcome = mine ? screened : 0;
-    need = mine && outcome < 0 && !fp64_class_entry(a, t, D);
-    head_mark(a, HM_SCREENED);
-    return outcome;
+    return mine ? decide(t, shi, cfg.gp.num_outputs) : 0;
 }
 
-// ... and with the fp64 mean head_round_means left for its slot: the comparison of the fp64 mean stage
-SLB_DEV int head_mean_decision(const slb_sweep& cfg, filter_side& t, double vx, const double* shi,
-                               const double* mu_s, const double* merr_s, int slot) {
-    double mu[SLB_MAX_OUT], merr[SLB_MAX_OUT];
-    for (int j = 0; j < SLB_MAX_OUT; ++j) {
-        mu[j] = mu_s[slot * SLB_MAX_OUT + j];
-        merr[j] = merr_s[slot * SLB_MAX_OUT + j];
-    }
-    mean_decision_terms(cfg, t, vx, mu, merr);
-    return decide(t, shi, cfg.gp.num_outputs);
-}
-
-// The three functions above for the closed form (head stage behind the grid kernel, D outputs): the
-// entry's fields in registers, the decision of stage 1 (cf_screened_outcome).  Only z goes in before the
-// sigma bounds; the other fields are loaded for the decision (fewer registers live across the DMMA chain).
+// A screened entry (D outputs): the entry's fields in registers, the decision of stage 1 (screened_outcome)
+// over the box of its screened mean first -- most are decided by the tighter variance bound alone; `need`:
+// it is still open and has no fp64-class mean, so head_mean_decision follows with vx = V(x).  Only z goes
+// in before the sigma bounds; the other fields are loaded for the decision (fewer registers live across the
+// DMMA chain).
 template <int DIN, int D>
 struct cf_entry { int k; int64_t rel; double vx, thr, z[DIN], mu[D], dm[D]; };   // k: list index, -1: none
 
@@ -1050,9 +952,11 @@ SLB_DEV int head_entry_decision(const slb_sweep& cfg, const filter_args& a, cf_e
         for (int j = 0; j < D; ++j) { t.mu[j] = e->coef[j]; t.dm[j] = e->dm[j]; }
     }
     vx = t.vx;
-    const int screened = cf_screened_outcome<D>(cfg, vx, t.thr, t.mu, t.dm, shi);
+    const int screened = screened_outcome<D>(cfg, vx, t.thr, t.mu, t.dm, shi);
     const int outcome = mine ? screened : 0;
-    bool finite = true;                         // an fp64-class mean (the grid kernel's entries)
+    // an entry of the factored grid kernel with finite bounds carries an fp64-class mean: decided from its
+    // box or sent to the refine pass without recomputing the mean.  An fp32-screened mean is recomputed.
+    bool finite = a.plan.mean_scheme == SLB_MEAN_GRID_FACTORED;
 #pragma unroll
     for (int j = 0; j < D; ++j) finite &= t.dm[j] < f64_inf();
     need = mine && outcome < 0 && !finite;
@@ -1060,6 +964,7 @@ SLB_DEV int head_entry_decision(const slb_sweep& cfg, const filter_args& a, cf_e
     return outcome;
 }
 
+// ... and with the fp64 mean head_round_means left for its slot: the comparison of the fp64 mean stage
 template <int DIN, int D>
 SLB_DEV int head_mean_decision(const slb_sweep& cfg, cf_entry<DIN, D>& t, double vx, const double (&shi)[D],
                                const double* mu_s, const double* merr_s, int slot) {
@@ -1075,7 +980,7 @@ SLB_DEV int head_mean_decision(const slb_sweep& cfg, cf_entry<DIN, D>& t, double
     return cf_decide<D>(terms, shi);
 }
 
-// the grid index of an entry (generic: the one head_group_entries loaded)
+// the grid index of an entry (complete: the one head_group_entries loaded)
 SLB_DEV int64_t entry_rel(const filter_side&, int64_t rel) { return rel; }
 template <int DIN, int D>
 SLB_DEV int64_t entry_rel(const cf_entry<DIN, D>& t, int64_t) { return t.rel; }
@@ -1100,8 +1005,9 @@ SLB_DEV void head_group_finish(const filter_args& a, bool mine, int outcome, int
     }
 }
 
-// CD = 0: every plan.  CD = D > 0: the closed form behind the grid kernel (SLB_MEAN_GRID_FACTORED, D outputs):
-// list entries loaded into registers, the decision of stage 1
+// CD = 0: complete list entries (SLB_MEAN_FP64).  CD = D > 0: screened entries of D outputs (both screened
+// schemes), loaded into registers and decided by the closed form of stage 1, their fp64 means recomputed
+// where the box leaves them open (head_round_means)
 template <int DIN, int CD>
 __global__ void __launch_bounds__(HT, 1)
 filter_head_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
@@ -1123,10 +1029,9 @@ filter_head_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
     double* xbuf = smem + lay.xbuf;
     double* mbuf = smem + lay.mbuf;
     const int nf = cfg.gp.num_factors;
-    const bool screened = lay.mean_scheme != SLB_MEAN_FP64;
-    // fp64 means are recomputed here only for entries without an fp64-class one (all of them after the
-    // fp32 screening kernel, those the grid kernel left with dm = inf: counts[2])
-    const bool means = screened && (lay.mean_scheme != SLB_MEAN_GRID_FACTORED || a.counts[2] != 0);
+    // screened lists: fp64 means are recomputed here only for entries without an fp64-class one (all of them
+    // after the fp32 screening kernel, those the grid kernel left with dm = inf: counts[2])
+    const bool means = CD > 0 && (lay.mean_scheme != SLB_MEAN_GRID_FACTORED || a.counts[2] != 0);
     if (threadIdx.x == 0) {
         for (int b = 0; b < 3; ++b) slb_bulk::mbar_init(bar + b, 1);
         slb_bulk::fence_barrier_init();
@@ -1191,7 +1096,8 @@ filter_head_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
         }
     }
     if (threadIdx.x < 2) s_stat[threadIdx.x] = 0;
-    if (screened && threadIdx.x < 2) reinterpret_cast<int*>(smem + lay.need)[threadIdx.x] = 0;
+    if constexpr (CD > 0)
+        if (threadIdx.x < 2) reinterpret_cast<int*>(smem + lay.need)[threadIdx.x] = 0;
     __syncthreads();
     const int64_t count = (int64_t)a.counts[0];
     const int64_t nwarps = (int64_t)gridDim.x * HW;
@@ -1243,20 +1149,25 @@ filter_head_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
                     if (f == 0) head_mark(a, HM_BOUND0);
                 }
                 head_mark(a, HM_BOUND);
-            } else if (early_means) {
-                slb_bulk::mbar_wait(bar + 0, 0);
-                slb_bulk::mbar_wait(bar + 2, 0);
-                head_round_means<DIN, CD>(cfg, a, nullptr, ngr * HP, grp0, count, mbuf, tab512, mu_s, merr_s,
-                                      nbw * 32, HT - nbw * 32);
-                head_mark(a, HM_MEANS);
+            } else if constexpr (CD > 0) {
+                if (early_means) {
+                    slb_bulk::mbar_wait(bar + 0, 0);
+                    slb_bulk::mbar_wait(bar + 2, 0);
+                    head_round_means<DIN, CD>(cfg, a, nullptr, ngr * HP, grp0, count, mbuf, tab512, mu_s, merr_s,
+                                              nbw * 32, HT - nbw * 32);
+                    head_mark(a, HM_MEANS);
+                }
             }
             __syncthreads();
-            if (means && !early_means) {                  // no warp to spare: the means after the bounds
-                slb_bulk::mbar_wait(bar + 0, 0);
-                slb_bulk::mbar_wait(bar + 2, 0);
-                head_round_means<DIN, CD>(cfg, a, nullptr, ngr * HP, grp0, count, mbuf, tab512, mu_s, merr_s, 0, HT);
-                head_mark(a, HM_MEANS);
-                __syncthreads();
+            if constexpr (CD > 0) {
+                if (means && !early_means) {              // no warp to spare: the means after the bounds
+                    slb_bulk::mbar_wait(bar + 0, 0);
+                    slb_bulk::mbar_wait(bar + 2, 0);
+                    head_round_means<DIN, CD>(cfg, a, nullptr, ngr * HP, grp0, count, mbuf, tab512, mu_s, merr_s, 0,
+                                              HT);
+                    head_mark(a, HM_MEANS);
+                    __syncthreads();
+                }
             }
             if (warp < ngr) {
                 entry_t t;
@@ -1274,7 +1185,8 @@ filter_head_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
                 double vx = 0.0;
                 bool need;
                 int outcome = head_entry_decision(cfg, a, t, shi, mine, vx, need);
-                if (need) outcome = head_mean_decision(cfg, t, vx, shi, mu_s, merr_s, slot);
+                if constexpr (CD > 0)
+                    if (need) outcome = head_mean_decision(cfg, t, vx, shi, mu_s, merr_s, slot);
                 head_mark(a, HM_DECIDED);
                 head_group_finish(a, mine, outcome, entry_rel(t, rel), s_stat);
             }
@@ -1302,7 +1214,7 @@ filter_head_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
                 outcome = head_entry_decision(cfg, a, t, shi, mine, vx, need);
                 if (need) need_s[2 + atomicAdd(need_s + (round & 1), 1)] = warp * HP + lane;
             }
-            if (screened) {
+            if constexpr (CD > 0) {
                 if (threadIdx.x == 0) need_s[(round + 1) & 1] = 0;       // the next round's counter
                 __syncthreads();
                 const int nneed = need_s[round & 1];
@@ -1415,21 +1327,22 @@ filter_plan stage1_plan(const slb_sweep& cfg) {
     return p;
 }
 
-template <int DIN>
+// D = 0: the fp64 mean stage.  D > 0: a screened plan's D outputs (the closed-form kernels)
+template <int DIN, int D>
 int launch_filter(cudaStream_t st, const slb_sweep& cfg, const filter_args& a) {
     static std::atomic<bool> configured[64];
     int device = 0;
     SLB_CUDA(cudaGetDevice(&device));
     if (device < 0 || device >= 64 || !configured[device].load(std::memory_order_acquire)) {
-        SLB_CUDA(cudaFuncSetAttribute(filter_mean_kernel<DIN>,
-                                      cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-        SLB_CUDA(cudaFuncSetAttribute(filter_mean32_kernel<DIN>,
-                                      cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-        SLB_CUDA(cudaFuncSetAttribute(filter_head_kernel<DIN, 0>,
+        if constexpr (D == 0)
+            SLB_CUDA(cudaFuncSetAttribute(filter_mean_kernel<DIN>,
+                                          cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+        else
+            SLB_CUDA(cudaFuncSetAttribute(filter_mean32_kernel<DIN, D>,
+                                          cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+        SLB_CUDA(cudaFuncSetAttribute(filter_head_kernel<DIN, D>,
                                       cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        if constexpr (DIN == 3) {
-            SLB_CUDA(cudaFuncSetAttribute(filter_head_kernel<DIN, GRID_OUTPUTS>,
-                                          cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        if constexpr (DIN == 3 && D == GRID_OUTPUTS) {
             SLB_CUDA(cudaFuncSetAttribute(filter_grid_mean_kernel<GRID_OUTPUTS>,
                                           cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           (int)grid_mean_smem_bytes()));
@@ -1441,13 +1354,12 @@ int launch_filter(cudaStream_t st, const slb_sweep& cfg, const filter_args& a) {
         if (device >= 0 && device < 64) configured[device].store(true, std::memory_order_release);
     }
     const int64_t blocks = (a.n + FT - 1) / FT;
-    // the grid kernel and the head stage behind it run the closed form: d_in = 3 and two outputs
-    const bool closed = a.plan.mean_scheme == SLB_MEAN_GRID_FACTORED;
-    SLB_CHECK(!closed || (DIN == 3 && cfg.gp.num_outputs == GRID_OUTPUTS),
-              "filtered sweep: the factored grid mean needs d_in = 3 and %d outputs", GRID_OUTPUTS);
     switch (a.plan.mean_scheme) {
     case SLB_MEAN_GRID_FACTORED:
-        if constexpr (DIN == 3) {
+        // grid_mean_applicable: d_in = 3 and two outputs
+        SLB_CHECK(DIN == 3 && D == GRID_OUTPUTS, "filtered sweep: the factored grid mean needs d_in = 3 and %d outputs",
+                  GRID_OUTPUTS);
+        if constexpr (DIN == 3 && D == GRID_OUTPUTS) {
             // tiles of GR rows x GC columns over the rows the range touches (it may start and end mid-row)
             const int64_t n1 = cfg.grid.num_points[1];
             const int64_t r0 = a.idx_begin / n1, r1 = (a.idx_begin + a.n - 1) / n1;
@@ -1456,24 +1368,35 @@ int launch_filter(cudaStream_t st, const slb_sweep& cfg, const filter_args& a) {
         }
         break;
     case SLB_MEAN_FP32_SCREENED:
-        filter_mean32_kernel<DIN><<<(unsigned)blocks, FT,
-                                    mean32_smem_bytes(DIN, a.max_outputs_per_factor, a.chunk_rows, FT / 32), st>>>(cfg, a);
+        if constexpr (D > 0)
+            filter_mean32_kernel<DIN, D><<<(unsigned)blocks, FT,
+                                           mean32_smem_bytes(DIN, a.max_outputs_per_factor, a.chunk_rows, FT / 32),
+                                           st>>>(cfg, a);
         break;
     default:
-        filter_mean_kernel<DIN><<<(unsigned)blocks, FT,
-                                  mean_smem_bytes(DIN, a.max_outputs_per_factor, a.chunk_rows), st>>>(cfg, a);
+        if constexpr (D == 0)
+            filter_mean_kernel<DIN><<<(unsigned)blocks, FT,
+                                      mean_smem_bytes(DIN, a.max_outputs_per_factor, a.chunk_rows), st>>>(cfg, a);
     }
     SLB_LAUNCH_CHECK();
     if (!(g_filter_stages & 1)) return 0;
-    const size_t head_smem = (size_t)a.plan.doubles * sizeof(double);
-    if constexpr (DIN == 3) {
-        if (closed) filter_head_kernel<DIN, GRID_OUTPUTS><<<HEAD_CTAS, HT, head_smem, st>>>(cfg, a);
-        else filter_head_kernel<DIN, 0><<<HEAD_CTAS, HT, head_smem, st>>>(cfg, a);
-    } else {
-        filter_head_kernel<DIN, 0><<<HEAD_CTAS, HT, head_smem, st>>>(cfg, a);
-    }
+    filter_head_kernel<DIN, D><<<HEAD_CTAS, HT, (size_t)a.plan.doubles * sizeof(double), st>>>(cfg, a);
     SLB_LAUNCH_CHECK();
     return 0;
+}
+
+// The instantiation of a plan: d_in = d + m (slb_validate_sweep: m >= 1, so d_in >= 2) and, for a screened
+// plan, its D = d outputs (screening_applicable: D <= 4), D = d_in - m with m <= SLB_MAX_ACT = 2
+static_assert(SLB_MAX_ACT == 2, "the screened instantiations cover m = 1, 2");
+int dispatch_filter(cudaStream_t st, const slb_sweep& cfg, const filter_args& a) {
+    return slb_dispatch_dim<2, 6>(cfg.gp.input_dim, "GP input_dim", [&](auto din) {
+        constexpr int DIN = decltype(din)::value;
+        if (a.plan.mean_scheme == SLB_MEAN_FP64) return launch_filter<DIN, 0>(st, cfg, a);
+        constexpr int DLO = DIN - 2 > 1 ? DIN - 2 : 1, DHI = DIN - 1 < 4 ? DIN - 1 : 4;
+        return slb_dispatch_dim<DLO, DHI>(cfg.gp.num_outputs, "screened filter: outputs", [&](auto d) {
+            return launch_filter<DIN, decltype(d)::value>(st, cfg, a);
+        });
+    });
 }
 
 }  // namespace
@@ -1597,9 +1520,7 @@ int slb_lyapunov_sweep_filtered(void* stream, const slb_sweep* cfg, int64_t idx_
         a.n = n; a.idx_begin = idx_begin + off;
         a.negative = negative_dev + off;
         a.values = values_dev ? values_dev + off : nullptr;
-        int rc = slb_dispatch_dim<1, 6>(din, "GP input_dim", [&](auto D) {
-            return launch_filter<D>(st, *cfg, a);
-        });
+        int rc = dispatch_filter(st, *cfg, a);
         if (rc) return rc;
         if (!(g_filter_stages & 2)) continue;
         rc = slb_launch_refine(st, *cfg, n, idx_begin + off, a.list_b, a.counts + 1,

@@ -14,14 +14,16 @@ Coverage (compiled shape or run-time path -> test; every case under the stage-1 
 head schedules, split 3|8 and round loop 3|16):
 
 ===========================================================  =================================================
-filter_grid_mean_kernel<3> (default), filter_mean32_kernel<3>  test_pendulum (M = 500; 0, 1, 8, 64, 65, 200),
-(3|32), filter_mean_kernel<3> (7); filter_head_kernel<3>        test_lv_forms, test_shared_factor_short_scales
+filter_grid_mean_kernel<2> (default), filter_mean32_kernel<3,   test_pendulum (M = 500; 0, 1, 8, 64, 65, 200),
+2> (3|32), filter_mean_kernel<3> (7); filter_head_kernel<3, 2>  test_lv_forms, test_shared_factor_short_scales
+(both screened schemes), filter_head_kernel<3, 0> (fp64)
 stage 1 / head edges D_hi, D_lo (D_lo with c_j < 0)            test_lv_forms["linear"] (LINEAR without abs)
 variance floor (floor_rel in [1.05e-9, 2e-9]), M = 8, 64       test_variance_floor
-filter_mean_kernel<DIN>, filter_mean32_kernel<DIN> (DIN <= 4),  test_input_dimensions (d_in = 2..6)
-filter_head_kernel<DIN>, DIN 2..6
+filter_mean_kernel<DIN>, filter_head_kernel<DIN, 0>, DIN 2..6;  test_input_dimensions (d_in = 2..6 with m = 1;
+filter_mean32_kernel<DIN, D>, filter_head_kernel<DIN, D>,       d_in = 3..6 with m = 2)
+D = DIN - m <= 4, m = 1, 2 (screening_slack at D = 1..4)
 kernel_expr_diag (prior sigma, head kss), Linear / White        test_expressions (d_in = 2..6, fp64 scheme)
-filter_head_kernel<6>, head tables in global memory; empty     test_five_factors, test_empty_factor
+filter_head_kernel<6, 0>, head tables in global memory; empty  test_five_factors, test_empty_factor
 factor
 screening_slack branches: const, abs-linear, 1-norm, scaled,  test_lv_forms
 signed LINEAR, scaled quadratic V
@@ -43,7 +45,7 @@ import gp_posterior_reference as R
 import oracle as O
 import safe_learning_b200 as sl
 from safe_learning_b200 import _native as nat
-from test_gpu_gp_shapes import _workload
+from test_gpu_gp_shapes import FILTER_SHAPES, _workload
 
 pytestmark = pytest.mark.gpu
 
@@ -380,12 +382,12 @@ def test_variance_floor(M):
 DIMS = {1: [1201], 2: [45, 37], 3: [13, 11, 12], 4: [7, 6, 7, 6], 5: [5, 5, 5, 5, 5]}
 
 
-@pytest.mark.parametrize("din", range(2, 7))
-def test_input_dimensions(din):
-    d = din - 1
-    wl = _workload(d, 1, 120, DIMS[d], seed=50 + din, shared=d == 4)
-    schemes = ("grid", "fp32", "fp64") if din == 3 else ("fp32", "fp64") if d <= 4 else ("fp64",)
-    _gp_workload_case("d_in=%d rbf" % din, wl, DIMS[d], schemes, din)
+@pytest.mark.parametrize("din,m", FILTER_SHAPES)
+def test_input_dimensions(din, m):
+    d = din - m
+    wl = _workload(d, m, 120, DIMS[d], seed=50 + din + 10 * (m - 1), shared=d == 4)
+    schemes = ("grid", "fp32", "fp64") if (din, m) == (3, 1) else ("fp32", "fp64") if d <= 4 else ("fp64",)
+    _gp_workload_case("d_in=%d m=%d rbf" % (din, m), wl, DIMS[d], schemes, din)
 
 
 @pytest.mark.parametrize("din", range(2, 7))

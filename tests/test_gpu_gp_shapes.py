@@ -15,8 +15,8 @@ MODE_SWEEP_GRID / MODE_SWEEP_STATES (mean, err, decrease)       test_sweep_grid_
 refine pass, TP = 32 split over G = 1..8 CTAs, FS > 1,          test_refine_pass (slb_debug_refine; DIN 2..6 --
 unsplit 32-point tiles, persistent 64-point tiles               DIN 1 needs m = 0, which a sweep cannot have),
 (> 132 tiles), RBF / expression, 1 / 2 / 5 factors              test_split_plan_covers_every_shape
-filter_mean_kernel / filter_mean32_kernel, DIN 2..6             test_filter_every_input_dimension (both first
-                                                                stages, RBF and expressions)
+filter_mean_kernel<DIN>, DIN 2..6; filter_mean32_kernel<DIN,    test_filter_every_input_dimension (both first
+D> and filter_head_kernel<DIN, D>, D = DIN - m, m = 1, 2         stages, m = 1, 2), RBF and expressions
 filter_head_kernel<6>, head tables in global memory (5 factors) test_filter_five_factors_head_tables_in_global
 stack with an empty factor                                      test_filter_empty_factor
 =============================================================  ================================================
@@ -429,12 +429,18 @@ def _oracle_negative(wl, states, tau):
     return dec < thr
 
 
-@pytest.mark.parametrize("din", range(2, 7))
-def test_filter_every_input_dimension(din, mean_stage):
+# (d_in, m): every d_in with one action, and two actions wherever the fp32 screening kernel then runs (D = d_in - 2
+# outputs, 1..4) -- with the m = 1 cases every (d_in, D) the screened kernels are compiled for
+FILTER_SHAPES = ([pytest.param(din, 1, id=str(din)) for din in range(2, 7)] +
+                 [pytest.param(din, 2, id="%d-m2" % din) for din in range(3, 7)])
+
+
+@pytest.mark.parametrize("din,m", FILTER_SHAPES)
+def test_filter_every_input_dimension(din, m, mean_stage):
     """Plain RBF factors (fp32 screening where D <= 4), with either first stage."""
-    d = din - 1
+    d = din - m
     num = {1: [401], 2: [45, 37], 3: [13, 11, 12], 4: [7, 6, 7, 6], 5: [5, 5, 5, 5, 5]}[d]
-    wl = _workload(d, 1, 120, num, seed=50 + din, shared=d == 4)
+    wl = _workload(d, m, 120, num, seed=50 + din + 10 * (m - 1), shared=d == 4)
     stage = 32 if mean_stage == "fp32 screening" and d <= 4 else 64
     _filter_check(wl, want_stage1=stage)
 

@@ -4,7 +4,8 @@ library.  Stage 1's factored grid kernel (``filter_grid_mean_kernel<2>``) and th
 memory goes to L2 in these kernels: they give almost all of L1 to shared memory).  The grid kernel has no
 stack at all and stays within 128 registers, so that two of its 256-thread CTAs fit on an SM.  The head
 kernel keeps one 8-byte spill slot: a value held across the 72-DMMA chain of its sigma bound at the 128
-registers of a 512-thread CTA (the generic instantiation: a 3.9 KB frame)."""
+registers of a 512-thread CTA.  The head stage of the fp32 screening scheme runs the same closed form at every
+(d_in, D) it is compiled for, within a 64-byte frame (the fp64 scheme's ``filter_head_kernel<DIN, 0>``: 480 B)."""
 import os
 import re
 import shutil
@@ -59,3 +60,15 @@ def test_grid_kernel_has_no_stack_and_fits_two_ctas_per_sm(usage):
 def test_closed_form_head_kernel_keeps_its_entries_in_registers(usage):
     res = _one(usage, r"filter_head_kernelILi3ELi2EE")
     assert res["STACK"] <= 8 and res["LOCAL"] == 0, res
+
+
+def test_screened_head_kernels_keep_their_entries_in_registers(usage):
+    shapes = {}
+    for name, res in usage.items():
+        m = re.search(r"filter_head_kernelILi(\d)ELi([1-9])EE", name)
+        if m:
+            shapes[(int(m.group(1)), int(m.group(2)))] = res
+    # D = d_in - m outputs, m = 1, 2, D <= 4
+    assert sorted(shapes) == [(2, 1), (3, 1), (3, 2), (4, 2), (4, 3), (5, 3), (5, 4), (6, 4)]
+    for shape, res in shapes.items():
+        assert res["STACK"] <= 64 and res["LOCAL"] == 0, (shape, res)
