@@ -439,6 +439,15 @@ int slb_gp_vjp(void* stream, const slb_gp_stack* gp, const double* points_dev, i
 int64_t slb_gp_lml_grad_workspace(int32_t M);
 int slb_gp_lml_grad(void* stream, const double* X_dev, int32_t M, int32_t d_in, const slb_kernel* kern,
                     const double* Kinv_dev, const double* alpha_dev, double* grad_dev, void* workspace_dev);
+/* ---- the same gradient for a GP with k = 1..SLB_MAX_OUT target columns sharing one kernel and noise (gpflow's
+ *      GPR with Y [M, k]): alpha_dev [M, k] row-major = K^-1 (Y - m(X)) and W = sum_c alpha_c alpha_c^T - k K^-1,
+ *      formed per pair as w = -k Kinv_ij, then w = fma(alpha_ic, alpha_jc, w) for c = 0 .. k-1.  Still one pass
+ *      over the lower triangle (each pair's d K / d theta evaluated once) with the same workspace.  k = 1 is
+ *      fma(alpha_i, alpha_j, -Kinv_ij): slb_gp_lml_grad is this call with k = 1, bit for bit.  Host checks
+ *      (before any launch): those of slb_gp_lml_grad and 1 <= k <= SLB_MAX_OUT. */
+int slb_gp_lml_grad_cols(void* stream, const double* X_dev, int32_t M, int32_t d_in, const slb_kernel* kern,
+                         const double* Kinv_dev, const double* alpha_dev, int32_t k, double* grad_dev,
+                         void* workspace_dev);
 
 /* ---- the fused Lyapunov sweep over flat grid indices [idx_begin, idx_end):
  *      index -> x (functions.py:714-731) -> u = policy(x) -> [x,u] -> GP mean / beta*sigma

@@ -202,6 +202,7 @@ SIGNATURES = {
     "slb_gp_vjp": (C.c_int, [_vp, C.POINTER(SlbGpStack), _dp, _i64, _dp, _dp, _dp, _vp]),
     "slb_gp_lml_grad_workspace": (C.c_int64, [_i32]),
     "slb_gp_lml_grad": (C.c_int, [_vp, _dp, _i32, _i32, C.POINTER(SlbKernel), _dp, _dp, _dp, _vp]),
+    "slb_gp_lml_grad_cols": (C.c_int, [_vp, _dp, _i32, _i32, C.POINTER(SlbKernel), _dp, _dp, _i32, _dp, _vp]),
 }
 
 _lib = None

@@ -1,12 +1,17 @@
 // gp_hyper.cu -- gradient of the GP log marginal likelihood with respect to every slot of a covariance
 // expression (slb_kernel), the device half of GPRCached.log_likelihood_and_gradient / optimize (gpflow 0.4.0
-// GPR.build_likelihood).  With K = kern.K(X) + noise I, alpha = K^-1 d and W = alpha alpha^T - K^-1:
+// GPR.build_likelihood).  With K = kern.K(X) + noise I, k target columns D = Y - m(X) [M, k],
+// alpha = K^-1 D [M, k] and W = sum_c alpha_c alpha_c^T - k K^-1:
 //   d LML / d theta = 1/2 sum_ij W_ij d K_ij / d theta,     d LML / d noise = 1/2 tr W.
-// K^-1 and alpha come from the host's Cholesky (torch / cuSOLVER); this file reads K^-1 once.
+// K^-1 and alpha come from the host's Cholesky (torch / cuSOLVER); this file reads K^-1 once, whatever k is.
 //
 // Tile kernel: one CTA per SLB_GP_HYPER_TILE x SLB_GP_HYPER_TILE tile (bi, bj), bi >= bj, of the lower
-// triangle.  Thread t owns column t % HT of the tile and every (HTHREADS / HT)-th row, so a warp reads 32
-// consecutive doubles of a K^-1 row.  Per pair (i >= j) it evaluates every primitive's value and what its
+// triangle.  It stages the k alpha columns of its row and column panels, and per pair forms
+// w = -k Kinv_ij, then w = fma(alpha_ic, alpha_jc, w) for c = 0 .. k-1 in that order.  k = 1 is its own
+// instantiation (COLS = false) with the one-column arithmetic fma(alpha_i, alpha_j, -Kinv_ij) and one
+// staged column: the same value as the loop's (-1 * x is -x), without its runtime trip count.  Thread t owns
+// column t % HT of the tile and every (HTHREADS / HT)-th row, so a warp reads 32 consecutive doubles of a K^-1
+// row.  Per pair (i >= j) it evaluates every primitive's value and what its
 // partials need, forms each primitive's co-factor (the product of the other primitives of its term, by
 // prefix and suffix products: no division, a zero variance is fine), and adds
 //   c_ij * cofactor_p * d k_p / d slot   (c_ij = W_ij off the diagonal, which stands for (i, j) and (j, i);
@@ -95,14 +100,16 @@ SLB_DEV void tile_coords(int64_t t, int& bi, int& bj) {
     bj = (int)(t - (int64_t)b * (b + 1) / 2);
 }
 
-template <int DIN>
+template <int DIN, bool COLS>
 __global__ void __launch_bounds__(HTHREADS, 2)
 gp_lml_grad_tile_kernel(const __grid_constant__ slb_kernel K, const double* __restrict__ X, int M,
-                        const double* __restrict__ Kinv, const double* __restrict__ alpha,
+                        const double* __restrict__ Kinv, const double* __restrict__ alpha, int kcols,
                         double* __restrict__ part) {
     constexpr int S = 1 + DIN;
     constexpr int NP = SLB_MAX_KPRIM;
-    __shared__ double xr[HT * DIN], xc[HT * DIN], ar[HT], ac[HT];
+    constexpr int KMAX = COLS ? SLB_MAX_OUT : 1;
+    const int kc = COLS ? kcols : 1;
+    __shared__ double xr[HT * DIN], xc[HT * DIN], ar[HT * KMAX], ac[HT * KMAX];
     __shared__ double red[HWARPS][NSLOT];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int64_t t = blockIdx.x;
@@ -114,9 +121,10 @@ gp_lml_grad_tile_kernel(const __grid_constant__ slb_kernel K, const double* __re
         xr[e] = r0 + k < M ? X[(int64_t)r0 * DIN + e] : 0.0;
         xc[e] = c0 + k < M ? X[(int64_t)c0 * DIN + e] : 0.0;
     }
-    for (int k = tid; k < HT; k += HTHREADS) {
-        ar[k] = r0 + k < M ? alpha[r0 + k] : 0.0;
-        ac[k] = c0 + k < M ? alpha[c0 + k] : 0.0;
+    for (int e = tid; e < HT * kc; e += HTHREADS) {       // alpha is [M, kc] row-major
+        const int k = e / kc;
+        ar[e] = r0 + k < M ? alpha[(int64_t)r0 * kc + e] : 0.0;
+        ac[e] = c0 + k < M ? alpha[(int64_t)c0 * kc + e] : 0.0;
     }
     __syncthreads();
 
@@ -134,7 +142,13 @@ gp_lml_grad_tile_kernel(const __grid_constant__ slb_kernel K, const double* __re
         const int i = r0 + ii;
         if (i >= M || j >= M || j > i) continue;          // j > i only in a diagonal tile
         const bool diag = i == j;
-        const double wij = fma(ar[ii], ac[jj], -__ldg(Kinv + (int64_t)i * M + j));
+        double wij;
+        if constexpr (COLS) {
+            wij = -(double)kc * __ldg(Kinv + (int64_t)i * M + j);
+            for (int c = 0; c < kc; ++c) wij = fma(ar[ii * kc + c], ac[jj * kc + c], wij);
+        } else {
+            wij = fma(ar[ii], ac[jj], -__ldg(Kinv + (int64_t)i * M + j));
+        }
         const double cij = diag ? 0.5 * wij : wij;
         if (diag) accn += cij;
         double x[DIN];
@@ -233,10 +247,13 @@ int64_t tile_count(int32_t M) {
 
 template <int DIN>
 int launch_lml_grad(cudaStream_t st, const double* X, int M, const slb_kernel& K, const double* Kinv,
-                    const double* alpha, double* grad, double* part) {
+                    const double* alpha, int kc, double* grad, double* part) {
     const int64_t tiles = tile_count(M);
     SLB_CHECK(tiles <= 0x7fffffff, "slb_gp_lml_grad: M = %d needs too many tiles for one launch", M);
-    gp_lml_grad_tile_kernel<DIN><<<(unsigned)tiles, HTHREADS, 0, st>>>(K, X, M, Kinv, alpha, part);
+    if (kc == 1)
+        gp_lml_grad_tile_kernel<DIN, false><<<(unsigned)tiles, HTHREADS, 0, st>>>(K, X, M, Kinv, alpha, 1, part);
+    else
+        gp_lml_grad_tile_kernel<DIN, true><<<(unsigned)tiles, HTHREADS, 0, st>>>(K, X, M, Kinv, alpha, kc, part);
     SLB_LAUNCH_CHECK();
     gp_lml_grad_sum_kernel<<<NSLOT, RT, 0, st>>>(part, tiles, grad);
     SLB_LAUNCH_CHECK();
@@ -253,12 +270,13 @@ extern "C" int64_t slb_gp_lml_grad_workspace(int32_t M) {
     return tile_count(M) * NSLOT * (int64_t)sizeof(double);
 }
 
-extern "C" int slb_gp_lml_grad(void* stream, const double* X_dev, int32_t M, int32_t d_in, const slb_kernel* kern,
-                               const double* Kinv_dev, const double* alpha_dev, double* grad_dev,
-                               void* workspace_dev) {
-    const char* who = "slb_gp_lml_grad";
+namespace {
+
+int lml_grad(const char* who, void* stream, const double* X_dev, int32_t M, int32_t d_in, const slb_kernel* kern,
+             const double* Kinv_dev, const double* alpha_dev, int32_t k, double* grad_dev, void* workspace_dev) {
     SLB_CHECK(M >= 0, "%s: negative M (%d)", who, M);
     SLB_CHECK(d_in >= 1 && d_in <= SLB_MAX_IN, "%s: d_in %d outside 1..%d", who, d_in, SLB_MAX_IN);
+    SLB_CHECK(k >= 1 && k <= SLB_MAX_OUT, "%s: %d target columns outside 1..%d", who, k, SLB_MAX_OUT);
     SLB_CHECK(kern != nullptr, "%s: null kernel descriptor", who);
     if (slb_validate_kernel(*kern, d_in, who)) return 1;
     SLB_CHECK(kern->num_prims >= 1,
@@ -272,7 +290,23 @@ extern "C" int slb_gp_lml_grad(void* stream, const double* X_dev, int32_t M, int
     SLB_CHECK(X_dev != nullptr && Kinv_dev != nullptr && alpha_dev != nullptr && grad_dev != nullptr &&
               workspace_dev != nullptr, "%s: null X, Kinv, alpha, grad or workspace with M = %d", who, M);
     return slb_dispatch_dim<1, 6>(d_in, "slb_gp_lml_grad: d_in", [&](auto DIN) {
-        return launch_lml_grad<DIN>((cudaStream_t)stream, X_dev, M, *kern, Kinv_dev, alpha_dev, grad_dev,
+        return launch_lml_grad<DIN>((cudaStream_t)stream, X_dev, M, *kern, Kinv_dev, alpha_dev, k, grad_dev,
                                     static_cast<double*>(workspace_dev));
     });
+}
+
+}  // namespace
+
+extern "C" int slb_gp_lml_grad_cols(void* stream, const double* X_dev, int32_t M, int32_t d_in,
+                                    const slb_kernel* kern, const double* Kinv_dev, const double* alpha_dev,
+                                    int32_t k, double* grad_dev, void* workspace_dev) {
+    return lml_grad("slb_gp_lml_grad_cols", stream, X_dev, M, d_in, kern, Kinv_dev, alpha_dev, k, grad_dev,
+                    workspace_dev);
+}
+
+extern "C" int slb_gp_lml_grad(void* stream, const double* X_dev, int32_t M, int32_t d_in, const slb_kernel* kern,
+                               const double* Kinv_dev, const double* alpha_dev, double* grad_dev,
+                               void* workspace_dev) {
+    return lml_grad("slb_gp_lml_grad", stream, X_dev, M, d_in, kern, Kinv_dev, alpha_dev, 1, grad_dev,
+                    workspace_dev);
 }

@@ -1997,21 +1997,27 @@ class GPRCached(object):
     it into the fragment order the sweep kernel streams (``slb_pack_factor``), and
     ``alpha = L^-1 scale (Y - m(X))``.  GPs that share X, kernel, noise and scale share one
     factor (the stacked GPs of a ``FunctionStack`` often do).
+
+    ``Y`` may have k = 1..``SLB_MAX_OUT`` columns (gpflow's ``GPR`` with several targets): one kernel and
+    noise for all of them, hence one factor; each column has its own ``alpha`` / ``gamma`` tables, stored
+    as one 2-D device tensor per kind with a row per column (a 1-D tensor for k = 1).  A ``LinearSystem``
+    prior mean then has k rows, row c being column c's prior mean.
     """
 
     def __init__(self, x, y, kern, mean_function=None, scale=1., name="GPRCached",
                  noise_variance=1.0):
         self.name = name
         self._X = np.atleast_2d(np.asarray(x, dtype=np.float64))
-        self._Y = np.atleast_2d(np.asarray(y, dtype=np.float64))
-        if self._Y.shape[1] != 1:
-            raise DimensionError("one-output GPs only; stack them with FunctionStack")
+        self._Y = self._checked_targets(y, self._X.shape[0])
         if not isinstance(kern, Kernel):
             raise TypeError("kern must be built from safe_learning_b200 kernels (RBF, Matern12/32/52, "
                             "Linear, Constant, White and their sums / products), got %r"
                             % type(kern).__name__)
         if mean_function is not None and not isinstance(mean_function, LinearSystem):
-            raise NotImplementedError("prior mean must be None or a one-row LinearSystem")
+            raise NotImplementedError("prior mean must be None or a LinearSystem with one row per output")
+        if mean_function is not None and mean_function.output_dim != self._Y.shape[1]:
+            raise DimensionError("the prior mean has %d rows for %d target columns: row c is column c's "
+                                 "prior mean" % (mean_function.output_dim, self._Y.shape[1]))
         if self._X.shape[1] > nat.SLB_MAX_IN:
             raise DimensionError("GP input dimension above %d" % nat.SLB_MAX_IN)
         self.kern = kern
@@ -2022,11 +2028,27 @@ class GPRCached(object):
         self._alpha_dev = None
         self._gamma_dev = None
         self._gamma_f_dev = None
-        self._gamma_l1 = 0.0
+        self._gamma_l1_cols = [0.0]
         self._prior_dev = None
         self._stale = True
         self._version = 0
         self._hyper_seen = None
+
+    @staticmethod
+    def _checked_targets(y, rows):
+        """``y`` as a float64 [rows, k] array, 1 <= k <= SLB_MAX_OUT (a 1-D ``y`` is one row)."""
+        y = np.atleast_2d(np.asarray(y, dtype=np.float64))
+        if y.ndim != 2 or y.shape[0] != rows:
+            raise DimensionError("Y has shape %s but X has %d rows: one target row per input row"
+                                 % (y.shape, rows))
+        if not 1 <= y.shape[1] <= nat.SLB_MAX_OUT:
+            raise DimensionError("Y has %d columns; a GP has 1..%d outputs" % (y.shape[1], nat.SLB_MAX_OUT))
+        return y
+
+    @property
+    def output_dim(self):
+        """k, the number of target columns."""
+        return self._Y.shape[1]
 
     # data ------------------------------------------------------------------------------
     @property
@@ -2054,8 +2076,9 @@ class GPRCached(object):
 
     @property
     def alpha(self):
+        """``L^-1 scale (Y - m(X))``, [M, k]."""
         self._ensure()
-        return self._alpha_dev[:self._X.shape[0]].cpu().numpy()[:, None]
+        return self._alpha_dev.reshape(self.output_dim, -1)[:, :self._X.shape[0]].T.cpu().numpy()
 
     # factorisation -----------------------------------------------------------------------
     def _factor_key(self):
@@ -2269,8 +2292,13 @@ class GPRCached(object):
             self._finish_cache(fac)
 
     def _finish_cache(self, fac):
-        """alpha / gamma / prior mean for this GP's targets on factor `fac` (functions.py:405-409)."""
-        M = fac.M
+        """alpha / gamma / prior mean for this GP's targets on factor `fac` (functions.py:405-409).
+
+        Each kind of table is one device tensor with a row per target column, every row zero padded
+        to a multiple of 8 doubles (16-byte aligned, as the filter's bulk copies need); for k = 1 it is
+        the 1-D row itself.  Column c is solved on its own, ``L^-1 t_c``, so that it is the same bits
+        as a one-column GP's table on the same factor."""
+        M, k = fac.M, self.output_dim
         self._factor = fac
         target = dev.to_device(self._Y)
         if self.mean_function is not None:
@@ -2280,21 +2308,24 @@ class GPRCached(object):
         else:
             self._prior_dev = None
         target = self._scale * target
-        alpha = fac.Linv @ target
-        gamma = fac.Linv.T @ alpha
-        padded = dev.zeros((max(8 * fac.nrb, 8),))
-        padded[:M] = alpha[:, 0]
-        self._alpha_dev = padded
-        self._gamma_dev = gamma[:, 0].contiguous() if M else dev.zeros((1,))
         # the filter's mean weights: scale^2 gamma, times the RBF variance on the plain path
         # (whose kernel values are then <= 1), zero padded to the row count of Xf; and the bound
         # sum_i (|L^-1|^T |alpha|)_i of everything that rounds when the mean is summed
         fold = self._scale ** 2 * (float(self.kern.variance) if fac.plain else 1.0)
-        self._gamma_f_dev = dev.zeros((fac.Xf.shape[0],))
-        self._gamma_l1 = 0.0
-        if M:
-            self._gamma_f_dev[:M] = fold * gamma[:, 0]
-            self._gamma_l1 = abs(fold) * float((fac.Linv.abs().T @ alpha.abs()).sum().item())
+        alpha_t = dev.zeros((k, max(8 * fac.nrb, 8)))
+        gamma_t = dev.zeros((k, max(M, 1) if k == 1 else max(8 * fac.nrb, 8)))
+        gamma_f_t = dev.zeros((k, fac.Xf.shape[0]))
+        self._gamma_l1_cols = [0.0] * k
+        for c in range(k):
+            alpha = fac.Linv @ target[:, c:c + 1].contiguous()
+            gamma = fac.Linv.T @ alpha
+            alpha_t[c, :M] = alpha[:, 0]
+            if M:
+                gamma_t[c, :M] = gamma[:, 0]
+                gamma_f_t[c, :M] = fold * gamma[:, 0]
+                self._gamma_l1_cols[c] = abs(fold) * float((fac.Linv.abs().T @ alpha.abs()).sum().item())
+        one = (lambda t: t[0]) if k == 1 else (lambda t: t)
+        self._alpha_dev, self._gamma_dev, self._gamma_f_dev = one(alpha_t), one(gamma_t), one(gamma_f_t)
         self._stale = False
         self._hyper_seen = self._hyper_state()
         self._version += 1
@@ -2303,9 +2334,10 @@ class GPRCached(object):
     def torch_predict(self, points):
         """``build_predict`` (``functions.py:417-458``) on a device tensor [n, d_in] in torch
         operations (cuBLAS / cuSOLVER on the cached factor), differentiable with respect to
-        ``points``: latent mean and variance, [n, 1] each."""
+        ``points``: latent mean and variance, [n, k] each (the one variance tiled over the k columns,
+        like the reference's ``tf.tile``)."""
         self._ensure()
-        fac, s = self._factor, self._scale
+        fac, s, k = self._factor, self._scale, self.output_dim
         s2 = s * s
         mx = 0.0
         if self.mean_function is not None:
@@ -2313,14 +2345,14 @@ class GPRCached(object):
             mx = s * (points @ self.mean_function._matrix_dev.T)               # :439
         kss = s2 * self.kern.Kdiag_device(points)                                # :450
         if fac.M == 0:
-            return mx / s + 0.0 * points[:, :1], (kss / s2).unsqueeze(1)
+            return (mx / s + 0.0 * points[:, :1]).expand(-1, k), (kss / s2).unsqueeze(1).expand(-1, k)
         x_train = dev.to_device(self._X)
         kx = s2 * self.kern.K_device(x_train, points)                            # :438  [M, n]
         a = torch.linalg.solve_triangular(fac.L, kx, upper=False)                # :441
-        alpha = self._alpha_dev[:fac.M].unsqueeze(1)
+        alpha = self._alpha_dev.reshape(k, -1)[:, :fac.M].T
         fmean = (a.T @ alpha + mx) / s                                           # :442, :455
         fvar = (kss - (a * a).sum(dim=0)) / s2                                   # :451, :456
-        return fmean, fvar.unsqueeze(1)
+        return fmean, fvar.unsqueeze(1).expand(-1, k)
 
     # descriptor pieces -------------------------------------------------------------------
     def fill_factor(self, f):
@@ -2342,13 +2374,17 @@ class GPRCached(object):
             self.kern.fill(f.kernel, self._X.shape[1])
         return fac.key
 
-    def fill_output(self, o, factor_index, beta):
+    def fill_output(self, o, factor_index, beta, column=0):
+        """Output slot ``o`` for target column ``column``: row ``column`` of every per-column table."""
         self._ensure()
+
+        def row(t):
+            return t.data_ptr() + 8 * column * t.shape[-1]
         o.factor, o.beta = factor_index, float(beta)
-        o.alpha = self._alpha_dev.data_ptr()
-        o.gamma = self._gamma_dev.data_ptr()
-        o.prior_mean = None if self._prior_dev is None else self._prior_dev.data_ptr()
-        o.gamma_f, o.gamma_l1 = self._gamma_f_dev.data_ptr(), self._gamma_l1
+        o.alpha = row(self._alpha_dev)
+        o.gamma = row(self._gamma_dev)
+        o.prior_mean = None if self._prior_dev is None else row(self._prior_dev.view(self.output_dim, -1))
+        o.gamma_f, o.gamma_l1 = row(self._gamma_f_dev), self._gamma_l1_cols[column]
 
     # hyper-parameters and the log marginal likelihood (gpflow 0.4.0 GPR.build_likelihood) ------------
     def _hyper_params(self):
@@ -2375,16 +2411,19 @@ class GPRCached(object):
         """LML and, if ``want_grad``, its gradient in ``slb_gp_lml_grad``'s descriptor slots.  Its own
         factorisation of ``K + noise I`` (torch / cuSOLVER): the cached posterior factor and the filter
         tables are not touched.  A matrix that is not positive definite raises
-        ``torch.linalg.LinAlgError``."""
+        ``torch.linalg.LinAlgError``.  With k target columns the LML is the sum of the columns' log
+        densities under the one kernel and noise (gpflow's ``GPR``), and the gradient is one fused pass
+        (``slb_gp_lml_grad_cols``)."""
         lib = nat.load()
         M, din = self._X.shape
+        k = self.output_dim
         kstruct = nat.SlbKernel()
         self.kern.fill(kstruct, din)
         slots = np.zeros(nat.SLB_GP_HYPER_SLOTS)
         if M == 0:
             if want_grad:           # the descriptor checks still run; nothing is launched
-                nat.check(lib.slb_gp_lml_grad(None, None, 0, din, kstruct, None, None, None, None),
-                          "slb_gp_lml_grad")
+                nat.check(lib.slb_gp_lml_grad_cols(None, None, 0, din, kstruct, None, None, k, None, None),
+                          "slb_gp_lml_grad_cols")
             return 0.0, slots
         X = dev.to_device(self._X)
         K = self.kern.K_device(X) + torch.eye(M, dtype=torch.float64, device=X.device) * self.likelihood.variance
@@ -2393,15 +2432,15 @@ class GPRCached(object):
         if self.mean_function is not None:
             d = d - self.mean_function.evaluate_device(self._X)
         a = torch.linalg.solve_triangular(L, d, upper=False)
-        lml = -0.5 * M * np.log(2 * np.pi) - torch.log(torch.diagonal(L)).sum() - 0.5 * (a * a).sum()
+        lml = -0.5 * k * M * np.log(2 * np.pi) - k * torch.log(torch.diagonal(L)).sum() - 0.5 * (a * a).sum()
         if want_grad:
-            alpha = torch.cholesky_solve(d, L)[:, 0].contiguous()
+            alpha = torch.cholesky_solve(d, L).contiguous()                     # [M, k] row-major
             kinv = torch.cholesky_inverse(L).contiguous()
             work = dev.empty((int(lib.slb_gp_lml_grad_workspace(M)) // 8,))
             grad = dev.empty((nat.SLB_GP_HYPER_SLOTS,))
-            nat.check(lib.slb_gp_lml_grad(dev.stream(), X.data_ptr(), M, din, kstruct, kinv.data_ptr(),
-                                          alpha.data_ptr(), grad.data_ptr(), work.data_ptr()),
-                      "slb_gp_lml_grad")
+            nat.check(lib.slb_gp_lml_grad_cols(dev.stream(), X.data_ptr(), M, din, kstruct, kinv.data_ptr(),
+                                               alpha.data_ptr(), k, grad.data_ptr(), work.data_ptr()),
+                      "slb_gp_lml_grad_cols")
             slots = grad.cpu().numpy()
         return float(lml.item()), slots
 
@@ -2605,14 +2644,17 @@ class PackedCache(object):
 
 
 def _build_stack(gps, betas):
-    """slb_gp_stack for a list of GPRCached models (factor sharing by key)."""
+    """slb_gp_stack for a list of GPRCached models (factor sharing by key): a GP with k target columns
+    takes k consecutive outputs on its one factor, all with its beta."""
     stack = nat.SlbGpStack()
-    if len(gps) > nat.SLB_MAX_OUT:
-        raise DimensionError("at most %d stacked GPs" % nat.SLB_MAX_OUT)
-    stack.num_outputs = len(gps)
+    total = sum(gp.output_dim for gp in gps)
+    if total > nat.SLB_MAX_OUT:
+        raise DimensionError("at most %d stacked GP outputs, got %d" % (nat.SLB_MAX_OUT, total))
+    stack.num_outputs = total
     stack.input_dim = gps[0].X.shape[1]
     keys = []
-    for o, (gp, beta) in enumerate(zip(gps, betas)):
+    o = 0
+    for gp, beta in zip(gps, betas):
         if gp.X.shape[1] != stack.input_dim:
             raise DimensionError("stacked GPs must share the input dimension")
         gp._ensure()
@@ -2620,7 +2662,9 @@ def _build_stack(gps, betas):
         if key not in keys:
             gp.fill_factor(stack.factors[len(keys)])
             keys.append(key)
-        gp.fill_output(stack.outputs[o], keys.index(key), beta)
+        for c in range(gp.output_dim):
+            gp.fill_output(stack.outputs[o], keys.index(key), beta, c)
+            o += 1
     stack.num_factors = len(keys)
     return stack
 
@@ -2702,7 +2746,8 @@ class _GaussianProcessNode(UncertainFunction):
 
 
 class GaussianProcess(_GaussianProcessNode):
-    """``(mean, beta * sqrt(var))`` of a one-output GP (``functions.py:461-546``)."""
+    """``(mean, beta * sqrt(var))`` of a GP (``functions.py:461-546``), [n, k] each for a model with k
+    target columns (the one sigma in every column)."""
 
     def __init__(self, gaussian_process, beta=2., name="gaussian_process"):
         super().__init__(name)
@@ -2759,7 +2804,8 @@ class GaussianProcess(_GaussianProcessNode):
 
 
 class FunctionStack(_GaussianProcessNode):
-    """Stack of one-output GPs, one per state dimension (``functions.py:254-307``)."""
+    """Stack of GPs, their outputs side by side (``functions.py:254-307``); a member with k target
+    columns contributes k outputs."""
 
     def __init__(self, functions, name="function_stack"):
         super().__init__(name)
@@ -2811,8 +2857,20 @@ class FunctionStack(_GaussianProcessNode):
         return self.functions
 
     def add_data_point(self, x, y):
-        for fun, yi in zip(self.functions, np.asarray(y).squeeze()):
-            fun.add_data_point(x, yi)
+        """Append observations to every member: ``y`` holds the stack's outputs side by side, and each
+        member takes its ``output_dim`` columns."""
+        if all(f.output_dim == 1 for f in self.functions):
+            for fun, yi in zip(self.functions, np.asarray(y).squeeze()):
+                fun.add_data_point(x, yi)
+            return
+        y = np.asarray(y, dtype=np.float64)
+        y = y.reshape(-1, self.output_dim) if y.ndim < 2 else y
+        if y.shape[1] != self.output_dim:
+            raise DimensionError("y has %d columns, the stack has %d outputs" % (y.shape[1], self.output_dim))
+        start = 0
+        for fun in self.functions:
+            fun.add_data_point(x, y[:, start:start + fun.output_dim])
+            start += fun.output_dim
 
 
 def _gp_mean(stack, points):
