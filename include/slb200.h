@@ -500,6 +500,15 @@ int slb_filter_mean_scheme(const slb_sweep* cfg);
 int slb_lyapunov_sweep_filtered(void* stream, const slb_sweep* cfg, int64_t idx_begin,
                                 int64_t idx_end, uint8_t* negative_dev, double* values_dev,
                                 void* workspace_dev, int64_t* stats_dev);
+/* one step of update_safe_set on a single process: the filtered sweep of [idx_begin, idx_end) (arguments
+ * as slb_lyapunov_sweep_filtered, its flags into negative_dev) whose decision kernels fold the first-fail
+ * key as they decide each point, then the prefix rule on that key -- what slb_first_fail followed by
+ * slb_apply_prefix compute on the sweep's flags, with the same key_dev, safe_dev and prefix_stats_dev.
+ * values_dev [n]: V over the range (read only); initial_dev may be NULL. */
+int slb_safe_set_step(void* stream, const slb_sweep* cfg, int64_t idx_begin, int64_t idx_end,
+                      uint8_t* negative_dev, const double* values_dev, const uint8_t* initial_dev,
+                      void* workspace_dev, int64_t* stats_dev, slb_fail_key* key_dev, uint8_t* safe_dev,
+                      slb_prefix_stats* prefix_stats_dev);
 /* diagnostics: the refine pass of slb_lyapunov_sweep_filtered alone, on a caller's point list:
  * list_dev [*count_dev] (device) holds indices relative to idx_begin, each in [0, n_max), and
  * 0 <= n_max <= the pass length of slb_filter_workspace.  Both tile-size launches, the row / factor

@@ -157,6 +157,8 @@ SIGNATURES = {
     "slb_debug_filter_lists": (C.c_int, [_i64, C.POINTER(C.c_int64)]),
     "slb_lyapunov_sweep_filtered": (C.c_int, [_vp, C.POINTER(SlbSweep), _i64, _i64, _dp, _dp, _vp,
                                               _vp]),
+    "slb_safe_set_step": (C.c_int, [_vp, C.POINTER(SlbSweep), _i64, _i64, _dp, _dp, _dp, _vp, _vp, _vp,
+                                    _dp, _vp]),
     "slb_debug_refine": (C.c_int, [_vp, C.POINTER(SlbSweep), _i64, _i64, _vp, _vp, _vp, _dp, _dp, _dp,
                                    _vp]),
     "slb_first_fail_workspace": (C.c_int64, [_i64]),

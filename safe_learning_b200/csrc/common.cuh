@@ -90,6 +90,83 @@ SLB_DEV double key_value(uint64_t k) {
     return __longlong_as_double((long long)b);
 }
 
+// ---- first-fail key folded where the flags are decided (filter.cu, gp_tile.cuh; read by light.cu)
+// The key of a sweep is the lexicographic minimum of (value_key(V), flat index) over the points that are
+// neither negative nor initial, n_ok the number of those that are.  The decision kernels fold every point
+// when its flag becomes final, so the record holds the key once the last of them has finished.  It is
+// stored complemented -- hi = ~value_key, lo = INT64_MAX - index -- so that a zeroed record is the
+// identity (no failing point) and the minimum is a 128-bit maximum.  Minimum and sum do not depend on
+// the order of the updates: the result is exact and deterministic.
+struct __align__(16) slb_fold {
+    unsigned long long lo, hi;         // complemented key (see above)
+    unsigned long long n_ok;
+    unsigned int ticket;               // apply_prefix_kernel: blocks that have added their statistics
+    unsigned int _pad;
+    unsigned long long acc[4];         // apply_prefix_kernel: slb_prefix_stats accumulated over its blocks
+};
+// What a sweep folds into: V of the range (the values the prefix rule orders by), the initial safe set
+// (may be null) and the record; all indexed relative to the pass like the flags.  rec == nullptr: no fold.
+struct slb_fold_target {
+    const double* values;
+    const uint8_t* initial;
+    slb_fold* rec;
+};
+
+SLB_DEV unsigned long long atom_cas128(slb_fold* p, unsigned long long lo, unsigned long long hi,
+                                       unsigned long long new_lo, unsigned long long new_hi,
+                                       unsigned long long* got_hi) {
+    unsigned long long got_lo;
+    asm volatile("{\n\t.reg .b128 d, c, s;\n\t"
+                 "mov.b128 c, {%2, %3};\n\t"
+                 "mov.b128 s, {%4, %5};\n\t"
+                 "atom.global.cas.b128 d, [%6], c, s;\n\t"
+                 "mov.b128 {%0, %1}, d;\n\t}"
+                 : "=l"(got_lo), "=l"(*got_hi)
+                 : "l"(lo), "l"(hi), "l"(new_lo), "l"(new_hi), "l"(p)
+                 : "memory");
+    return got_lo;
+}
+
+// (kv, ki) into the record: 128-bit maximum of the complemented key.  hi only grows, so a key whose hi
+// is below the one already there cannot win and costs one load, not an atomic.
+SLB_DEV void fold_key(slb_fold* rec, uint64_t kv, int64_t ki) {
+    const unsigned long long hi = ~kv, lo = (unsigned long long)(INT64_MAX - ki);
+    unsigned long long cur_hi;
+    asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(cur_hi) : "l"(&rec->hi) : "memory");
+    if (hi < cur_hi) return;
+    unsigned long long cur_lo = 0;
+    while (hi > cur_hi || (hi == cur_hi && lo > cur_lo)) {
+        unsigned long long got_hi;
+        const unsigned long long got_lo = atom_cas128(rec, cur_lo, cur_hi, lo, hi, &got_hi);
+        if (got_lo == cur_lo && got_hi == cur_hi) return;
+        cur_lo = got_lo;
+        cur_hi = got_hi;
+    }
+}
+
+// A warp's points whose flags are final (warp-collective: all 32 lanes call it).  `mine`: the lane holds
+// such a point, `negative` its flag, rel its index relative to the pass starting at idx_begin.  One
+// n_ok add and at most one key update per warp.
+SLB_DEV void fold_decided(const slb_fold_target& t, bool mine, bool negative, int64_t rel, int64_t idx_begin) {
+    const bool ok = mine && (negative || (t.initial != nullptr && t.initial[rel] != 0));
+    const bool fail = mine && !ok;
+    const unsigned okb = __ballot_sync(0xffffffffu, ok);
+    const unsigned failb = __ballot_sync(0xffffffffu, fail);
+    uint64_t kv = fail ? value_key(t.values[rel]) : ~0ull;
+    int64_t ki = fail ? idx_begin + rel : INT64_MAX;
+    if (failb != 0) {
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) {
+            const uint64_t ov = __shfl_xor_sync(0xffffffffu, kv, off);
+            const int64_t oi = __shfl_xor_sync(0xffffffffu, ki, off);
+            if (ov < kv || (ov == kv && oi < ki)) { kv = ov; ki = oi; }
+        }
+    }
+    if ((threadIdx.x & 31) != 0) return;
+    if (okb != 0) atomicAdd(&t.rec->n_ok, (unsigned long long)__popc(okb));
+    if (failb != 0) fold_key(t.rec, kv, ki);
+}
+
 // Table-driven exp(x) for x <= 0 (<= 1 ulp against glibc on 2e7 points, tools/exp_neg_tab_check.c):
 // x = (64 k + j) ln2/64 + r, |r| <= ln2/128;  exp(x) = 2^k * T[j] * (1 + r + ... + r^5/120).
 // 10 fp64 operations; T (64 correctly rounded doubles) is read from a shared-memory

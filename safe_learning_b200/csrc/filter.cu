@@ -61,7 +61,13 @@ constexpr int HW = HT / 32;            // ... its 16 warps
 constexpr int HP = 8;                  // ... list entries per warp and round: the n dimension of a DMMA
 constexpr int HEAD_CTAS = SLB_NUM_SMS;  // one CTA per SM (it stages the head factors in shared memory)
 constexpr int64_t CHUNK = 1 << 22;     // points per pass of the three stages (bounds the workspace)
-constexpr int64_t WS_HEAD = 64 + SLB_SPLIT_TICKET_BYTES + (int64_t)SLB_SPLIT_PARTIAL_BYTES;   // bytes before the lists
+// workspace: [0, 64) the counts, then the refine pass's tile tickets, the fold record of a step
+// (slb_safe_set_step: zeroed by the same memset as the counts and tickets), the refine pass's partial
+// sums, then the lists
+constexpr int64_t WS_FOLD = 64 + SLB_SPLIT_TICKET_BYTES;
+constexpr int64_t WS_PARTIAL = WS_FOLD + 128;
+constexpr int64_t WS_HEAD = WS_PARTIAL + (int64_t)SLB_SPLIT_PARTIAL_BYTES;   // bytes before the lists
+static_assert(sizeof(slb_fold) <= WS_PARTIAL - WS_FOLD && WS_FOLD % 16 == 0, "fold record slot");
 
 
 // terms of one undecided point, carried from stage 1 to stage 2
@@ -110,6 +116,7 @@ struct filter_args {
     unsigned long long* timing;        // slb_debug_head_timing: nullptr or [HEAD_CTAS + 1][8] %globaltimer
     unsigned long long* timing1;       // slb_debug_stage1_timing: nullptr or [tiles][8] %globaltimer
     int head_schedule;                 // head stage: 0 chosen from the list length, 1 split, 2 round loop
+    slb_fold_target fold;              // rec != nullptr: every kernel folds the points it decides (common.cuh)
 };
 
 // slb_debug_head_timing: timing[slot] = the latest %globaltimer (ns) at which a warp passed a mark.
@@ -376,6 +383,7 @@ SLB_DEV long long stage1_finish(const filter_args& a, bool valid, int64_t rel, i
     }
     const long long slot = list_append(undecided, a.counts + 0);
     if (undecided) a.list_a[slot] = rel;
+    if (a.fold.rec != nullptr) fold_decided(a.fold, valid && outcome >= 0, outcome > 0, rel, a.idx_begin);
     if (a.stats != nullptr) {
         count_stat(valid && !undecided, a.stats + 0);
         count_stat(valid, a.stats + 3);
@@ -620,6 +628,7 @@ filter_grid_mean_kernel(const __grid_constant__ slb_sweep cfg, const filter_args
         a.negative[rel] = outcome > 0 ? 1 : 0;
         if (a.values != nullptr) a.values[rel] = vx;
     }
+    if (a.fold.rec != nullptr) fold_decided(a.fold, valid && outcome >= 0, outcome > 0, rel, a.idx_begin);
     bool fp64 = sane;                             // every bound finite: an fp64-class mean
 #pragma unroll
     for (int j = 0; j < D; ++j) fp64 &= dm[j] < f64_inf();
@@ -995,6 +1004,7 @@ SLB_DEV void head_group_finish(const filter_args& a, bool mine, int outcome, int
     const int lane = threadIdx.x & 31;
     const bool undecided = mine && outcome < 0;
     if (mine && outcome >= 0) a.negative[rel] = outcome > 0 ? 1 : 0;
+    if (a.fold.rec != nullptr) fold_decided(a.fold, mine && outcome >= 0, outcome > 0, rel, a.idx_begin);
     const long long slot = list_append(undecided, a.counts + 1);
     if (undecided) a.list_b[slot] = rel;
     const unsigned dec = __ballot_sync(0xffffffffu, mine && !undecided);
@@ -1401,10 +1411,16 @@ int dispatch_filter(cudaStream_t st, const slb_sweep& cfg, const filter_args& a)
 
 }  // namespace
 
+// light.cu: the prefix rule on the key a step folded into `rec` (slb_safe_set_step)
+int slb_launch_apply_prefix_folded(cudaStream_t st, const double* values, const uint8_t* initial, int64_t n,
+                                   int64_t idx_begin, slb_fold* rec, slb_fail_key* key, uint8_t* safe,
+                                   slb_prefix_stats* stats);
+
 // gp_sweep.cu: the full posterior on the compacted list (count read on the device)
 int slb_launch_refine(cudaStream_t st, const slb_sweep& cfg, int64_t n_max, int64_t idx_begin,
                       const int64_t* list, const unsigned long long* count, uint8_t* negative,
-                      double* values, double* mean, double* err, double* split_partial, int* split_ticket);
+                      double* values, double* mean, double* err, double* split_partial, int* split_ticket,
+                      const slb_fold_target& fold);
 
 extern "C" {
 
@@ -1458,9 +1474,13 @@ int slb_debug_filter_lists(int64_t n, int64_t* offsets) {
     return 0;
 }
 
-int slb_lyapunov_sweep_filtered(void* stream, const slb_sweep* cfg, int64_t idx_begin,
-                                int64_t idx_end, uint8_t* negative_dev, double* values_dev,
-                                void* workspace_dev, int64_t* stats_dev) {
+}  // extern "C"
+
+// slb_lyapunov_sweep_filtered, and the sweep of slb_safe_set_step with fold.rec != nullptr: the record at
+// WS_FOLD is zeroed with the first pass's counts and accumulates over all passes
+static int filtered_sweep(cudaStream_t st, const slb_sweep* cfg, int64_t idx_begin, int64_t idx_end,
+                          uint8_t* negative_dev, double* values_dev, void* workspace_dev, int64_t* stats_dev,
+                          slb_fold_target fold) {
     int m;
     if (slb_validate_sweep(cfg, false, &m)) return 1;
     if (slb_validate_range("slb_lyapunov_sweep_filtered", idx_begin, idx_end, cfg->grid.nindex)) return 1;
@@ -1490,14 +1510,13 @@ int slb_lyapunov_sweep_filtered(void* stream, const slb_sweep* cfg, int64_t idx_
     if (n_all == 0) return 0;
     SLB_CHECK(negative_dev != nullptr && workspace_dev != nullptr,
               "slb_lyapunov_sweep_filtered: negative_dev and workspace_dev are required");
-    cudaStream_t st = (cudaStream_t)stream;
     char* ws = static_cast<char*>(workspace_dev);
     const int64_t cap = n_all < CHUNK ? n_all : CHUNK;
     filter_args a;
     memset(&a, 0, sizeof(a));
     a.counts = reinterpret_cast<unsigned long long*>(ws);
     int* tickets = reinterpret_cast<int*>(ws + 64);
-    double* partial = reinterpret_cast<double*>(ws + 64 + SLB_SPLIT_TICKET_BYTES);
+    double* partial = reinterpret_cast<double*>(ws + WS_PARTIAL);
     a.list_a = reinterpret_cast<int64_t*>(ws + WS_HEAD);
     a.list_b = a.list_a + cap;
     a.side_a = reinterpret_cast<filter_side*>(a.list_b + cap);
@@ -1516,19 +1535,53 @@ int slb_lyapunov_sweep_filtered(void* stream, const slb_sweep* cfg, int64_t idx_
     a.timing1 = g_stage1_timing;
     for (int64_t off = 0; off < n_all; off += CHUNK) {
         const int64_t n = n_all - off < CHUNK ? n_all - off : CHUNK;
-        SLB_CUDA(cudaMemsetAsync(a.counts, 0, 64 + SLB_SPLIT_TICKET_BYTES, st));
+        const bool first_fold = fold.rec != nullptr && off == 0;
+        SLB_CUDA(cudaMemsetAsync(a.counts, 0, first_fold ? WS_PARTIAL : WS_FOLD, st));
         a.n = n; a.idx_begin = idx_begin + off;
         a.negative = negative_dev + off;
         a.values = values_dev ? values_dev + off : nullptr;
+        a.fold = fold;
+        if (fold.rec != nullptr) {
+            a.fold.values = fold.values + off;
+            a.fold.initial = fold.initial ? fold.initial + off : nullptr;
+        }
         int rc = dispatch_filter(st, *cfg, a);
         if (rc) return rc;
         if (!(g_filter_stages & 2)) continue;
         rc = slb_launch_refine(st, *cfg, n, idx_begin + off, a.list_b, a.counts + 1,
                                negative_dev + off, values_dev ? values_dev + off : nullptr,
-                               nullptr, nullptr, partial, tickets);
+                               nullptr, nullptr, partial, tickets, a.fold);
         if (rc) return rc;
     }
     return 0;
+}
+
+extern "C" {
+
+int slb_lyapunov_sweep_filtered(void* stream, const slb_sweep* cfg, int64_t idx_begin,
+                                int64_t idx_end, uint8_t* negative_dev, double* values_dev,
+                                void* workspace_dev, int64_t* stats_dev) {
+    return filtered_sweep((cudaStream_t)stream, cfg, idx_begin, idx_end, negative_dev, values_dev, workspace_dev,
+                          stats_dev, slb_fold_target{});
+}
+
+int slb_safe_set_step(void* stream, const slb_sweep* cfg, int64_t idx_begin, int64_t idx_end,
+                      uint8_t* negative_dev, const double* values_dev, const uint8_t* initial_dev,
+                      void* workspace_dev, int64_t* stats_dev, slb_fail_key* key_dev, uint8_t* safe_dev,
+                      slb_prefix_stats* prefix_stats_dev) {
+    SLB_CHECK(cfg != nullptr, "slb_safe_set_step: null config");
+    SLB_CHECK(idx_end > idx_begin, "slb_safe_set_step: empty range [%lld, %lld)", (long long)idx_begin,
+              (long long)idx_end);
+    SLB_CHECK(values_dev != nullptr && workspace_dev != nullptr && key_dev != nullptr && safe_dev != nullptr &&
+                  prefix_stats_dev != nullptr,
+              "slb_safe_set_step: null values, workspace, key, safe set or statistics");
+    cudaStream_t st = (cudaStream_t)stream;
+    slb_fold* rec = reinterpret_cast<slb_fold*>(static_cast<char*>(workspace_dev) + WS_FOLD);
+    const int rc = filtered_sweep(st, cfg, idx_begin, idx_end, negative_dev, nullptr, workspace_dev, stats_dev,
+                                  slb_fold_target{values_dev, initial_dev, rec});
+    if (rc) return rc;
+    return slb_launch_apply_prefix_folded(st, values_dev, initial_dev, idx_end - idx_begin, idx_begin, rec,
+                                          key_dev, safe_dev, prefix_stats_dev);
 }
 
 int slb_debug_refine(void* stream, const slb_sweep* cfg, int64_t idx_begin, int64_t n_max,
@@ -1549,8 +1602,8 @@ int slb_debug_refine(void* stream, const slb_sweep* cfg, int64_t idx_begin, int6
     char* ws = static_cast<char*>(workspace_dev);
     SLB_CUDA(cudaMemsetAsync(ws + 64, 0, SLB_SPLIT_TICKET_BYTES, st));
     return slb_launch_refine(st, *cfg, n_max, idx_begin, list_dev, count_dev, negative_dev, values_dev, mean_dev,
-                             err_dev, reinterpret_cast<double*>(ws + 64 + SLB_SPLIT_TICKET_BYTES),
-                             reinterpret_cast<int*>(ws + 64));
+                             err_dev, reinterpret_cast<double*>(ws + WS_PARTIAL), reinterpret_cast<int*>(ws + 64),
+                             slb_fold_target{});
 }
 
 }  // extern "C"

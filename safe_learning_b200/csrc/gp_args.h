@@ -30,6 +30,7 @@ struct slb_gp_args {
     // SLB_SPLIT_ITEMS CTAs.
     double* split_partial;
     int* split_ticket;
+    slb_fold_target fold;   // refine mode: rec != nullptr folds every decided point (common.cuh)
     long long* timing;      // diagnostics: [tile][warp][8]: cycles in {generate, contract, epilogue, total}, globaltimer ns {start, end}, cycles waiting at barriers, 0
 };
 

@@ -86,16 +86,18 @@ static int64_t g_refine_split = 32 * SLB_NUM_SMS;   // longest list that gets 32
 // to spare (up to SLB_SPLIT_MAX groups of equal triangular area, gp_tile.cuh): the tile kernel's
 // duration is set by the M^2 / 2 contraction of one tile, so a few hundred points in whole tiles keep
 // a few dozen SMs busy while the rest idle; split 8 ways a 32-point tile's share is ~8 times shorter.
-// mean / err: NULL, or [n_max, D] rows indexed like `negative` (slb_debug_refine)
+// mean / err: NULL, or [n_max, D] rows indexed like `negative` (slb_debug_refine); fold: see slb_fold_target
 int slb_launch_refine(cudaStream_t st, const slb_sweep& cfg, int64_t n_max, int64_t idx_begin,
                       const int64_t* list, const unsigned long long* count, uint8_t* negative,
-                      double* values, double* mean, double* err, double* split_partial, int* split_ticket) {
+                      double* values, double* mean, double* err, double* split_partial, int* split_ticket,
+                      const slb_fold_target& fold) {
     slb_gp_args a;
     memset(&a, 0, sizeof(a));
     a.idx_begin = idx_begin; a.mode = MODE_SWEEP_GRID;
     a.negative = negative; a.values = values;
     a.mean = mean; a.err = err;
     a.index_list = list; a.count = count;
+    a.fold = fold;
     a.timing = g_timing_buffer;            // slb_debug_phase_timing: per-warp phase clocks of the refine CTAs
     const int tps[2] = {32, 64};
     const int64_t lo[2] = {0, g_refine_split};

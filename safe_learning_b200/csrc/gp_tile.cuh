@@ -601,14 +601,19 @@ SLB_DEV void gp_tile_body(const slb_sweep& cfg, const slb_gp_args& a, unsigned c
         }
         if (a.mode == MODE_PREDICT) return;
         __syncthreads();
+        bool neg = false;
         if (tid < TP && live) {
             const slb_decision r =
                 lyapunov_combine(pre[p], pre[TP + p], pre[2 * TP + p], pre[3 * TP + p]);
+            neg = r.negative;
             a.negative[rel] = r.negative ? 1 : 0;
             if (a.values != nullptr) a.values[rel] = r.vx;
             if (a.decrease != nullptr) a.decrease[rel] = r.decrease;
             if (a.threshold != nullptr) a.threshold[rel] = r.threshold;
         }
+        // refine pass of a step that folds its key (filter.cu): the warps of the tile's points (TP is a
+        // multiple of 32)
+        if (a.fold.rec != nullptr && tid < TP) fold_decided(a.fold, live, neg, rel, a.idx_begin);
     }
 }
 

@@ -594,15 +594,24 @@ __global__ void combine_fail_keys_kernel(const slb_fail_key* __restrict__ gather
 // `world` release flags of the current sweep in this rank's own slot array (local HBM/L2), reduces
 // the keys (lexicographic min, n_ok sum) and block 0 publishes the winner to `key`.  A rank whose
 // peer does not show up within ~10 s gives up and marks the result (key->_pad = -1).
+// fold != nullptr (single process, slb_safe_set_step): the key comes from the record the decision kernels
+// folded it into, block 0 publishes it to `key`; the statistics are added up in the record (zeroed with it)
+// and the last block to finish copies them to `stats`.
 template <bool X>
 __global__ void __launch_bounds__(LT)
 apply_prefix_kernel(const double* __restrict__ values, const uint8_t* __restrict__ initial, int64_t n,
                     int64_t idx_begin, slb_fail_key* __restrict__ key,
                     uint8_t* __restrict__ safe, slb_prefix_stats* __restrict__ stats,
-                    const slb_exchange x) {
+                    const slb_exchange x, slb_fold* __restrict__ fold) {
     uint64_t kv;
     int64_t ki;
-    if (X) {
+    if (fold != nullptr) {
+        kv = ~fold->hi;
+        ki = INT64_MAX - (int64_t)fold->lo;
+        if (blockIdx.x == 0 && threadIdx.x == 0) {
+            key->key_value = kv; key->key_index = ki; key->n_ok = (int64_t)fold->n_ok; key->_pad = 0;
+        }
+    } else if (X) {
         __shared__ int64_t s_k[SLB_MAX_RANKS][3];
         __shared__ int s_timeout;
         if (threadIdx.x == 0) s_timeout = 0;
@@ -669,12 +678,26 @@ apply_prefix_kernel(const double* __restrict__ values, const uint8_t* __restrict
         atomicMax(&s_acc[3], max_all);
     }
     __syncthreads();
-    if (threadIdx.x == 0) {
+    if (threadIdx.x != 0) return;
+    if (fold == nullptr) {
         atomicAdd(reinterpret_cast<unsigned long long*>(&stats->n_safe), s_acc[0]);
         atomicAdd(reinterpret_cast<unsigned long long*>(&stats->n_below), s_acc[1]);
         atomicMax(reinterpret_cast<unsigned long long*>(&stats->max_below), s_acc[2]);
         atomicMax(reinterpret_cast<unsigned long long*>(&stats->max_all), s_acc[3]);
+        return;
     }
+    unsigned long long* acc = fold->acc;
+    atomicAdd(acc + 0, s_acc[0]);
+    atomicAdd(acc + 1, s_acc[1]);
+    atomicMax(acc + 2, s_acc[2]);
+    atomicMax(acc + 3, s_acc[3]);
+    __threadfence();
+    if (atomicAdd(&fold->ticket, 1u) != gridDim.x - 1) return;
+    __threadfence();
+    stats->n_safe = (int64_t)__ldcg(acc + 0);
+    stats->n_below = (int64_t)__ldcg(acc + 1);
+    stats->max_below = __ldcg(acc + 2);
+    stats->max_all = __ldcg(acc + 3);
 }
 
 // ---- Bellman sweep (bellman.cuh) ----------------------------------------------------------
@@ -908,10 +931,24 @@ static int apply_prefix(const char* who, void* stream, const double* values_dev,
     memset(&none, 0, sizeof(none));
     if (x != nullptr && x->world > 1)
         apply_prefix_kernel<true><<<blocks, LT, 0, st>>>(values_dev, initial_dev, n, idx_begin, key_dev,
-                                                         safe_dev, stats_dev, *x);
+                                                         safe_dev, stats_dev, *x, nullptr);
     else
         apply_prefix_kernel<false><<<blocks, LT, 0, st>>>(values_dev, initial_dev, n, idx_begin, key_dev,
-                                                          safe_dev, stats_dev, x != nullptr ? *x : none);
+                                                          safe_dev, stats_dev, x != nullptr ? *x : none, nullptr);
+    SLB_LAUNCH_CHECK();
+    return 0;
+}
+
+// filter.cu (slb_safe_set_step): the prefix rule on the key folded into `rec` by the step's sweep, which
+// also zeroed the record; no memset of its own
+int slb_launch_apply_prefix_folded(cudaStream_t st, const double* values, const uint8_t* initial, int64_t n,
+                                   int64_t idx_begin, slb_fold* rec, slb_fail_key* key, uint8_t* safe,
+                                   slb_prefix_stats* stats) {
+    const int64_t want = (n + LT - 1) / LT;
+    const unsigned blocks = (unsigned)(want > 2048 ? 2048 : (want < 1 ? 1 : want));
+    slb_exchange none;
+    memset(&none, 0, sizeof(none));
+    apply_prefix_kernel<false><<<blocks, LT, 0, st>>>(values, initial, n, idx_begin, key, safe, stats, none, rec);
     SLB_LAUNCH_CHECK();
     return 0;
 }

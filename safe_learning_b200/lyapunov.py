@@ -645,6 +645,16 @@ class Lyapunov(object):
                   "slb_lyapunov_sweep")
         return self._negative_dev, details
 
+    def _filter_buffers(self, n):
+        """Workspace of a filtered sweep of ``n`` points and the filter's statistics (device)."""
+        lib = nat.load()
+        need = int(lib.slb_filter_workspace(n)) // 8 + 1
+        if self._filter_ws is None or self._filter_ws.numel() < need:
+            self._filter_ws = dev.empty((need,), torch.int64)
+        if self._filter_stats is None:
+            self._filter_stats = dev.zeros((4,), torch.int64)
+        return self._filter_ws, self._filter_stats
+
     def compute_negative_range(self, begin, end, out=None):
         """``negative`` for the flat grid indices ``[begin, end)`` on the default path (filtered
         when the dynamics are a GP, see ``filter``) -> device uint8 tensor."""
@@ -654,15 +664,10 @@ class Lyapunov(object):
         if out is None:
             out = dev.empty((n,), torch.uint8)
         if self._filter_enabled(cfg):
-            need = int(lib.slb_filter_workspace(n)) // 8 + 1
-            if self._filter_ws is None or self._filter_ws.numel() < need:
-                self._filter_ws = dev.empty((need,), torch.int64)
-            if self._filter_stats is None:
-                self._filter_stats = dev.zeros((4,), torch.int64)
+            ws, stats = self._filter_buffers(n)
             nat.check(lib.slb_lyapunov_sweep_filtered(dev.stream(), cfg, begin, end,
-                                                      out.data_ptr(), None,
-                                                      self._filter_ws.data_ptr(),
-                                                      self._filter_stats.data_ptr()),
+                                                      out.data_ptr(), None, ws.data_ptr(),
+                                                      stats.data_ptr()),
                       "slb_lyapunov_sweep_filtered")
         else:
             nat.check(lib.slb_lyapunov_sweep(dev.stream(), cfg, begin, end, out.data_ptr(),
@@ -822,6 +827,21 @@ class Lyapunov(object):
 
         def enqueue():
             st = dev.stream()
+            if not adaptive and world == 1 and not self._is_composed():
+                cfg = self.sweep_descriptor()
+                if self._filter_enabled(cfg):
+                    # the filter's decision kernels fold the first-fail key as they decide: one memset,
+                    # the three stages and the prefix kernel (slb_safe_set_step)
+                    if self._negative_dev is None or self._negative_dev.numel() != n_local:
+                        self._negative_dev = dev.empty((n_local,), torch.uint8)
+                    ws, stats = self._filter_buffers(n_local)
+                    nat.check(lib.slb_safe_set_step(st, cfg, self._begin, self._end,
+                                                    self._negative_dev.data_ptr(),
+                                                    self._values_dev.data_ptr(), dev.ptr(initial),
+                                                    ws.data_ptr(), stats.data_ptr(),
+                                                    self._key_dev.data_ptr(), self._safe_dev.data_ptr(),
+                                                    self._stats_dev.data_ptr()), "slb_safe_set_step")
+                    return
             neg = flags if adaptive else self.compute_negative()
             args = (st, self._values_dev.data_ptr(), neg.data_ptr(), dev.ptr(initial), n_local,
                     self._begin, self._workspace.data_ptr(), self._key_dev.data_ptr())
@@ -848,7 +868,8 @@ class Lyapunov(object):
                                            self._safe_dev.data_ptr(), self._workspace.data_ptr(),
                                            self._stats_dev.data_ptr()), "slb_apply_prefix")
 
-        # CUDA-graph replay of the launches of a sweep (memsets + 8 kernels; no collective call
+        # CUDA-graph replay of the launches of a sweep (one memset + 5 kernels on the filtered single-process
+        # path, memsets + 8 kernels otherwise; no collective call
         # inside when the keys travel through peer memory) while nothing they depend on changes:
         # the second sweep with an unchanged descriptor is captured, later ones replay it.  It saves
         # device time between the launches and the host enqueue time per sweep, which is what
