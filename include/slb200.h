@@ -342,6 +342,13 @@ int         slb_debug_head_timing(void* buffer_dev);
  * work items 0, 1, 2 and 3 (and later) done, means done, exit} (tools/stage1_timeline.py); pass NULL to
  * switch it off (default) */
 int         slb_debug_stage1_timing(void* buffer_dev);
+/* diagnostics: when buffer_dev != NULL (uint64 [512][16], zeroed by the caller), every later filtered sweep
+ * whose refine pass runs row-split 32-point tiles raises entry [c][m] to the %globaltimer (ns) at which the
+ * last warp of its CTA c passed mark m = {entry, prologue done, j-panel 0, 1, 2, 3 (and later) generated,
+ * j-panel 0, 1, 2, 3 (and later) contracted, partial sums written, ticket taken, factor epilogues done,
+ * decision and fold done, exit}, and sets [c][15] = 1 in the CTAs that finished a tile
+ * (tools/refine_timeline.py); pass NULL to switch it off (default) */
+int         slb_debug_refine_timing(void* buffer_dev);
 /* Records an event (owned by the library, one per device) on `stream` that every later launch reading
  * the packed factors (slb_gp_factor.Wpack: the full posterior of slb_gp_predict / slb_lyapunov_sweep /
  * slb_lyapunov_points and the refine pass of slb_lyapunov_sweep_filtered) waits for on ITS stream.  A

@@ -137,6 +137,7 @@ SIGNATURES = {
     "slb_debug_phase_timing": (C.c_int, [_vp]),
     "slb_debug_head_timing": (C.c_int, [_vp]),
     "slb_debug_stage1_timing": (C.c_int, [_vp]),
+    "slb_debug_refine_timing": (C.c_int, [_vp]),
     "slb_record_factor_dependency": (C.c_int, [_vp]),
     "slb_restore_tables": (C.c_int, [_vp, _vp, _i64, _i64, _vp, _vp]),
     "slb_debug_refine_split": (C.c_int, [_i64]),

@@ -1035,24 +1035,30 @@ SLB_DEV void lyapunov_state_terms_closed(const slb_sweep& cfg, const double (&x)
 }
 
 // (2) sum_j L_V(mu)_j err_j, L_V evaluated at the predicted MEAN                :344-347
-SLB_DEV double lyapunov_error_bound(const slb_sweep& cfg, const double* mu, const double* err) {
-    const int d = cfg.grid.ndim;
-    double tmp[SLB_MAX_OUT];
-    double bound;
-    if (cfg.lipschitz_v.kind != SLB_FN_NONE) {
-        const int nl = eval_fn_small(cfg.lipschitz_v, mu, tmp);
-        if (nl == 1) {
-            bound = f64mul(tmp[0], err[0]);
-            for (int j = 1; j < d; ++j) bound = f64add(bound, f64mul(tmp[0], err[j]));
-        } else {
-            bound = f64mul(tmp[0], err[0]);
-            for (int j = 1; j < d; ++j) bound = f64add(bound, f64mul(tmp[j], err[j]));
-        }
-    } else {
-        bound = f64mul(cfg.lv_const, err[0]);
-        for (int j = 1; j < d; ++j) bound = f64add(bound, f64mul(cfg.lv_const, err[j]));
-    }
+// ... from L_V(mu)'s nl columns lv (one column: the same factor for every j)
+SLB_DEV double lyapunov_error_sum(const double* lv, int nl, const double* err, int d) {
+    double bound = f64mul(lv[0], err[0]);
+    for (int j = 1; j < d; ++j) bound = f64add(bound, f64mul(nl == 1 ? lv[0] : lv[j], err[j]));
     return bound;
+}
+
+SLB_DEV double lyapunov_error_bound(const slb_sweep& cfg, const double* mu, const double* err) {
+    double lv[SLB_MAX_OUT];
+    int nl = 1;
+    lv[0] = cfg.lv_const;
+    if (cfg.lipschitz_v.kind != SLB_FN_NONE) nl = eval_fn_small(cfg.lipschitz_v, mu, lv);
+    return lyapunov_error_sum(lv, nl, err, cfg.grid.ndim);
+}
+
+// ... the same for the closed form (D outputs = the state's dims, L_V absent or LINEAR as in
+// lyapunov_state_terms_closed)
+template <int D>
+SLB_DEV double lyapunov_error_bound_closed(const slb_sweep& cfg, const double (&mu)[D], const double (&err)[D]) {
+    int nl = 1;
+    slb_vec<SLB_MAX_LIN_OUT> lv;
+    lv.v[0] = cfg.lv_const;
+    if (cfg.lipschitz_v.kind != SLB_FN_NONE) lv = eval_linear_reg<D, SLB_MAX_LIN_OUT>(cfg.lipschitz_v, mu, nl);
+    return lyapunov_error_sum(lv.v, nl, err, D);
 }
 
 // (3) V(mu); then decrease = (V(mu) - V(x)) + bound  and  negative = decrease < threshold

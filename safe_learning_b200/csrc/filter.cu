@@ -19,15 +19,16 @@
 //                mean of gp_mean_grid.cuh with its fp64-class bound: 2-D grids, z = [x0, x1, u], a linear
 //                policy (grid_mean_applicable).
 //              The last two decide a point when the outcome is the same over the whole box mu +- dm
-//              (screened_outcome) and leave list A entries in the screened layout: z, threshold, V(x) in
-//              dec0, the screened mean in coef and its bound in dm;
+//              (screened_outcome) and leave list A entries in the screened layout: z, threshold, V(x),
+//              the screened mean in coef and its bound in dm;
 //   stage 2  (filter_head_kernel, one CTA per SM, a warp per 8 entries of list A) the posterior variance
 //            given a HEAD SUBSET of at most SLB_HEAD_RANK training points (chosen by the host in pivoted-
 //            Cholesky order, its own small factor: slb_gp_factor.Wheadp / Xhead); decide with the
 //            tighter bound -- screened entries first over their box, then, unless their mean is
 //            fp64-class already, with the mean recomputed in fp64 by the whole CTA (head_round_means).
 //            Two schedules: a warp per group, or per (group, factor) pair when the list is short;
-//   rest     compacted into list B for the full fp64 posterior (gp_tile_kernel, gp_sweep.cu).
+//   rest     compacted into list B for the full fp64 posterior (gp_tile_kernel, gp_sweep.cu), which takes
+//            z, V(x) and the threshold from the entry's list A terms (slot_b).
 // Certification.  A point is only decided when the outcome holds with a guard band that covers
 // (a) 1e-6 relative to the magnitudes involved (five orders above the rounding differences between
 // two fp64 evaluation orders of the posterior; the GP tolerance of the parity contract is 1e-5) and
@@ -70,10 +71,10 @@ constexpr int64_t WS_HEAD = WS_PARTIAL + (int64_t)SLB_SPLIT_PARTIAL_BYTES;   // 
 static_assert(sizeof(slb_fold) <= WS_PARTIAL - WS_FOLD && WS_FOLD % 16 == 0, "fold record slot");
 
 
-// terms of one undecided point, carried from stage 1 to stage 2
-struct filter_side { double dec0, thr, guard, coef[SLB_MAX_OUT], z[SLB_MAX_IN], dm[SLB_MAX_OUT]; };
-// fp32 screening stage: dec0 = V(x), coef[j] = screened mean of output j, dm[j] = its certified bound
-// (the head stage rebuilds the mean-dependent terms from them, and from an fp64 mean where needed)
+// terms of one undecided point (filter_side, gp_args.h): z, thr and vx in every layout.  fp64 mean stage: dec0 =
+// V(mu) - V(x), guard and coef as decide() reads them.  Screened stages: coef[j] = screened mean of output j,
+// dm[j] = its certified bound (the head stage rebuilds the mean-dependent terms from them, and from an fp64
+// mean where needed)
 
 // What stage1_plan decides for a sweep: the mean scheme of stage 1 (which fixes the layout of list A) and
 // the shared memory of a head CTA, as offsets in doubles from its base.  [0, 4) there: three mbarriers
@@ -105,6 +106,7 @@ struct filter_args {
     int64_t* list_a;                   // undecided after stage 1 (index relative to the range)
     filter_side* side_a;               // their terms, same order
     int64_t* list_b;                   // undecided after stage 2 -> full posterior
+    int64_t* slot_b;                   // ... the list A slot of each (the refine pass reads its terms)
     unsigned long long* counts;        // [0] entries of list_a, [1] entries of list_b, [2] see filter_plan
     unsigned long long* stats;         // nullptr or [4], see slb200.h
     int chunk_rows;                    // training rows per staged slice (multiple of 8)
@@ -413,7 +415,7 @@ SLB_DEV void stage1_screened_finish(const slb_sweep& cfg, const filter_args& a, 
     const long long slot = stage1_finish(a, valid, rel, sane ? screened : -1, vx);
     if (slot >= 0) {
         filter_side* dst = a.side_a + slot;
-        dst->dec0 = vx;
+        dst->vx = vx;
         dst->thr = thr;
 #pragma unroll
         for (int c = 0; c < DIN; ++c) dst->z[c] = z[c];
@@ -455,6 +457,7 @@ filter_mean_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
 
     double shi[SLB_MAX_OUT];
     prior_sigma_bound<DIN>(cfg.gp, t.z, shi);
+    t.vx = vx;
     const long long slot = stage1_finish(a, valid, rel, sane ? decide(t, shi, cfg.gp.num_outputs) : -1, vx);
     if (slot >= 0) a.side_a[slot] = t;
     timing_mark(a, HEAD_CTAS * 8);
@@ -662,13 +665,13 @@ filter_grid_mean_kernel(const __grid_constant__ slb_sweep cfg, const filter_args
     }
     __syncthreads();
     if (undecided) {
-        // the list A entry in the screened layout: V(x) in dec0, the threshold, z, the mean and its bound (the
-        // head stage rebuilds the mean-dependent terms)
+        // the list A entry in the screened layout: V(x), the threshold, z, the mean and its bound (the head
+        // stage rebuilds the mean-dependent terms)
         unsigned long long slot = *s_base + __popc(und & ((1u << lane) - 1));
         for (int w = 0; w < warp; ++w) slot += s_cnt[w];
         a.list_a[slot] = rel;
         filter_side* dst = a.side_a + slot;
-        dst->dec0 = vx;
+        dst->vx = vx;
         dst->thr = thr;
         dst->z[0] = x[0];
         dst->z[1] = x[1];
@@ -955,7 +958,7 @@ SLB_DEV int head_entry_decision(const slb_sweep& cfg, const filter_args& a, cf_e
     if (t.k >= 0) {
         t.rel = a.list_a[t.k];
         const filter_side* e = a.side_a + t.k;
-        t.vx = e->dec0;
+        t.vx = e->vx;
         t.thr = e->thr;
 #pragma unroll
         for (int j = 0; j < D; ++j) { t.mu[j] = e->coef[j]; t.dm[j] = e->dm[j]; }
@@ -989,24 +992,33 @@ SLB_DEV int head_mean_decision(const slb_sweep& cfg, cf_entry<DIN, D>& t, double
     return cf_decide<D>(terms, shi);
 }
 
-// the grid index of an entry (complete: the one head_group_entries loaded)
+// the grid index of an entry (complete: the one head_group_entries loaded) and its list A slot (lane p of group
+// grp holds entry grp HP + p)
 SLB_DEV int64_t entry_rel(const filter_side&, int64_t rel) { return rel; }
 template <int DIN, int D>
 SLB_DEV int64_t entry_rel(const cf_entry<DIN, D>& t, int64_t) { return t.rel; }
+SLB_DEV int64_t entry_slot(const filter_side&, int64_t grp) { return grp * HP + (threadIdx.x & 31); }
+template <int DIN, int D>
+SLB_DEV int64_t entry_slot(const cf_entry<DIN, D>& t, int64_t) { return t.k; }
 
 // every copy lands in this CTA's shared memory before the CTA may leave
 SLB_DEV void head_wait_landings(uint64_t* bar) {
     for (int b = 0; b < 3; ++b) slb_bulk::mbar_wait(bar + b, 0);
 }
 
-// a lane's final outcome: the flag of a decided point, list B for an undecided one (warp-collective)
-SLB_DEV void head_group_finish(const filter_args& a, bool mine, int outcome, int64_t rel, unsigned* s_stat) {
+// a lane's final outcome: the flag of a decided point, list B (and its list A slot k) for an undecided one
+// (warp-collective)
+SLB_DEV void head_group_finish(const filter_args& a, bool mine, int outcome, int64_t rel, int64_t k,
+                               unsigned* s_stat) {
     const int lane = threadIdx.x & 31;
     const bool undecided = mine && outcome < 0;
     if (mine && outcome >= 0) a.negative[rel] = outcome > 0 ? 1 : 0;
     if (a.fold.rec != nullptr) fold_decided(a.fold, mine && outcome >= 0, outcome > 0, rel, a.idx_begin);
     const long long slot = list_append(undecided, a.counts + 1);
-    if (undecided) a.list_b[slot] = rel;
+    if (undecided) {
+        a.list_b[slot] = rel;
+        a.slot_b[slot] = k;
+    }
     const unsigned dec = __ballot_sync(0xffffffffu, mine && !undecided);
     const unsigned und = __ballot_sync(0xffffffffu, undecided);
     if (lane == 0) {
@@ -1198,7 +1210,8 @@ filter_head_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
                 if constexpr (CD > 0)
                     if (need) outcome = head_mean_decision(cfg, t, vx, shi, mu_s, merr_s, slot);
                 head_mark(a, HM_DECIDED);
-                head_group_finish(a, mine, outcome, entry_rel(t, rel), s_stat);
+                head_group_finish(a, mine, outcome, entry_rel(t, rel),
+                                  entry_slot(t, grp0 + (int64_t)warp * gridDim.x), s_stat);
             }
             __syncthreads();                              // sd_s, mu_s are the next round's
         }
@@ -1239,7 +1252,7 @@ filter_head_kernel(const __grid_constant__ slb_sweep cfg, const filter_args a) {
             }
             if (active) {
                 head_mark(a, HM_DECIDED);
-                head_group_finish(a, mine, outcome, entry_rel(t, rel), s_stat);
+                head_group_finish(a, mine, outcome, entry_rel(t, rel), entry_slot(t, grp), s_stat);
             }
         }
     }
@@ -1420,7 +1433,8 @@ int slb_launch_apply_prefix_folded(cudaStream_t st, const double* values, const 
 int slb_launch_refine(cudaStream_t st, const slb_sweep& cfg, int64_t n_max, int64_t idx_begin,
                       const int64_t* list, const unsigned long long* count, uint8_t* negative,
                       double* values, double* mean, double* err, double* split_partial, int* split_ticket,
-                      const slb_fold_target& fold);
+                      const slb_fold_target& fold, const filter_side* side, const int64_t* side_slot,
+                      bool closed);
 
 extern "C" {
 
@@ -1459,8 +1473,8 @@ int64_t slb_filter_workspace(int64_t n) {
     if (n < 0) n = 0;
     if (n > CHUNK) n = CHUNK;     // longer ranges are swept in passes of CHUNK points
     // [0] |list A|, [1] |list B| (uint64, 64 bytes reserved), tile tickets and partial sums of the
-    // row-split refine pass, list A, list B, terms of list A
-    return WS_HEAD + n * (int64_t)(2 * sizeof(int64_t) + sizeof(filter_side));
+    // row-split refine pass, list A, list B, the list A slots of list B, terms of list A
+    return WS_HEAD + n * (int64_t)(3 * sizeof(int64_t) + sizeof(filter_side));
 }
 
 int slb_debug_filter_lists(int64_t n, int64_t* offsets) {
@@ -1519,7 +1533,8 @@ static int filtered_sweep(cudaStream_t st, const slb_sweep* cfg, int64_t idx_beg
     double* partial = reinterpret_cast<double*>(ws + WS_PARTIAL);
     a.list_a = reinterpret_cast<int64_t*>(ws + WS_HEAD);
     a.list_b = a.list_a + cap;
-    a.side_a = reinterpret_cast<filter_side*>(a.list_b + cap);
+    a.slot_b = a.list_b + cap;
+    a.side_a = reinterpret_cast<filter_side*>(a.slot_b + cap);
     a.stats = reinterpret_cast<unsigned long long*>(stats_dev);
     // rows per staged slice: two buffers of (d_in + 1 + outputs per factor) doubles per row within
     // ~24 KB, so that 7 CTAs stay resident per SM
@@ -1550,7 +1565,8 @@ static int filtered_sweep(cudaStream_t st, const slb_sweep* cfg, int64_t idx_beg
         if (!(g_filter_stages & 2)) continue;
         rc = slb_launch_refine(st, *cfg, n, idx_begin + off, a.list_b, a.counts + 1,
                                negative_dev + off, values_dev ? values_dev + off : nullptr,
-                               nullptr, nullptr, partial, tickets, a.fold);
+                               nullptr, nullptr, partial, tickets, a.fold, a.side_a, a.slot_b,
+                               a.plan.mean_scheme == SLB_MEAN_GRID_FACTORED);
         if (rc) return rc;
     }
     return 0;
@@ -1603,7 +1619,7 @@ int slb_debug_refine(void* stream, const slb_sweep* cfg, int64_t idx_begin, int6
     SLB_CUDA(cudaMemsetAsync(ws + 64, 0, SLB_SPLIT_TICKET_BYTES, st));
     return slb_launch_refine(st, *cfg, n_max, idx_begin, list_dev, count_dev, negative_dev, values_dev, mean_dev,
                              err_dev, reinterpret_cast<double*>(ws + WS_PARTIAL), reinterpret_cast<int*>(ws + 64),
-                             slb_fold_target{});
+                             slb_fold_target{}, nullptr, nullptr, false);
 }
 
 }  // extern "C"

@@ -7,6 +7,13 @@ enum { MODE_SWEEP_GRID = 0, MODE_SWEEP_STATES = 1, MODE_PREDICT = 2 };
 enum { SLB_SPLIT_ITEMS = 512, SLB_SPLIT_MAX = 8, SLB_SPLIT_TICKET_BYTES = 2048 };
 // bytes of the split workspace: partial sums of SLB_SPLIT_ITEMS CTAs (64-point upper bound per tile)
 #define SLB_SPLIT_PARTIAL_BYTES ((size_t)SLB_SPLIT_ITEMS * SLB_MAX_OUT * (1 + SLB_MAX_OUT) * 64 * sizeof(double))
+// slb_debug_refine_timing: marks per CTA of the row-split refine launch
+enum { SLB_REFINE_MARKS = 16 };
+
+// Terms of one point the decision filter (filter.cu) left undecided, carried from stage 1 to the head stage
+// and, for the points of list B, to the refine pass.  Every mean scheme stores z = [x, policy(x)], thr =
+// threshold(x) and vx = V(x) as the tile prologue computes them; the other fields per scheme (filter.cu).
+struct filter_side { double dec0, thr, guard, vx, coef[SLB_MAX_OUT], z[SLB_MAX_IN], dm[SLB_MAX_OUT]; };
 
 struct slb_gp_args {
     const double* points;   // MODE_SWEEP_STATES: [n, d]; MODE_PREDICT: [n, d_in]
@@ -31,6 +38,14 @@ struct slb_gp_args {
     double* split_partial;
     int* split_ticket;
     slb_fold_target fold;   // refine mode: rec != nullptr folds every decided point (common.cuh)
+    // refine pass of the filtered sweep: the stage-1 terms of list entry i are side[side_slot[i]] (its list A
+    // entry); the tile reads them instead of evaluating the policy and V.  NULL: computed from the index.
+    const filter_side* side;
+    const int64_t* side_slot;
+    // with side: the sweep is the filter's closed form (grid_mean_applicable, two outputs, d_in = 3), and the
+    // tile is finished by the register-only evaluators
+    int32_t closed;
+    unsigned long long* marks;   // slb_debug_refine_timing: [CTA][SLB_REFINE_MARKS] %globaltimer, or NULL
     long long* timing;      // diagnostics: [tile][warp][8]: cycles in {generate, contract, epilogue, total}, globaltimer ns {start, end}, cycles waiting at barriers, 0
 };
 

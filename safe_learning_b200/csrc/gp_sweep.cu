@@ -73,6 +73,7 @@ int slb_launch_det_sweep(cudaStream_t st, const slb_sweep& cfg, const double* st
                          double* threshold, double* mean);
 
 static long long* g_timing_buffer = nullptr;
+static unsigned long long* g_refine_timing = nullptr;   // slb_debug_refine_timing
 
 // The full posterior for the points the decision filter (filter.cu) could not decide: `list`
 // holds their indices relative to idx_begin, `count` (device) how many there are.  The list is
@@ -86,11 +87,13 @@ static int64_t g_refine_split = 32 * SLB_NUM_SMS;   // longest list that gets 32
 // to spare (up to SLB_SPLIT_MAX groups of equal triangular area, gp_tile.cuh): the tile kernel's
 // duration is set by the M^2 / 2 contraction of one tile, so a few hundred points in whole tiles keep
 // a few dozen SMs busy while the rest idle; split 8 ways a 32-point tile's share is ~8 times shorter.
-// mean / err: NULL, or [n_max, D] rows indexed like `negative` (slb_debug_refine); fold: see slb_fold_target
+// mean / err: NULL, or [n_max, D] rows indexed like `negative` (slb_debug_refine); fold: see slb_fold_target;
+// side / side_slot / closed: see slb_gp_args (NULL: the terms are computed from the list's indices)
 int slb_launch_refine(cudaStream_t st, const slb_sweep& cfg, int64_t n_max, int64_t idx_begin,
                       const int64_t* list, const unsigned long long* count, uint8_t* negative,
                       double* values, double* mean, double* err, double* split_partial, int* split_ticket,
-                      const slb_fold_target& fold) {
+                      const slb_fold_target& fold, const filter_side* side, const int64_t* side_slot,
+                      bool closed) {
     slb_gp_args a;
     memset(&a, 0, sizeof(a));
     a.idx_begin = idx_begin; a.mode = MODE_SWEEP_GRID;
@@ -98,6 +101,8 @@ int slb_launch_refine(cudaStream_t st, const slb_sweep& cfg, int64_t n_max, int6
     a.mean = mean; a.err = err;
     a.index_list = list; a.count = count;
     a.fold = fold;
+    a.side = side; a.side_slot = side_slot;
+    a.closed = side != nullptr && closed;
     a.timing = g_timing_buffer;            // slb_debug_phase_timing: per-warp phase clocks of the refine CTAs
     const int tps[2] = {32, 64};
     const int64_t lo[2] = {0, g_refine_split};
@@ -106,12 +111,13 @@ int slb_launch_refine(cudaStream_t st, const slb_sweep& cfg, int64_t n_max, int6
         if (lo[v] >= hi[v] || lo[v] >= n_max) continue;
         a.count_min = lo[v]; a.count_max = hi[v];
         a.n = n_max < hi[v] ? n_max : hi[v];        // the grid never needs to cover more
-        a.split_partial = nullptr; a.split_ticket = nullptr;
+        a.split_partial = nullptr; a.split_ticket = nullptr; a.marks = nullptr;
         if (v == 0 && split_partial != nullptr) {
             // at least one CTA per SM, so that short lists have CTAs to spread their rows over
             if (a.n < (int64_t)SLB_NUM_SMS * tps[v]) a.n = (int64_t)SLB_NUM_SMS * tps[v];
             if ((a.n + tps[v] - 1) / tps[v] <= SLB_SPLIT_ITEMS) {
                 a.split_partial = split_partial; a.split_ticket = split_ticket;
+                a.marks = g_refine_timing;
             }
         }
         const int rc = dispatch_gp_tile(st, cfg, a, tps[v]);
@@ -168,6 +174,11 @@ int slb_record_factor_dependency(void* stream) {
 
 int slb_debug_phase_timing(void* buffer_dev) {
     g_timing_buffer = static_cast<long long*>(buffer_dev);
+    return 0;
+}
+
+int slb_debug_refine_timing(void* buffer_dev) {
+    g_refine_timing = static_cast<unsigned long long*>(buffer_dev);
     return 0;
 }
 

@@ -182,8 +182,23 @@ SLB_DEV void row_lane_reduce(const double (&v)[2 * NBT], int lane, double* red_q
     }
 }
 
-// One tile (or one row / factor share of it) on the calling CTA: the body of gp_tile_kernel.
-template <int DIN, bool TIMING, bool KEXPR>
+// slb_debug_refine_timing: marks[CTA][slot] = the latest %globaltimer (ns) at which a warp of the CTA passed
+// the mark; the 32-point refine tiles only.  RM_GEN / RM_MMA + k: j-panel k (k = 3: the last ones) generated /
+// contracted; RM_FINISHER: 1 in the CTA that finished its tile
+enum { RM_ENTRY, RM_PROLOGUE, RM_GEN, RM_MMA = RM_GEN + 4, RM_PARTIAL = RM_MMA + 4, RM_TICKET, RM_FACTORS, RM_DECIDED,
+       RM_EXIT, RM_FINISHER };
+static_assert(RM_FINISHER < SLB_REFINE_MARKS, "refine marks");
+SLB_DEV void refine_mark(const slb_gp_args& a, int slot) {
+    if (TP != 32 || a.marks == nullptr || (threadIdx.x & 31) != 0) return;
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    atomicMax(a.marks + blockIdx.x * SLB_REFINE_MARKS + slot, t);
+}
+
+// One tile (or one row / factor share of it) on the calling CTA: the body of gp_tile_kernel.  CD > 0: the
+// refine pass of the filter's closed form (CD outputs), which reads its terms from stage 1's list A entries and
+// finishes the tile with the register-only evaluators.
+template <int DIN, bool TIMING, bool KEXPR, int CD>
 SLB_DEV void gp_tile_body(const slb_sweep& cfg, const slb_gp_args& a, unsigned char* smem_raw,
                           const int64_t tile_index, const int64_t npts, const int grp, const int G,
                           const int fsel, const int FS, const bool first_tile) {
@@ -232,15 +247,50 @@ SLB_DEV void gp_tile_body(const slb_sweep& cfg, const slb_gp_args& a, unsigned c
     if (tid < 64) exptab[tid] = exp_entry;
 
     // ---- stage 1: query points z = [x, policy(x)]  (lyapunov.py:436-437, utilities.py:143)
-    if (tid < TP) {
-        int64_t rel = tile0 + tid;
-        if (rel > npts - 1) rel = npts - 1;
-        if (a.index_list != nullptr) rel = a.index_list[rel];
-        double z[SLB_MAX_IN];
-        if (a.mode == MODE_PREDICT) {
+    if (tid < 2 * TP && (CD > 0 || a.side != nullptr)) {
+        // refine pass of the filtered sweep: stage 1 computed the point's z, V(x) and threshold with the
+        // arithmetic below and left them in its list A entry
+        const int p = tid & (TP - 1);
+        int64_t i = tile0 + p;
+        if (i > npts - 1) i = npts - 1;
+        const filter_side* e = a.side + a.side_slot[i];
+        if (tid < TP) {
 #pragma unroll
-            for (int c = 0; c < DIN; ++c) z[c] = a.points[rel * DIN + c];
+            for (int c = 0; c < DIN; ++c) zraw[c * TP + p] = e->z[c];
         } else {
+            pre[p] = e->vx;
+            pre[TP + p] = e->thr;
+        }
+    } else if constexpr (CD == 0) {
+        if (tid < TP) {
+            int64_t rel = tile0 + tid;
+            if (rel > npts - 1) rel = npts - 1;
+            if (a.index_list != nullptr) rel = a.index_list[rel];
+            double z[SLB_MAX_IN];
+            if (a.mode == MODE_PREDICT) {
+#pragma unroll
+                for (int c = 0; c < DIN; ++c) z[c] = a.points[rel * DIN + c];
+            } else {
+                const int d = cfg.grid.ndim;
+                double x[SLB_MAX_DIM];
+                if (a.mode == MODE_SWEEP_GRID) {
+                    grid_index_to_state(cfg.grid, a.idx_begin + rel, x);
+                } else {
+                    for (int c = 0; c < d; ++c) x[c] = a.points[rel * d + c];
+                }
+                double u[SLB_MAX_OUT];
+                const int m = eval_fn_small(cfg.policy, x, u);
+                for (int c = 0; c < d; ++c) z[c] = x[c];
+                for (int c = 0; c < m; ++c) z[d + c] = u[c];
+            }
+#pragma unroll
+            for (int c = 0; c < DIN; ++c) zraw[c * TP + tid] = z[c];
+        } else if (tid < 2 * TP && a.mode != MODE_PREDICT) {
+            // warps 2-3, concurrently: the terms of the decision that need only x
+            const int p = tid - TP;
+            int64_t rel = tile0 + p;
+            if (rel > npts - 1) rel = npts - 1;
+            if (a.index_list != nullptr) rel = a.index_list[rel];
             const int d = cfg.grid.ndim;
             double x[SLB_MAX_DIM];
             if (a.mode == MODE_SWEEP_GRID) {
@@ -248,30 +298,12 @@ SLB_DEV void gp_tile_body(const slb_sweep& cfg, const slb_gp_args& a, unsigned c
             } else {
                 for (int c = 0; c < d; ++c) x[c] = a.points[rel * d + c];
             }
-            double u[SLB_MAX_OUT];
-            const int m = eval_fn_small(cfg.policy, x, u);
-            for (int c = 0; c < d; ++c) z[c] = x[c];
-            for (int c = 0; c < m; ++c) z[d + c] = u[c];
+            lyapunov_state_terms(cfg, x, a.mode == MODE_SWEEP_GRID ? a.idx_begin + rel : -1, &pre[p],
+                                 &pre[TP + p]);
         }
-#pragma unroll
-        for (int c = 0; c < DIN; ++c) zraw[c * TP + tid] = z[c];
-    } else if (tid < 2 * TP && a.mode != MODE_PREDICT) {
-        // warps 2-3, concurrently: the terms of the decision that need only x
-        const int p = tid - TP;
-        int64_t rel = tile0 + p;
-        if (rel > npts - 1) rel = npts - 1;
-        if (a.index_list != nullptr) rel = a.index_list[rel];
-        const int d = cfg.grid.ndim;
-        double x[SLB_MAX_DIM];
-        if (a.mode == MODE_SWEEP_GRID) {
-            grid_index_to_state(cfg.grid, a.idx_begin + rel, x);
-        } else {
-            for (int c = 0; c < d; ++c) x[c] = a.points[rel * d + c];
-        }
-        lyapunov_state_terms(cfg, x, a.mode == MODE_SWEEP_GRID ? a.idx_begin + rel : -1, &pre[p],
-                             &pre[TP + p]);
     }
     __syncthreads();
+    refine_mark(a, RM_PROLOGUE);
 
     // Row blocks are dealt by `wslot`; warps w and w+4 share an SMSP (and its fp64 pipe), so
     // their slots sum to 7 and every SMSP gets the same share of the triangular panels.
@@ -441,6 +473,7 @@ SLB_DEV void gp_tile_body(const slb_sweep& cfg, const slb_gp_args& a, unsigned c
                     if (TIMING) { t_s0 = clock64(); t_gen += t_s0 - t_mark; }
                     __syncthreads();
                     if (TIMING) t_sync += clock64() - t_s0;
+                    refine_mark(a, RM_GEN + min(jp, 3));
                 }
                 if (TIMING) t_mark = clock64();
                 // ---- contraction phase: acc[rows of this warp, 64 points] += W[rows, panel] K
@@ -465,6 +498,7 @@ SLB_DEV void gp_tile_body(const slb_sweep& cfg, const slb_gp_args& a, unsigned c
                 if (mend[2] > mprev) { mma_run<2>(acc, ap, mprev, mend[2], ks_lane); mprev = mend[2]; }
                 if (mend[3] > mprev) { mma_run<3>(acc, ap, mprev, mend[3], ks_lane); mprev = mend[3]; }
                 if (TIMING) t_mma += clock64() - t_mark;
+                refine_mark(a, RM_MMA + min(jp, 3));
             }
             if (TIMING) t_mark = clock64();
 
@@ -521,6 +555,7 @@ SLB_DEV void gp_tile_body(const slb_sweep& cfg, const slb_gp_args& a, unsigned c
             double* part = a.split_partial + ((size_t)blockIdx.x * SLB_MAX_OUT + f) * (NRED * TP);
             for (int i = tid; i < NRED * TP; i += NT) part[i] = tot[i];
             __syncthreads();
+            refine_mark(a, RM_PARTIAL);
             continue;
         }
         factor_epilogue(f, general, s2);
@@ -534,7 +569,9 @@ SLB_DEV void gp_tile_body(const slb_sweep& cfg, const slb_gp_args& a, unsigned c
         __syncthreads();
         if (tid == 0) s_ticket = atomicAdd(a.split_ticket + tile_index, 1);
         __syncthreads();
+        refine_mark(a, RM_TICKET);
         if (s_ticket != G * FS - 1) {
+            refine_mark(a, RM_EXIT);
             if (TIMING && lane == 0) {             // row-group CTAs that do not finish the tile
                 long long* t = a.timing + ((size_t)blockIdx.x * NW + warp) * 8;
                 long long g_end;
@@ -566,6 +603,7 @@ SLB_DEV void gp_tile_body(const slb_sweep& cfg, const slb_gp_args& a, unsigned c
             factor_epilogue(f, general, f64mul(F.scale, F.scale));
             __syncthreads();
         }
+        refine_mark(a, RM_FACTORS);
     }
 
     if (TIMING && lane == 0) {
@@ -581,7 +619,24 @@ SLB_DEV void gp_tile_body(const slb_sweep& cfg, const slb_gp_args& a, unsigned c
         const bool live = tile0 + p < npts;
         int64_t rel = live ? tile0 + p : 0;
         if (a.index_list != nullptr) rel = a.index_list[rel];
-        if (tid < 2 * TP && live) {
+        if constexpr (CD > 0) {
+            // the closed form: lyapunov_decide's arithmetic by the register-only evaluators
+            if (tid < 2 * TP && live) {
+                double mu[CD], er[CD];
+#pragma unroll
+                for (int o = 0; o < CD; ++o) {
+                    mu[o] = post[o * TP + p];
+                    er[o] = post[(SLB_MAX_OUT + o) * TP + p];
+                }
+                if (tid < TP) {
+                    if (a.mean != nullptr) for (int o = 0; o < CD; ++o) a.mean[rel * CD + o] = mu[o];
+                    if (a.err != nullptr) for (int o = 0; o < CD; ++o) a.err[rel * CD + o] = er[o];
+                    pre[2 * TP + p] = eval_quadratic_reg<CD>(cfg.lyapunov, mu);
+                } else {
+                    pre[3 * TP + p] = lyapunov_error_bound_closed<CD>(cfg, mu, er);
+                }
+            }
+        } else if (tid < 2 * TP && live) {
             double mu[SLB_MAX_OUT], er[SLB_MAX_OUT];
             for (int o = 0; o < D; ++o) {
                 mu[o] = post[o * TP + p];
@@ -614,18 +669,19 @@ SLB_DEV void gp_tile_body(const slb_sweep& cfg, const slb_gp_args& a, unsigned c
         // refine pass of a step that folds its key (filter.cu): the warps of the tile's points (TP is a
         // multiple of 32)
         if (a.fold.rec != nullptr && tid < TP) fold_decided(a.fold, live, neg, rel, a.idx_begin);
+        refine_mark(a, RM_DECIDED);
+        if (split) {
+            refine_mark(a, RM_EXIT);
+            if (TP == 32 && a.marks != nullptr && tid == 0) a.marks[blockIdx.x * SLB_REFINE_MARKS + RM_FINISHER] = 1;
+        }
     }
 }
 
+// The kernel: the tiles of this CTA (refine mode: from the list length and the split), one after the other.
 // KEXPR: at least one factor carries a covariance expression (slb_kernel) instead of the plain
 // RBF; the RBF-only instantiation keeps the lean generation loop.
-// TPV (= TP) only makes the kernel's NAME unique per translation unit: the units for the two tile
-// sizes are compiled from this one source file, nvcc derives the prefix of internal-linkage
-// kernels from the file name, and equally named kernels of different modules were resolved to
-// the same device function (observed: the 64-point launch ran the 32-point code).
-template <int DIN, bool TIMING, bool KEXPR, int TPV>
-__global__ void __launch_bounds__(NT, CTAS_PER_SM)
-gp_tile_kernel(const __grid_constant__ slb_sweep cfg, const slb_gp_args a) {
+template <int DIN, bool TIMING, bool KEXPR, int CD>
+SLB_DEV void gp_tile_run(const slb_sweep& cfg, const slb_gp_args& a) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     int64_t tile_index = blockIdx.x;
     int64_t tile_end = tile_index + 1, tile_step = 1;
@@ -668,26 +724,46 @@ gp_tile_kernel(const __grid_constant__ slb_sweep cfg, const slb_gp_args a) {
             tile_step = gridDim.x;
         }
         if (tile_index * TP >= npts) return;
+        refine_mark(a, RM_ENTRY);
     }
     for (int64_t tile = tile_index; tile < tile_end; tile += tile_step) {
-        gp_tile_body<DIN, TIMING, KEXPR>(cfg, a, smem_raw, tile, npts, grp, G, fsel, FS, tile == tile_index);
+        gp_tile_body<DIN, TIMING, KEXPR, CD>(cfg, a, smem_raw, tile, npts, grp, G, fsel, FS, tile == tile_index);
         if (tile + tile_step < tile_end) __syncthreads();     // shared memory is reused by the next tile
     }
+}
+
+// TPV (= TP) only makes the kernel's NAME unique per translation unit: the units for the two tile
+// sizes are compiled from this one source file, nvcc derives the prefix of internal-linkage
+// kernels from the file name, and equally named kernels of different modules were resolved to
+// the same device function (observed: the 64-point launch ran the 32-point code).
+template <int DIN, bool TIMING, bool KEXPR, int TPV>
+__global__ void __launch_bounds__(NT, CTAS_PER_SM)
+gp_tile_kernel(const __grid_constant__ slb_sweep cfg, const slb_gp_args a) {
+    gp_tile_run<DIN, TIMING, KEXPR, 0>(cfg, a);
+}
+
+// the refine pass of the filter's closed form, CD outputs (gp_tile_body; plain RBF factors)
+template <int DIN, int CD, int TPV>
+__global__ void __launch_bounds__(NT, CTAS_PER_SM)
+gp_tile_closed_kernel(const __grid_constant__ slb_sweep cfg, const slb_gp_args a) {
+    gp_tile_run<DIN, false, false, CD>(cfg, a);
 }
 
 // TPV: see gp_tile_kernel -- nvcc emits templates of this unnamed namespace as WEAK symbols under a
 // prefix derived from the source file name, so the two tile-size units would otherwise share
 // one launch function (the first one linked: every refine pass ran with 64-point tiles).
-template <int DIN, bool TIMING, bool KEXPR, int TPV = TP>
+template <int DIN, bool TIMING, bool KEXPR, int CD = 0, int TPV = TP>
 int launch_gp_tile(cudaStream_t st, const slb_sweep& cfg, const slb_gp_args& a) {
     static_assert(TPV == TP, "TPV only disambiguates the symbol");
     // the opt-in to > 48 KB of dynamic shared memory is a per-device function attribute
     // (atomic flags: sweeps may be issued from several host threads)
     static std::atomic<bool> configured[64];
+    void (*kernel)(slb_sweep, slb_gp_args) = gp_tile_kernel<DIN, TIMING, KEXPR, TP>;
+    if constexpr (CD > 0) kernel = gp_tile_closed_kernel<DIN, CD, TP>;
     int device = 0;
     SLB_CUDA(cudaGetDevice(&device));
     if (device < 0 || device >= 64 || !configured[device].load(std::memory_order_acquire)) {
-        SLB_CUDA(cudaFuncSetAttribute(gp_tile_kernel<DIN, TIMING, KEXPR, TP>,
+        SLB_CUDA(cudaFuncSetAttribute(kernel,
                                       cudaFuncAttributeMaxDynamicSharedMemorySize,
                                       (int)SMEM_TOTAL));
         if (device >= 0 && device < 64) configured[device].store(true, std::memory_order_release);
@@ -695,7 +771,7 @@ int launch_gp_tile(cudaStream_t st, const slb_sweep& cfg, const slb_gp_args& a) 
     int64_t tiles = (a.n + TP - 1) / TP;
     // unsplit refine launches are persistent (see gp_tile_kernel): one CTA per SM
     if (a.count != nullptr && a.split_partial == nullptr && tiles > PREFETCH_CTAS) tiles = PREFETCH_CTAS;
-    gp_tile_kernel<DIN, TIMING, KEXPR, TP><<<(unsigned)tiles, NT, SMEM_TOTAL, st>>>(cfg, a);
+    kernel<<<(unsigned)tiles, NT, SMEM_TOTAL, st>>>(cfg, a);
     SLB_LAUNCH_CHECK();
     return 0;
 }

@@ -1,7 +1,7 @@
 // gp_tile_inst.cu -- one translation unit per GP input dimension and tile size (compiled with
 // -DSLB_TILE_DIN=1..6 -DSLB_TP=64|32, in parallel): the unit's instantiation of slb_gp_tile_launch
 // (gp_args.h) and through it of gp_tile_kernel (gp_tile.cuh) -- plain RBF, covariance expressions,
-// and (d_in = 3, 64 points) the phase-timing build.
+// (d_in = 3) the closed-form refine pass and (d_in = 3, 64 points) the phase-timing build.
 #include "gp_tile.cuh"
 
 #ifndef SLB_TILE_DIN
@@ -18,6 +18,10 @@ int slb_gp_tile_launch(cudaStream_t st, const slb_sweep& cfg, const slb_gp_args&
         slb_set_error("phase timing is compiled for d_in = 3, 64-point tiles only");
         return 1;
     }
+#endif
+#if SLB_TILE_DIN == 3
+    // the refine pass of the filter's closed form (two outputs; gp_tile_body)
+    if (a.closed) return launch_gp_tile<3, false, false, 2>(st, cfg, a);
 #endif
     return kexpr ? launch_gp_tile<DIN, false, true>(st, cfg, a)
                  : launch_gp_tile<DIN, false, false>(st, cfg, a);
